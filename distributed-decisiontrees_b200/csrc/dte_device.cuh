@@ -73,6 +73,13 @@ struct Plan {               // how the next walk will be launched
     }
 };
 
+// Shape of an ensemble in the device layout: what the planner and the walk read from the resident ensemble.
+struct EnsembleShape {
+    Geom g;                           // geometry the ensemble was loaded with (D and F fix the layout)
+    uint32_t T = 0, Tpad = 0, Dtop = 0, top_stride = 1, nb = 1;
+    bool wide = false;
+};
+
 // The ensemble in the device layout, still in host memory (built once, uploaded to one or many devices).
 //   top[t][2^(D-2)]    8-byte heap records {thr bits, fidx | (8 + 8*missing_right) << 16} for levels 0..D-3
 //   bottom[t][2^(D-2)] one record per level-(D-2) node: that node, its two children and their four leaves;
@@ -80,9 +87,7 @@ struct Plan {               // how the next walk will be launched
 // Source layout (SURVEY R1): per tree W = heap array of 2^(D+1)-1 fp32 words padded to w_cls lines, FI = 2^D-1
 // u16 padded to f_cls lines (DTPU.sv:282-338,579-596).
 struct PackedEnsemble {
-    Geom g;
-    uint32_t T = 0, Tpad = 0, Dtop = 0, top_stride = 1, nb = 1;
-    bool wide = false;
+    EnsembleShape shape;
     std::vector<uint2> top;
     std::vector<uint4> bottom;
 };
@@ -145,8 +150,7 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     const bool wide = max_f >= 512;
     const uint32_t BV = wide ? 4 : 2;
 
-    out.g = g;
-    out.T = count; out.Tpad = Tpad; out.Dtop = Dtop; out.top_stride = top_stride; out.nb = nb; out.wide = wide;
+    out.shape = {g, count, Tpad, Dtop, top_stride, nb, wide};
     out.top.assign((size_t)Tpad * top_stride, make_uint2(0u, 8u << 16));
     out.bottom.assign((size_t)Tpad * nb * BV, make_uint4(0, 0, 0, 0));
     std::vector<uint32_t> Wk((2u << Dk) - 1);
@@ -234,9 +238,7 @@ struct Dev {
     bool timing_pending = false;
 
     // ---- resident ensemble ----
-    Geom g;                           // geometry the resident ensemble was loaded with
-    uint32_t T = 0, Tpad = 0, Dtop = 0, top_stride = 1, nb = 1;
-    bool wide = false;
+    EnsembleShape shape;              // of the resident ensemble; a run's K, S and missing are passed to launch_walk
     uint2* d_top = nullptr;
     uint4* d_bottom = nullptr;
     uint64_t ensemble_bytes = 0;
@@ -275,19 +277,19 @@ inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages
 
 inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
     Plan p;
-    p.wide = d.wide;
-    const uint32_t F = d.g.F();
+    p.wide = d.shape.wide;
+    const uint32_t F = d.shape.g.F();
     const size_t budget = (size_t)d.smem_optin;
     // tuple groups (32 tuples, F*128 B of shared memory each) that fit next to the ring
     auto max_groups = [&](int ilp, int pair, int nstages) -> int {
-        const size_t fixed = tile_smem(F, 0, ilp * pair, nstages, d.top_stride);
+        const size_t fixed = tile_smem(F, 0, ilp * pair, nstages, d.shape.top_stride);
         if (fixed >= budget) return 0;
         const int warp_cap = (pair == 4) ? 20 : (ilp == 8 ? 8 : 12);   // thread bound of dt_walk_tile (+1 producer warp)
         int g = (int)std::min<size_t>((size_t)(warp_cap / pair), (budget - fixed) / ((size_t)F * 128));
         if (tune.warps) g = std::min(g, std::max(1, tune.warps / pair));
         return g;
     };
-    const bool can_stage = d.Dtop >= 3;          // below that there is nothing worth staging
+    const bool can_stage = d.shape.Dtop >= 3;          // below that there is nothing worth staging
     // staged candidates {trees per warp, warps per tuple group, ring stages}; the candidate that fits with the most
     // walks in flight wins (dte_autotune times the alternatives on the resident ensemble).
     const int cand[6][3] = {{4, 2, 1}, {2, 4, 1}, {8, 1, 1}, {8, 1, 2}, {4, 1, 2}, {4, 1, 1}};
@@ -305,8 +307,8 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
             if (g >= 1 && score > best) {
                 best = score;
                 staged.variant = KERNEL_TILE_STAGED;
-                staged.ilp = ilp; staged.pair = pair; staged.nstages = st; staged.nwarps = g * pair; staged.wide = d.wide;
-                staged.smem = tile_smem(F, g, ilp * pair, st, d.top_stride);
+                staged.ilp = ilp; staged.pair = pair; staged.nstages = st; staged.nwarps = g * pair; staged.wide = d.shape.wide;
+                staged.smem = tile_smem(F, g, ilp * pair, st, d.shape.top_stride);
             }
             if (tune.ilp && tune.stages && tune.pair) break;
         }
@@ -316,8 +318,8 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
         const int ilp = (tune.ilp == 4) ? 4 : 8;
         const int g = max_groups(ilp, 1, 0);
         if (g >= 1) {
-            tile.variant = KERNEL_TILE; tile.ilp = ilp; tile.pair = 1; tile.nstages = 0; tile.nwarps = g; tile.wide = d.wide;
-            tile.smem = tile_smem(F, g, ilp, 0, d.top_stride);
+            tile.variant = KERNEL_TILE; tile.ilp = ilp; tile.pair = 1; tile.nstages = 0; tile.nwarps = g; tile.wide = d.shape.wide;
+            tile.smem = tile_smem(F, g, ilp, 0, d.shape.top_stride);
         }
     }
     if (want == KERNEL_TILE_STAGED && staged.nwarps >= 1) return staged;
@@ -334,10 +336,10 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
 // barrier hand-offs cost more than they hide.
 inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
     if (pl.variant != KERNEL_TILE_STAGED) return 0xFFFFFFFFu;
-    const bool phased = tune.phased >= 1 || (tune.phased == -1 && d.Dtop >= 10);
+    const bool phased = tune.phased >= 1 || (tune.phased == -1 && d.shape.Dtop >= 10);
     // part A = levels 0..Lw; DTE_TUNE phased=k moves the split k-1 levels further up (smaller part A)
     const uint32_t up = tune.phased > 1 ? (uint32_t)tune.phased - 1 : 0;
-    return (phased && d.Dtop >= 3 + up && pl.nstages <= 4) ? d.Dtop - 3 - up : 0xFFFFFFFFu;
+    return (phased && d.shape.Dtop >= 3 + up && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
 template <int ILP, int P, bool STAGED, bool WIDE, int NT>
@@ -358,9 +360,10 @@ cudaError_t launch_tile(const WalkParams& wp, int grid, int threads, size_t smem
     return launch_tile_nt<ILP, P, STAGED, WIDE, NT_MAX>(wp, grid, threads, smem, st);
 }
 
-// Launch the walk of n tuples on device d (cudaSetDevice already done).  Returns a cudaError_t.
-inline cudaError_t launch_walk(Dev& d, const Tune& tune, int want_variant, const void* d_tuples, size_t n, float* d_scores,
-                               uint8_t* d_labels, cudaStream_t st, bool accumulate, const char** why) {
+// Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
+// `run`; the layout comes from the resident ensemble.  Returns a cudaError_t.
+inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int want_variant, const void* d_tuples, size_t n,
+                               float* d_scores, uint8_t* d_labels, cudaStream_t st, bool accumulate, const char** why) {
     *why = nullptr;
     if (n == 0) return cudaSuccess;
     const Plan pl = make_plan(d, tune, want_variant);
@@ -371,14 +374,14 @@ inline cudaError_t launch_walk(Dev& d, const Tune& tune, int want_variant, const
     wp.scores = d_scores;
     wp.labels = d_labels;
     wp.n = n;
-    wp.F = d.g.F();
-    wp.Dtop = d.Dtop;
-    wp.top_stride = d.top_stride;
-    wp.nb = d.nb;
+    wp.F = d.shape.g.F();
+    wp.Dtop = d.shape.Dtop;
+    wp.top_stride = d.shape.top_stride;
+    wp.nb = d.shape.nb;
     // slots beyond S are never issued (DTPU.sv:519-531); groups past the last tree add exact zeros
-    wp.groups = (uint32_t)std::min<uint64_t>((uint64_t)d.g.S * d.g.K, d.Tpad / 8);
-    wp.K = d.g.K;
-    wp.missing = d.g.missing;
+    wp.groups = (uint32_t)std::min<uint64_t>((uint64_t)run.S * run.K, d.shape.Tpad / 8);
+    wp.K = run.K;
+    wp.missing = run.missing;
     wp.nwarps = (uint32_t)pl.nwarps;
     wp.nstages = (uint32_t)pl.nstages;
     wp.accumulate = accumulate ? 1u : 0u;

@@ -19,6 +19,7 @@
 #include <dlfcn.h>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <thread>
 
 using namespace dte;
@@ -56,6 +57,16 @@ struct NcclApi {
     }
 };
 constexpr int kNcclFloat32 = 7, kNcclSum = 0;        // ncclDataType_t / ncclRedOp_t values of nccl.h
+
+// How a run is partitioned over the ring (SURVEY 8(e)); set by decide_partition only.
+enum class Part {
+    Whole,        // single device, keeps every tuple
+    OwnBatches,   // single device standing for one ring position (dte_set_node): keeps only its dealt batches
+    Dealt,        // multi-device, data-sharded: trees replicated, data batches dealt round-robin over the ring
+    Chunked,      // multi-device, ensemble-sharded: tree chunks in ring order, data broadcast, partials ring-combined
+};
+// dte_info.partition: 0 one device, 1 data-sharded, 2 ensemble-sharded
+uint32_t info_partition(Part p) { return p == Part::Dealt ? 1u : p == Part::Chunked ? 2u : 0u; }
 }  // namespace
 
 struct dte_engine {
@@ -83,12 +94,14 @@ struct dte_engine {
     std::vector<std::vector<unsigned char>> tree_w, tree_f;   // tree lines kept per ring position (weights | indexes)
 
     // ---- partition of the current run (decided at `start` / load) ----
+    // A multi-device handle starts as Dealt, which dte_get_info reports before any run.  dealing() divides by
+    // deal_lines / tuple_cls; it runs only for a partition decide_partition accepted (result reads once ring_cap != 0,
+    // the data receiver in ST_DATA, prepare_data_phase after a decision), and that decision has set deal_lines.
+    Part part = Part::Whole;
     uint32_t ndev_ring = 1;           // numDevs (reg 203[39:32])
-    int prog_partition = -1;          // how the RESIDENT ensemble was placed: 0 one device, 1 replicated, 2 chunks in ring order
+    uint64_t deal_lines = 0;          // Dealt / OwnBatches: data lines per dealt batch
+    std::optional<Part> placed;       // how the RESIDENT ensemble was placed (none until a placement completes)
     int prog_pos2dev[kMaxRing];       // ... and on which devices (a run must use the same placement)
-    bool group = false;               // ensemble-sharded lock-step group: data broadcast, partial scores ring-combined
-    bool deal = false;                // data lines dealt round-robin in batches of deal_lines
-    uint64_t deal_lines = 0;
 
     // ---- data / result accounting since `start` ----
     uint64_t data_lines_in = 0;       // data lines received
@@ -166,63 +179,13 @@ int decode_geom(dte_engine* e, Geom& g) {
     return DTE_OK;
 }
 
-// A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
-// layout and the validated feature-index range; K, S and the missing pattern are free to change).
-int check_resident(dte_engine* e, const Geom& g) {
-    if (e->multi() && e->prog_partition >= 0) {
-        const int now = e->group ? 2 : 1;
-        if (now != e->prog_partition)
-            return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
-                        now == 2 ? "ensemble-sharded" : "data-sharded", e->prog_partition == 2 ? "in per-device chunks" : "replicated");
-        if (now == 2 && memcmp(e->pos2dev, e->prog_pos2dev, sizeof(int) * e->devs.size()))
-            return fail(e, DTE_ERR_CONFIG, "devices_list (registers 208-210) changed since the tree chunks were programmed: the ring order of the partial sums would change");
-    }
-    for (Dev& d : e->devs) {
-        if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
-        if (d.g.tuple_cls != g.tuple_cls || d.g.D != g.D)
-            return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
-                        g.F(), g.D, d.g.F(), d.g.D);
-    }
-    return DTE_OK;
-}
-
-void free_ensemble(Dev& d) {
-    cudaSetDevice(d.ordinal);
-    if (d.d_top) cudaFree(d.d_top);
-    if (d.d_bottom) cudaFree(d.d_bottom);
-    d.d_top = nullptr;
-    d.d_bottom = nullptr;
-    d.T = d.Tpad = 0;
-    d.ensemble_bytes = 0;
-}
-
-int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk) {
-    CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
-    free_ensemble(d);
-    CUDA_TRY(e, cudaMalloc(&d.d_top, pk.top.size() * sizeof(uint2)));
-    CUDA_TRY(e, cudaMalloc(&d.d_bottom, pk.bottom.size() * sizeof(uint4)));
-    CUDA_TRY(e, cudaMemcpy(d.d_top, pk.top.data(), pk.top.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    CUDA_TRY(e, cudaMemcpy(d.d_bottom, pk.bottom.data(), pk.bottom.size() * sizeof(uint4), cudaMemcpyHostToDevice));
-    d.g = pk.g;
-    d.T = pk.T; d.Tpad = pk.Tpad; d.Dtop = pk.Dtop; d.top_stride = pk.top_stride; d.nb = pk.nb; d.wide = pk.wide;
-    d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.bottom.size() * sizeof(uint4);
-    return DTE_OK;
-}
-
-int pack_or_fail(dte_engine* e, const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl,
-                 uint32_t first, uint32_t count, PackedEnsemble& pk) {
-    std::string msg;
-    const int rc = pack_ensemble(g, wl, n_wl, fl, n_fl, first, count, pk, msg);
-    if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
-    return DTE_OK;
-}
-
 // ---- partition of a run: registers 201 / 203 / 208-210 ---------------------------------------------
 struct Flags {
     bool data_distributed, host_node, bcast_data, bcast_trees, aggreg, multiple, rx_enabled;
     uint64_t batch_cls, chunk_w, chunk_f;
     uint32_t ndev;
+    // the tree stream is cut into per-position chunks (PCIeReceiver.sv:241-264) unless broadcast_trees
+    bool cut_trees() const { return multiple && !bcast_trees && ndev > 1; }
 };
 Flags decode_flags(const dte_engine* e) {
     const uint64_t r201 = e->regs[1], r203 = e->regs[3];
@@ -246,12 +209,18 @@ int owner_of(const dte_engine* e, uint32_t pos) {
     return pos == e->node_index ? 0 : -1;
 }
 
+// The device whose results this handle exposes and whose counters the status registers report (see decide_partition).
+Dev& host_dev(dte_engine* e) { return e->devs[(size_t)e->pos2dev[0]]; }
+const Dev& host_dev(const dte_engine* e) { return e->devs[(size_t)e->pos2dev[0]]; }
+
 // Decide how the run is partitioned.  Single-device handles keep the raw RTL filter semantics (one process per
 // GPU replaying the same stream, dte_set_node); a multi-device handle supports exactly the two partitions of
 // SURVEY 8(e) and refuses the rest.
+// host_dev, the device of ring position 0 (the host node), is right in every partition: a single-device handle never
+// permutes pos2dev, so it is devs[0]; Dealt deals from the host node first and Chunked combines the partials there.
 int decide_partition(dte_engine* e, const Geom& g) {
     const Flags f = decode_flags(e);
-    bool group = false, deal = false;
+    Part part = Part::Whole;
     int pos2dev[kMaxRing];
     const size_t G = e->devs.size();
     for (uint32_t i = 0; i < (uint32_t)kMaxRing; ++i) pos2dev[i] = (int)i;
@@ -270,9 +239,9 @@ int decide_partition(dte_engine* e, const Geom& g) {
             }
         }
         if (f.bcast_trees && !f.bcast_data && !f.aggreg) {
-            deal = true;
+            part = Part::Dealt;
         } else if (!f.bcast_trees && f.bcast_data && f.aggreg) {
-            group = true;
+            part = Part::Chunked;
             for (size_t a = 0; a < G; ++a)
                 for (size_t b = 0; b < G; ++b) {
                     int ok = 1;
@@ -285,17 +254,102 @@ int decide_partition(dte_engine* e, const Geom& g) {
                         "broadcast_data + aggreg_enabled (tree chunks, ring combine)", (unsigned long long)(e->regs[1] & 0xFF));
         }
     } else if (split && !f.bcast_data && !f.data_distributed) {
-        deal = true;                                 // this process keeps the batches of its own ring position
+        part = Part::OwnBatches;                     // this process keeps the batches of its own ring position
     }
-    if (deal && (f.batch_cls == 0 || f.batch_cls % g.tuple_cls))
+    const bool deals = part == Part::Dealt || part == Part::OwnBatches;
+    if (deals && (f.batch_cls == 0 || f.batch_cls % g.tuple_cls))
         return fail(e, DTE_ERR_CONFIG, "reg 201: core_data_batch_cls=%llu must be a positive multiple of tuple_numcls=%u",
                     (unsigned long long)f.batch_cls, g.tuple_cls);
     e->ndev_ring = f.ndev;
-    e->group = group;
-    e->deal = deal;
-    e->deal_lines = deal ? f.batch_cls : 0;
+    e->part = part;
+    e->deal_lines = deals ? f.batch_cls : 0;
     memcpy(e->pos2dev, pos2dev, sizeof pos2dev);
     return DTE_OK;
+}
+
+// A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
+// layout and the validated feature-index range; K, S and the missing pattern are free to change).
+int check_resident(dte_engine* e, const Geom& g) {
+    if (e->multi() && e->placed) {
+        if (e->part != *e->placed)
+            return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
+                        e->part == Part::Chunked ? "ensemble-sharded" : "data-sharded", *e->placed == Part::Chunked ? "in per-device chunks" : "replicated");
+        if (e->part == Part::Chunked && memcmp(e->pos2dev, e->prog_pos2dev, sizeof(int) * e->devs.size()))
+            return fail(e, DTE_ERR_CONFIG, "devices_list (registers 208-210) changed since the tree chunks were programmed: the ring order of the partial sums would change");
+    }
+    for (Dev& d : e->devs) {
+        if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
+        if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
+            return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
+                        g.F(), g.D, d.shape.g.F(), d.shape.g.D);
+    }
+    return DTE_OK;
+}
+
+// ---- placement of the ensemble on the devices ---------------------------------------------------------
+void free_ensemble(Dev& d) {
+    cudaSetDevice(d.ordinal);
+    if (d.d_top) cudaFree(d.d_top);
+    if (d.d_bottom) cudaFree(d.d_bottom);
+    d.d_top = nullptr;
+    d.d_bottom = nullptr;
+    d.shape.T = d.shape.Tpad = 0;    // the geometry stays: the landing slots of a run in progress are cut by it
+    d.ensemble_bytes = 0;
+}
+
+int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk) {
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
+    free_ensemble(d);
+    CUDA_TRY(e, cudaMalloc(&d.d_top, pk.top.size() * sizeof(uint2)));
+    CUDA_TRY(e, cudaMalloc(&d.d_bottom, pk.bottom.size() * sizeof(uint4)));
+    CUDA_TRY(e, cudaMemcpy(d.d_top, pk.top.data(), pk.top.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    CUDA_TRY(e, cudaMemcpy(d.d_bottom, pk.bottom.data(), pk.bottom.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+    d.shape = pk.shape;
+    d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.bottom.size() * sizeof(uint4);
+    return DTE_OK;
+}
+
+// The trees one ring position receives: trees [first, first + count) of the given line streams (0, 0 = all of them).
+struct TreeShare {
+    const unsigned char *wl, *fl;     // weights / feature-index lines
+    size_t n_wl, n_fl;
+    uint32_t first, count;
+};
+
+// Place the ensemble for the run's partition: Chunked puts share[r] on the device of ring position r; every other
+// partition packs share[0] once and replicates it.  Records the placement for check_resident.
+int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share) {
+    const bool chunked = e->part == Part::Chunked;
+    PackedEnsemble pk;
+    for (size_t r = 0; r < e->devs.size(); ++r) {
+        if (chunked || r == 0) {
+            const TreeShare& s = share[r];
+            std::string msg;
+            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, pk, msg);
+            if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
+        }
+        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk));
+    }
+    e->placed = e->part;
+    memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
+    return DTE_OK;
+}
+
+// Program the devices from the tree lines the receiver kept: all of them in entry 0 unless the stream was cut, then
+// entry r for ring position r (a single-device handle: the entry of its own node).
+int program_devices(dte_engine* e, const Geom& g) {
+    const bool cut = decode_flags(e).cut_trees();
+    TreeShare share[kMaxRing];
+    const size_t n = e->part == Part::Chunked ? e->devs.size() : 1;
+    for (size_t r = 0; r < n; ++r) {
+        const size_t src = !cut ? 0 : e->multi() ? r : e->node_index;
+        const size_t lw = e->tree_w[src].size() / 16, lf = e->tree_f[src].size() / 16;
+        if (!lw || !lf) return e->multi() ? fail(e, DTE_ERR_CONFIG, "ring position %zu received no trees", r)
+                                          : fail(e, DTE_ERR_CONFIG, "node %u received no trees", e->node_index);
+        share[r] = {e->tree_w[src].data(), e->tree_f[src].data(), lw, lf, 0, 0};
+    }
+    return place_ensemble(e, g, share);
 }
 
 // ---- landing slots ------------------------------------------------------------------------------
@@ -400,10 +454,19 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
     return DTE_OK;
 }
 
+// Launch the walk of n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.
+int walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, float* scores, uint8_t* labels, cudaStream_t st,
+                 bool accumulate) {
+    const char* why = nullptr;
+    const cudaError_t rc = launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, scores, labels, st, accumulate, &why);
+    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
+    return DTE_OK;
+}
+
 // Walk the whole tuples that have landed in slot b of device d since the last submit and queue their results.
 int submit_dev(dte_engine* e, Dev& d, int b) {
     Slot& s = d.slot[b];
-    const size_t tb = d.g.tuple_bytes();
+    const size_t tb = d.shape.g.tuple_bytes();
     if (!d.cap_tuples || !tb) return DTE_OK;
     const size_t whole = s.fill / tb, cnt = whole - s.walked;
     if (!cnt) return DTE_OK;
@@ -412,10 +475,7 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // score buffer of this slot drained
     const bool labels = d.sink_sc && d.sink_lb;
-    const char* why = nullptr;
-    cudaError_t rc = launch_walk(d, e->tune, e->forced_variant, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked,
-                                 labels ? s.d_lb + s.walked : nullptr, d.s_main, false, &why);
-    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
+    TRY(walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked, labels ? s.d_lb + s.walked : nullptr, d.s_main, false));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
     TRY(enqueue_results(e, d, s, s.walked, cnt, labels));
     s.walked = whole;
@@ -481,7 +541,7 @@ void advance_slot(Dev& d) {
 // Land `bytes` of the tuple stream on device d (pinned memory is DMA'd in place, pageable memory goes through the
 // engine's staging ring, h2d_piece).  Full slots are submitted as they fill.
 int land_dev(dte_engine* e, Dev& d, const unsigned char* src, size_t bytes) {
-    const size_t cap_bytes = d.cap_tuples * d.g.tuple_bytes();
+    const size_t cap_bytes = d.cap_tuples * d.shape.g.tuple_bytes();
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     const bool pageable = bytes >= (256u << 10) && is_pageable(src);
     while (bytes) {
@@ -501,9 +561,6 @@ int land_dev(dte_engine* e, Dev& d, const unsigned char* src, size_t bytes) {
 }
 
 // ---- ensemble-sharded group: every device sees every tuple, partial scores are ring-combined ---------
-Dev& host_dev(dte_engine* e) { return e->devs[(size_t)e->pos2dev[0]]; }
-const Dev& host_dev(const dte_engine* e) { return e->devs[(size_t)e->pos2dev[0]]; }
-
 // one launch of the ring-order combine; vector path only when every pointer is line-aligned
 cudaError_t launch_ring_combine(const RingParts& parts, int G, float* out, uint8_t* labels, size_t n, int sm_count, cudaStream_t st) {
     bool vec = (reinterpret_cast<uintptr_t>(out) & 15u) == 0 && (!labels || (reinterpret_cast<uintptr_t>(labels) & 3u) == 0);
@@ -529,10 +586,37 @@ int nccl_setup(dte_engine* e) {
     return DTE_OK;
 }
 
+// DTE_OPT_COMBINE = 1: one ncclReduce of the partials of slot b into the host device's scores, then its labels.
+int nccl_combine(dte_engine* e, int b, size_t walked, size_t cnt, bool labels) {
+    const size_t G = e->devs.size();
+    Dev& h = host_dev(e);
+    Slot& hs = h.slot[b];
+    TRY(nccl_setup(e));
+    int rc = e->nccl.GroupStart();
+    for (size_t r = 0; r < G && !rc; ++r) {
+        Dev& d = e->devs[(size_t)e->pos2dev[r]];
+        rc = e->nccl.Reduce(d.slot[b].d_part + walked, hs.d_sc + walked, cnt, kNcclFloat32, kNcclSum, 0, e->nccl_comms[r], d.s_main);
+    }
+    const int rc2 = e->nccl.GroupEnd();
+    if (rc || rc2) return fail(e, DTE_ERR_CUDA, "ncclReduce failed: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(rc ? rc : rc2) : "?");
+    CUDA_TRY(e, cudaSetDevice(h.ordinal));
+    if (labels) {
+        labels_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, h.s_main>>>(hs.d_sc + walked, hs.d_lb + walked, cnt);
+        CUDA_TRY(e, cudaGetLastError());
+    }
+    for (Dev& d : e->devs) {                     // the reduce read d_part on every device's stream
+        CUDA_TRY(e, cudaSetDevice(d.ordinal));
+        CUDA_TRY(e, cudaEventRecord(d.slot[b].ev_walk, d.s_main));
+    }
+    CUDA_TRY(e, cudaSetDevice(h.ordinal));
+    for (Dev& d : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, d.slot[b].ev_walk, 0));
+    return DTE_OK;
+}
+
 int submit_group(dte_engine* e, int b) {
     const size_t G = e->devs.size();
     Dev& h = host_dev(e);
-    const size_t tb = h.g.tuple_bytes();
+    const size_t tb = h.shape.g.tuple_bytes();
     if (!h.cap_tuples || !tb) return DTE_OK;
     const size_t whole = h.slot[b].fill / tb, walked = h.slot[b].walked, cnt = whole - walked;
     if (!cnt) return DTE_OK;
@@ -545,9 +629,7 @@ int submit_group(dte_engine* e, int b) {
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));   // every piece has landed here
         CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, h.slot[b].ev_comb, 0));    // the previous combine is done with our partials
-        const char* why = nullptr;
-        cudaError_t rc = launch_walk(d, e->tune, e->forced_variant, s.d_tup + walked * tb, cnt, s.d_part + walked, nullptr, d.s_main, false, &why);
-        if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
+        TRY(walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_part + walked, nullptr, d.s_main, false));
         CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
         s.walked = whole;
     }
@@ -562,25 +644,7 @@ int submit_group(dte_engine* e, int b) {
         CUDA_TRY(e, launch_ring_combine(parts, (int)G, hs.d_sc + walked, labels ? hs.d_lb + walked : nullptr, cnt, h.sm_count, h.s_main));
         h.kernel_launches++;
     } else {
-        TRY(nccl_setup(e));
-        int rc = e->nccl.GroupStart();
-        for (size_t r = 0; r < G && !rc; ++r) {
-            Dev& d = e->devs[(size_t)e->pos2dev[r]];
-            rc = e->nccl.Reduce(d.slot[b].d_part + walked, hs.d_sc + walked, cnt, kNcclFloat32, kNcclSum, 0, e->nccl_comms[r], d.s_main);
-        }
-        const int rc2 = e->nccl.GroupEnd();
-        if (rc || rc2) return fail(e, DTE_ERR_CUDA, "ncclReduce failed: %s", e->nccl.GetErrorString ? e->nccl.GetErrorString(rc ? rc : rc2) : "?");
-        CUDA_TRY(e, cudaSetDevice(h.ordinal));
-        if (labels) {
-            labels_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, h.s_main>>>(hs.d_sc + walked, hs.d_lb + walked, cnt);
-            CUDA_TRY(e, cudaGetLastError());
-        }
-        for (Dev& d : e->devs) {                     // the reduce read d_part on every device's stream
-            CUDA_TRY(e, cudaSetDevice(d.ordinal));
-            CUDA_TRY(e, cudaEventRecord(d.slot[b].ev_walk, d.s_main));
-        }
-        CUDA_TRY(e, cudaSetDevice(h.ordinal));
-        for (Dev& d : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, d.slot[b].ev_walk, 0));
+        TRY(nccl_combine(e, b, walked, cnt, labels));
     }
     CUDA_TRY(e, cudaEventRecord(hs.ev_comb, h.s_main));
     CUDA_TRY(e, cudaEventRecord(hs.ev_walk, h.s_main));           // results of this slot are final after the combine
@@ -594,7 +658,7 @@ int submit_group(dte_engine* e, int b) {
 int land_group(dte_engine* e, const unsigned char* src, size_t bytes) {
     const size_t G = e->devs.size();
     Dev& h = host_dev(e);
-    const size_t cap_bytes = h.cap_tuples * h.g.tuple_bytes();
+    const size_t cap_bytes = h.cap_tuples * h.shape.g.tuple_bytes();
     static const size_t kMinPiece = 256u << 10;
     uint32_t rot = 0;
     const bool pageable = bytes >= kMinPiece && is_pageable(src);
@@ -639,7 +703,7 @@ int land_group(dte_engine* e, const unsigned char* src, size_t bytes) {
 
 // ---- run-level helpers ----------------------------------------------------------------------------
 int flush_all(dte_engine* e) {
-    if (e->group) return submit_group(e, host_dev(e).cur);
+    if (e->part == Part::Chunked) return submit_group(e, host_dev(e).cur);
     for (Dev& d : e->devs) TRY(submit_dev(e, d, d.cur));
     return DTE_OK;
 }
@@ -667,7 +731,7 @@ int drain_all(dte_engine* e) {
 
 bool fragment_pending(const dte_engine* e) {
     for (const Dev& d : e->devs)
-        if (d.cap_tuples && d.g.tuple_cls && d.slot[d.cur].fill % d.g.tuple_bytes()) return true;
+        if (d.cap_tuples && d.shape.g.tuple_cls && d.slot[d.cur].fill % d.shape.g.tuple_bytes()) return true;
     return false;
 }
 
@@ -680,37 +744,34 @@ void reset_pipeline(Dev& d) {
     d.tuples_landed = 0;
 }
 
-// Results exposed by this handle, in order: tuple i lives on device dev at local index loc (dte_partition.hpp).
-void locate_result(const dte_engine* e, uint64_t i, int& dev, uint64_t& loc) {
-    if (e->multi() && e->deal) {
-        const Deal deal{e->deal_lines / e->g.tuple_cls, e->devs.size()};
+// the dealt order of a Dealt run: batches of deal_lines / tuple_cls tuples over the handle's ring positions
+Deal dealing(const dte_engine* e) { return Deal{e->deal_lines / e->g.tuple_cls, e->devs.size()}; }
+
+// Results exposed by this handle, in order: tuple i lives on the returned device at local index loc (dte_partition.hpp).
+const Dev& locate_result(const dte_engine* e, uint64_t i, uint64_t& loc) {
+    if (e->part == Part::Dealt) {
         uint64_t pos;
-        deal.locate(i, pos, loc);
-        dev = e->pos2dev[pos];
-    } else {
-        dev = e->group ? e->pos2dev[0] : 0;
-        loc = i;
+        dealing(e).locate(i, pos, loc);
+        return e->devs[(size_t)e->pos2dev[pos]];
     }
+    loc = i;
+    return host_dev(e);
 }
 // how many leading results (in exposed order) the per-device local counts stand for
 uint64_t global_prefix(const dte_engine* e, bool completed) {
     auto cnt = [&](const Dev& d) { return completed ? d.res_done : d.res_enq; };
-    if (e->multi() && e->deal) {
-        const Deal deal{e->deal_lines / e->g.tuple_cls, e->devs.size()};
+    if (e->part == Part::Dealt) {
         uint64_t c[kMaxRing];
         for (size_t r = 0; r < e->devs.size(); ++r) c[r] = cnt(e->devs[(size_t)e->pos2dev[r]]);
-        return deal.prefix(c);
+        return dealing(e).prefix(c);
     }
-    return cnt(e->devs[(size_t)(e->group ? e->pos2dev[0] : 0)]);
+    return cnt(host_dev(e));
 }
 
 int prepare_data_phase(dte_engine* e, bool need_ring) {
     const uint32_t F = e->g.F();
     const size_t cap = default_chunk(e, F);
-    for (Dev& d : e->devs) {
-        TRY(ensure_slots(e, d, cap, F, e->group));
-        d.g.K = e->g.K; d.g.S = e->g.S; d.g.missing = e->g.missing;     // summation geometry of THIS run
-    }
+    for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked));
     if (need_ring) {
         // result queue: reg 207 says how many result lines the run produces; bounded either way
         uint64_t lines = e->opt_queue_lines ? e->opt_queue_lines : (e->regs[7] & 0xFFFFFFFFull) + 64;
@@ -718,11 +779,10 @@ int prepare_data_phase(dte_engine* e, bool need_ring) {
         lines = std::min<uint64_t>(std::max<uint64_t>(lines, 16), 1u << 26);
         e->ring_cap = lines * 4;
         const uint64_t G = e->devs.size();
-        const uint64_t bt = e->deal ? e->deal_lines / e->g.tuple_cls : 0;
         for (Dev& d : e->devs) {
-            const bool has_results = !e->group || &d == &host_dev(e);
+            const bool has_results = e->part != Part::Chunked || &d == &host_dev(e);
             if (!has_results) continue;
-            const uint64_t per = (e->multi() && e->deal) ? e->ring_cap / G + 2 * bt + cap : e->ring_cap + cap;
+            const uint64_t per = e->part == Part::Dealt ? e->ring_cap / G + 2 * dealing(e).bt + cap : e->ring_cap + cap;
             TRY(ensure_ring(e, d, per));
         }
     }
@@ -754,7 +814,7 @@ int infer_host(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_
         CUDA_TRY(e, cudaEventRecord(d.ev_t0, d.s_main));
     }
     int rc = DTE_OK;
-    if (e->group) {
+    if (e->part == Part::Chunked) {
         Dev& h = host_dev(e);
         h.sink_sc = h_scores;
         h.sink_lb = h_labels;
@@ -863,42 +923,20 @@ void destroy_dev(Dev& d) {
     if (d.s_d2h) cudaStreamDestroy(d.s_d2h);
 }
 
-// Program the devices from the tree lines gathered per ring position.
-//   replicated: every device gets all trees;  chunked: ring position r gets the lines kept for it.
-int program_devices(dte_engine* e, const Geom& g) {
-    const Flags f = decode_flags(e);
-    const bool replicate = f.bcast_trees || f.ndev <= 1 || !f.multiple;
-    PackedEnsemble pk;
-    if (e->multi()) {
-        for (size_t r = 0; r < e->devs.size(); ++r) {
-            const size_t src = replicate ? 0 : r;
-            if (!replicate || r == 0) {
-                const size_t lw = e->tree_w[src].size() / 16, lf = e->tree_f[src].size() / 16;
-                if (!lw || !lf) return fail(e, DTE_ERR_CONFIG, "ring position %zu received no trees", r);
-                TRY(pack_or_fail(e, g, e->tree_w[src].data(), lw, e->tree_f[src].data(), lf, 0, 0, pk));
-            }
-            TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk));
-        }
-    } else {
-        const size_t src = replicate ? 0 : e->node_index;
-        const size_t lw = e->tree_w[src].size() / 16, lf = e->tree_f[src].size() / 16;
-        if (!lw || !lf) return fail(e, DTE_ERR_CONFIG, "node %u received no trees", e->node_index);
-        TRY(pack_or_fail(e, g, e->tree_w[src].data(), lw, e->tree_f[src].data(), lf, 0, 0, pk));
-        TRY(upload_ensemble(e, e->devs[0], pk));
-    }
-    e->prog_partition = !e->multi() ? 0 : (replicate ? 1 : 2);
-    memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
-    return DTE_OK;
-}
-
 uint64_t cycles_of(const dte_engine* e, double ns) {
     return e->cycle_mhz ? (uint64_t)(ns * 1e-3 * e->cycle_mhz) : (uint64_t)ns;
 }
 
 // tuples served by cluster 0: tuple i uses clusters (i*K)%8 .. +K-1 (Core.sv:305-316)
 uint64_t cluster0_tuples(const dte_engine* e) {
-    const Dev& h = e->devs[(size_t)(e->multi() ? e->pos2dev[0] : 0)];
-    return (h.tuples_landed * std::max(1u, e->g.K) + 7) / 8;
+    return (host_dev(e).tuples_landed * std::max(1u, e->g.K) + 7) / 8;
+}
+
+// fold the run's cluster-0 count into the cumulative counters, which survive `start` (DTPUCluster.sv:85-97)
+void roll_cluster_counters(dte_engine* e) {
+    const uint64_t c0 = cluster0_tuples(e);
+    e->cum_c0 += c0;
+    e->cum_c0_lines += c0 * e->g.tuple_cls;
 }
 
 // process_done = total_pcie_out_cls_count == total_results_numcls (DTInference.sv:649-656); "produced" counts the
@@ -917,11 +955,120 @@ int check_done(dte_engine* e, bool* done) {
         e->t_done = Clock::now();
         e->running = false;
         e->state = dte_engine::ST_IDLE;                                         // PCIeReceiver.sv:289-292
-        const uint64_t c0 = cluster0_tuples(e);
-        e->cum_c0 += c0;
-        e->cum_c0_lines += c0 * e->g.tuple_cls;
+        roll_cluster_counters(e);
         for (Dev& d : e->devs) d.tuples_landed = 0;
     }
+    return DTE_OK;
+}
+
+// Tree lines (RECEIVE_TREES): keep the lines of this handle's ring positions and advance p / n_lines past the lines
+// consumed.  The last tree line programs the devices and opens the data phase.
+int receive_tree_lines(dte_engine* e, const unsigned char*& p, size_t& n_lines) {
+    const uint64_t total = e->regs[2] & 0xFFFFFFFFull, wtotal = e->regs[2] >> 32;   // reg 202
+    if (total == 0 || wtotal == 0 || wtotal >= total)
+        return fail(e, DTE_ERR_CONFIG, "reg 202: total_num_trees_cls=%llu total_num_weights_cls=%llu",
+                    (unsigned long long)total, (unsigned long long)wtotal);
+    if (!e->prog_seen) { e->prog_seen = e->prog_open = true; e->t_prog0 = Clock::now(); }
+    // Chunking (PCIeReceiver.sv:241-264): unless broadcast_trees, the weights stream is cut every
+    // numcls_local_weights lines and the index stream every numcls_local_findexes lines, chunk i going to
+    // devices_list[i % numDevs]; entry 0 is the host node itself (:160-178).  currDevID keeps rotating
+    // from the weights into the index stream, as in the RTL.
+    Flags f = decode_flags(e);
+    const bool cut = f.cut_trees();
+    if (cut && (e->regs[3] & 0xFFFFFFFFull) == 0 && wtotal % e->g.w_cls == 0) {
+        // extension: both 16-bit chunk fields left at 0 = "cut the trees evenly over numDevs" — chunks of more
+        // than 65535 lines (e.g. 1024 trees of depth 10 per device) cannot be written into reg 203
+        const uint64_t per = (wtotal / e->g.w_cls + f.ndev - 1) / f.ndev;
+        f.chunk_w = per * e->g.w_cls;
+        f.chunk_f = per * e->g.f_cls;
+    }
+    if (cut && (f.chunk_f == 0 || (!e->multi() && e->node_index >= f.ndev)))
+        return fail(e, DTE_ERR_CONFIG, "reg 203: numcls_local_findexes=%llu numDevs=%u node=%u",
+                    (unsigned long long)f.chunk_f, f.ndev, e->node_index);
+    const size_t take = (size_t)std::min<uint64_t>(n_lines, total - e->lines_received);
+    if (!cut) {
+        const uint64_t w_take = std::min<uint64_t>(take, wtotal > e->lines_received ? wtotal - e->lines_received : 0);
+        e->tree_w[0].insert(e->tree_w[0].end(), p, p + w_take * 16);
+        e->tree_f[0].insert(e->tree_f[0].end(), p + w_take * 16, p + take * 16);
+        e->prog_lines_local += take;
+        if (e->multi()) e->sl3_lines_sent += take;                       // broadcast to the ring as well
+    } else {
+        for (size_t i = 0; i < take; ++i) {
+            const bool is_w = e->lines_received + i < wtotal;
+            if (owner_of(e, e->cur_dev) >= 0) {
+                auto& v = is_w ? e->tree_w[e->cur_dev] : e->tree_f[e->cur_dev];
+                v.insert(v.end(), p + i * 16, p + i * 16 + 16);
+            }
+            if (e->cur_dev == (e->multi() ? 0u : e->node_index)) e->prog_lines_local++;
+            if (e->cur_dev != 0) e->sl3_lines_sent++;
+            uint64_t& cnt = is_w ? e->cur_w : e->cur_f;
+            if (++cnt == (is_w ? f.chunk_w : f.chunk_f)) {
+                cnt = 0;
+                e->cur_dev = (e->cur_dev + 1 == f.ndev) ? 0 : e->cur_dev + 1;
+            }
+        }
+    }
+    e->lines_received += take;
+    p += take * 16;
+    n_lines -= take;
+    if (e->lines_received == total) {
+        // prog_mode = (numcls_received < total_num_weights_cls), PCIeReceiver.sv:136-139
+        int rc = program_devices(e, e->g);
+        for (auto& v : e->tree_w) { v.clear(); v.shrink_to_fit(); }
+        for (auto& v : e->tree_f) { v.clear(); v.shrink_to_fit(); }
+        if (!rc) rc = prepare_data_phase(e, true);
+        e->t_prog1 = Clock::now();
+        e->prog_open = false;
+        if (rc) { e->state = dte_engine::ST_IDLE; e->running = false; return rc; }
+        e->state = dte_engine::ST_DATA;                                 // WAIT_DATA -> RECEIVE_DATA
+        e->cur_dev = 0;
+        e->cur_d = 0;
+    }
+    return DTE_OK;
+}
+
+// Data lines (RECEIVE_DATA): all n_lines land on the devices the run's partition sends them to.
+int receive_data_lines(dte_engine* e, const unsigned char* p, size_t n_lines) {
+    // back-pressure: the result queue is bounded (pcie_full_out, PCIeReceiver.sv:126)
+    const size_t tcl = e->g.tuple_cls;
+    uint64_t in_engine = (e->data_lines_in + n_lines) / tcl;                         // results queued once these lines are in
+    if (e->part == Part::OwnBatches) in_engine = in_engine / e->ndev_ring + e->deal_lines / tcl;   // this node keeps 1/numDevs of them
+    in_engine = in_engine > e->res_read ? in_engine - e->res_read : 0;
+    if (in_engine > e->ring_cap)
+        return fail(e, DTE_ERR_BACKPRESSURE, "result queue full (%llu results would wait, capacity %llu): read result lines first",
+                    (unsigned long long)in_engine, (unsigned long long)e->ring_cap);
+    const size_t tb = e->g.tuple_bytes();
+    const uint64_t lines_before = e->data_lines_in;
+    if (e->part == Part::Chunked) {
+        // data broadcast (InputDistributor.sv:199-204): every device receives every line
+        TRY(land_group(e, p, n_lines * 16));
+        for (Dev& d : e->devs) d.tuples_landed = (e->data_lines_in + n_lines) * 16 / tb;
+        e->sl3_lines_sent += n_lines;
+    } else if (e->part == Part::Whole) {
+        Dev& h = host_dev(e);
+        TRY(land_dev(e, h, p, n_lines * 16));
+        h.tuples_landed = (e->data_lines_in + n_lines) * 16 / tb;
+    } else {
+        // data dealing (PCIeReceiver.sv:298-307): batches of core_data_batch_cls lines round-robin over the ring
+        size_t left = n_lines;
+        while (left) {
+            const size_t run = (size_t)std::min<uint64_t>(left, e->deal_lines - e->cur_d);
+            const int dv = owner_of(e, e->cur_dev);
+            if (dv >= 0) {
+                Dev& d = e->devs[(size_t)dv];
+                TRY(land_dev(e, d, p, run * 16));
+                d.tuples_landed = d.slot[d.cur].fill / tb - d.slot[d.cur].walked + d.res_enq;   // whole tuples so far on this device
+            }
+            if (e->cur_dev != 0) e->sl3_lines_sent += run;
+            e->cur_d += run;
+            if (e->cur_d == e->deal_lines) { e->cur_d = 0; e->cur_dev = (e->cur_dev + 1 == e->ndev_ring) ? 0 : e->cur_dev + 1; }
+            p += run * 16;
+            left -= run;
+        }
+    }
+    e->data_lines_in += n_lines;
+    e->lines_received += n_lines;
+    e->tuples_in += (e->data_lines_in / tcl) - (lines_before / tcl);
     return DTE_OK;
 }
 
@@ -948,6 +1095,7 @@ int dte_create_multi(dte_t** engine, const int* gpu_ordinals, int n_gpus) {
     if (!e) return DTE_ERR_NOMEM;
     parse_tune(e->tune);
     e->devs.resize((size_t)n_gpus);
+    e->part = n_gpus > 1 ? Part::Dealt : Part::Whole;
     for (uint32_t i = 0; i < (uint32_t)kMaxRing; ++i) e->pos2dev[i] = (int)i;
     e->tree_w.resize(kMaxRing);
     e->tree_f.resize(kMaxRing);
@@ -1018,11 +1166,7 @@ int dte_softreg_write(dte_t* e, uint32_t addr, uint64_t data) {
     // `start` (EngineCSR.sv:191-193): Core FSM, counters and schedules reset (Core.sv:168-187);
     // the PU tree memories are NOT cleared (DTPU.sv:307-319) -> the resident ensemble stays.
     TRY(drain_all(e));                                    // results of an unfinished previous run are dropped
-    if (e->running) {                                     // cluster counters survive `start` (DTPUCluster.sv:85-97)
-        const uint64_t c0 = cluster0_tuples(e);
-        e->cum_c0 += c0;
-        e->cum_c0_lines += c0 * e->g.tuple_cls;
-    }
+    if (e->running) roll_cluster_counters(e);
     e->lines_received = 0;
     e->cur_w = e->cur_f = e->cur_d = 0;
     e->cur_dev = 0;
@@ -1064,8 +1208,7 @@ int dte_softreg_read(dte_t* e, uint32_t addr, uint64_t* data) {
     const Clock::time_point now = Clock::now();
     // appStatus (DTInference.sv:367-372): pairs of 32-bit debug counters, modelled from the run's counts
     const uint32_t S = std::max(1u, e->g.S), tcl = std::max(1u, e->g.tuple_cls);
-    const Dev& h = e->devs[(size_t)(e->multi() ? e->pos2dev[0] : 0)];
-    const uint64_t n_t = h.tuples_landed;
+    const uint64_t n_t = host_dev(e).tuples_landed;
     const uint64_t c0 = e->running ? cluster0_tuples(e) : 0;
     auto pair32 = [](uint64_t hi, uint64_t lo) { return ((hi & 0xFFFFFFFFull) << 32) | (lo & 0xFFFFFFFFull); };
     switch (addr) {
@@ -1105,118 +1248,11 @@ int dte_softreg_read(dte_t* e, uint32_t addr, uint64_t* data) {
 int dte_stream_write(dte_t* e, const void* cl128, size_t n_lines) {
     if (!e || (!cl128 && n_lines)) return DTE_ERR_ARG;
     const unsigned char* p = static_cast<const unsigned char*>(cl128);
-    bool landed = false;
-    while (n_lines) {
-        if (e->state == dte_engine::ST_TREES) {
-            const uint64_t total = e->regs[2] & 0xFFFFFFFFull, wtotal = e->regs[2] >> 32;   // reg 202
-            if (total == 0 || wtotal == 0 || wtotal >= total)
-                return fail(e, DTE_ERR_CONFIG, "reg 202: total_num_trees_cls=%llu total_num_weights_cls=%llu",
-                            (unsigned long long)total, (unsigned long long)wtotal);
-            if (!e->prog_seen) { e->prog_seen = e->prog_open = true; e->t_prog0 = Clock::now(); }
-            // Chunking (PCIeReceiver.sv:241-264): unless broadcast_trees, the weights stream is cut every
-            // numcls_local_weights lines and the index stream every numcls_local_findexes lines, chunk i going to
-            // devices_list[i % numDevs]; entry 0 is the host node itself (:160-178).  currDevID keeps rotating
-            // from the weights into the index stream, as in the RTL.
-            Flags f = decode_flags(e);
-            const bool cut = f.multiple && !f.bcast_trees && f.ndev > 1;
-            if (cut && (e->regs[3] & 0xFFFFFFFFull) == 0 && wtotal % e->g.w_cls == 0) {
-                // extension: both 16-bit chunk fields left at 0 = "cut the trees evenly over numDevs" — chunks of more
-                // than 65535 lines (e.g. 1024 trees of depth 10 per device) cannot be written into reg 203
-                const uint64_t per = (wtotal / e->g.w_cls + f.ndev - 1) / f.ndev;
-                f.chunk_w = per * e->g.w_cls;
-                f.chunk_f = per * e->g.f_cls;
-            }
-            if (cut && (f.chunk_f == 0 || (!e->multi() && e->node_index >= f.ndev)))
-                return fail(e, DTE_ERR_CONFIG, "reg 203: numcls_local_findexes=%llu numDevs=%u node=%u",
-                            (unsigned long long)f.chunk_f, f.ndev, e->node_index);
-            const size_t take = (size_t)std::min<uint64_t>(n_lines, total - e->lines_received);
-            if (!cut) {
-                const uint64_t w_take = std::min<uint64_t>(take, wtotal > e->lines_received ? wtotal - e->lines_received : 0);
-                e->tree_w[0].insert(e->tree_w[0].end(), p, p + w_take * 16);
-                e->tree_f[0].insert(e->tree_f[0].end(), p + w_take * 16, p + take * 16);
-                e->prog_lines_local += take;
-                if (e->multi()) e->sl3_lines_sent += take;                       // broadcast to the ring as well
-            } else {
-                for (size_t i = 0; i < take; ++i) {
-                    const bool is_w = e->lines_received + i < wtotal;
-                    if (owner_of(e, e->cur_dev) >= 0) {
-                        auto& v = is_w ? e->tree_w[e->cur_dev] : e->tree_f[e->cur_dev];
-                        v.insert(v.end(), p + i * 16, p + i * 16 + 16);
-                    }
-                    if (e->cur_dev == (e->multi() ? 0u : e->node_index)) e->prog_lines_local++;
-                    if (e->cur_dev != 0) e->sl3_lines_sent++;
-                    uint64_t& cnt = is_w ? e->cur_w : e->cur_f;
-                    if (++cnt == (is_w ? f.chunk_w : f.chunk_f)) {
-                        cnt = 0;
-                        e->cur_dev = (e->cur_dev + 1 == f.ndev) ? 0 : e->cur_dev + 1;
-                    }
-                }
-            }
-            e->lines_received += take;
-            p += take * 16;
-            n_lines -= take;
-            if (e->lines_received == total) {
-                // prog_mode = (numcls_received < total_num_weights_cls), PCIeReceiver.sv:136-139
-                int rc = program_devices(e, e->g);
-                for (auto& v : e->tree_w) { v.clear(); v.shrink_to_fit(); }
-                for (auto& v : e->tree_f) { v.clear(); v.shrink_to_fit(); }
-                if (!rc) rc = prepare_data_phase(e, true);
-                e->t_prog1 = Clock::now();
-                e->prog_open = false;
-                if (rc) { e->state = dte_engine::ST_IDLE; e->running = false; return rc; }
-                e->state = dte_engine::ST_DATA;                                 // WAIT_DATA -> RECEIVE_DATA
-                e->cur_dev = 0;
-                e->cur_d = 0;
-            }
-        } else if (e->state == dte_engine::ST_DATA) {
-            // back-pressure: the result queue is bounded (pcie_full_out, PCIeReceiver.sv:126)
-            const size_t tcl = e->g.tuple_cls;
-            uint64_t in_engine = (e->data_lines_in + n_lines) / tcl;                         // results queued once these lines are in
-            if (!e->multi() && e->deal) in_engine = in_engine / e->ndev_ring + e->deal_lines / tcl;   // this node keeps 1/numDevs of them
-            in_engine = in_engine > e->res_read ? in_engine - e->res_read : 0;
-            if (in_engine > e->ring_cap)
-                return fail(e, DTE_ERR_BACKPRESSURE, "result queue full (%llu results would wait, capacity %llu): read result lines first",
-                            (unsigned long long)in_engine, (unsigned long long)e->ring_cap);
-            const size_t tb = e->g.tuple_bytes();
-            const uint64_t lines_before = e->data_lines_in;
-            if (e->group) {
-                // data broadcast (InputDistributor.sv:199-204): every device receives every line
-                TRY(land_group(e, p, n_lines * 16));
-                for (Dev& d : e->devs) d.tuples_landed = (e->data_lines_in + n_lines) * 16 / tb;
-                e->sl3_lines_sent += n_lines;
-            } else if (!e->deal) {
-                TRY(land_dev(e, e->devs[0], p, n_lines * 16));
-                e->devs[0].tuples_landed = (e->data_lines_in + n_lines) * 16 / tb;
-            } else {
-                // data dealing (PCIeReceiver.sv:298-307): batches of core_data_batch_cls lines round-robin over the ring
-                size_t left = n_lines;
-                const unsigned char* q = p;
-                while (left) {
-                    const size_t run = (size_t)std::min<uint64_t>(left, e->deal_lines - e->cur_d);
-                    const int dv = owner_of(e, e->cur_dev);
-                    if (dv >= 0) {
-                        Dev& d = e->devs[(size_t)dv];
-                        TRY(land_dev(e, d, q, run * 16));
-                        d.tuples_landed = d.slot[d.cur].fill / tb - d.slot[d.cur].walked + d.res_enq;   // whole tuples so far on this device
-                    }
-                    if (e->cur_dev != 0) e->sl3_lines_sent += run;
-                    e->cur_d += run;
-                    if (e->cur_d == e->deal_lines) { e->cur_d = 0; e->cur_dev = (e->cur_dev + 1 == e->ndev_ring) ? 0 : e->cur_dev + 1; }
-                    q += run * 16;
-                    left -= run;
-                }
-            }
-            landed = true;
-            e->data_lines_in += n_lines;
-            e->lines_received += n_lines;
-            e->tuples_in += (e->data_lines_in / tcl) - (lines_before / tcl);
-            n_lines = 0;
-        } else {
-            return fail(e, DTE_ERR_STATE, "stream_write while the receiver is idle (write reg 200 first)");
-        }
-    }
-    if (landed) TRY(sync_sources(e));                     // the caller may reuse its buffer when we return
-    return DTE_OK;
+    while (n_lines && e->state == dte_engine::ST_TREES) TRY(receive_tree_lines(e, p, n_lines));
+    if (!n_lines) return DTE_OK;
+    if (e->state != dte_engine::ST_DATA) return fail(e, DTE_ERR_STATE, "stream_write while the receiver is idle (write reg 200 first)");
+    TRY(receive_data_lines(e, p, n_lines));
+    return sync_sources(e);                               // the caller may reuse its buffer when we return
 }
 
 int dte_stream_flush(dte_t* e) {
@@ -1236,10 +1272,10 @@ int dte_stream_read_packets(dte_t* e, void* cl128, uint8_t* last_flags, size_t m
     const uint64_t want_t = std::min<uint64_t>(e->res_read + (uint64_t)max_lines * 4, submitted);
     for (Dev& d : e->devs) TRY(poll_dev(e, d, 0));
     if (global_prefix(e, true) < want_t) {
-        if (e->multi() && e->deal) {
+        if (e->part == Part::Dealt) {
             for (Dev& d : e->devs) TRY(poll_dev(e, d, d.res_enq));
         } else {
-            TRY(poll_dev(e, e->devs[(size_t)(e->group ? e->pos2dev[0] : 0)], want_t));
+            TRY(poll_dev(e, host_dev(e), want_t));
         }
     }
     const uint64_t avail = std::min(global_prefix(e, true), want_t);
@@ -1247,23 +1283,21 @@ int dte_stream_read_packets(dte_t* e, void* cl128, uint8_t* last_flags, size_t m
     float* out = static_cast<float*>(cl128);
     uint64_t i = e->res_read;
     const uint64_t end = e->res_read + (uint64_t)n * 4;
-    const int host_ix = e->multi() ? e->pos2dev[0] : 0;
     while (i < end) {
-        int dv; uint64_t loc;
-        locate_result(e, i, dv, loc);
-        const Dev& d = e->devs[(size_t)dv];
+        uint64_t loc;
+        const Dev& d = locate_result(e, i, loc);
         uint64_t run = end - i;
-        if (e->multi() && e->deal) {
-            const uint64_t bt = e->deal_lines / e->g.tuple_cls;
+        if (e->part == Part::Dealt) {
+            const uint64_t bt = dealing(e).bt;
             run = std::min(run, bt - i % bt);
         }
         const size_t pos = (size_t)(loc % d.ring_cap);
         run = std::min<uint64_t>(run, d.ring_cap - pos);
         memcpy(out + (i - e->res_read), d.h_ring + pos, (size_t)run * 4);
-        if (dv != host_ix) e->sl3_res_lines += (run + 3) / 4;
+        if (&d != &host_dev(e)) e->sl3_res_lines += (run + 3) / 4;
         i += run;
     }
-    if (e->group) e->sl3_res_lines += n;                  // aggregate mode: every result line came back over the ring
+    if (e->part == Part::Chunked) e->sl3_res_lines += n;  // aggregate mode: every result line came back over the ring
     if (last_flags) {
         // `last` closes a PCIe packet every pcie_out_packet_numcls lines: reg 206[55:48], compared as the
         // 8-bit "minus one" copy (EngineCSR.sv:242, DTInference.sv:632-646,659-663)
@@ -1298,38 +1332,29 @@ int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, con
     const Clock::time_point t0 = Clock::now();
     Geom g;
     TRY(decode_geom(e, g));
+    if (e->multi()) TRY(decide_partition(e, g));
     const unsigned char* wl = static_cast<const unsigned char*>(weight_cls);
     const unsigned char* fl = static_cast<const unsigned char*>(findex_cls);
-    PackedEnsemble pk;
-    if (!e->multi()) {
-        TRY(pack_or_fail(e, g, wl, n_weight_cls, fl, n_findex_cls, first_tree, num_local_trees, pk));
-        TRY(upload_ensemble(e, e->devs[0], pk));
-    } else {
-        TRY(decide_partition(e, g));
+    TreeShare share[kMaxRing];
+    share[0] = {wl, fl, n_weight_cls, n_findex_cls, first_tree, num_local_trees};
+    if (e->part == Part::Chunked) {
         if (n_weight_cls % g.w_cls) return fail(e, DTE_ERR_ARG, "weights stream: %zu lines is not a multiple of %u lines per tree", n_weight_cls, g.w_cls);
         const uint32_t T_all = (uint32_t)(n_weight_cls / g.w_cls);
         if (num_local_trees == 0 && first_tree == 0) num_local_trees = T_all;
         const uint32_t G = (uint32_t)e->devs.size();
-        if (!e->group) {                             // replicated
-            TRY(pack_or_fail(e, g, wl, n_weight_cls, fl, n_findex_cls, first_tree, num_local_trees, pk));
-            for (Dev& d : e->devs) TRY(upload_ensemble(e, d, pk));
-        } else {
-            // contiguous chunks in ring order (PCIeReceiver.sv:241-264): reg 203's numcls_local_weights if it is a
-            // whole number of trees that covers the ensemble, else an even split
-            const Flags f = decode_flags(e);
-            const bool programmed = (e->regs[3] & 0xFFFF) != 0 && f.chunk_w % g.w_cls == 0 && (f.chunk_w / g.w_cls) * G >= num_local_trees;
-            const uint32_t per = programmed ? (uint32_t)(f.chunk_w / g.w_cls) : (num_local_trees + G - 1) / G;
-            for (uint32_t r = 0; r < G; ++r) {
-                const uint32_t lo = std::min(num_local_trees, r * per), hi = std::min(num_local_trees, (r + 1) * per);
-                if (hi == lo) return fail(e, DTE_ERR_CONFIG, "ring position %u would hold no trees (%u trees over %u devices)", r, num_local_trees, G);
-                TRY(pack_or_fail(e, g, wl, n_weight_cls, fl, n_findex_cls, first_tree + lo, hi - lo, pk));
-                TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk));
-            }
+        // contiguous chunks in ring order (PCIeReceiver.sv:241-264): reg 203's numcls_local_weights if it is a
+        // whole number of trees that covers the ensemble, else an even split
+        const Flags f = decode_flags(e);
+        const bool programmed = (e->regs[3] & 0xFFFF) != 0 && f.chunk_w % g.w_cls == 0 && (f.chunk_w / g.w_cls) * G >= num_local_trees;
+        const uint32_t per = programmed ? (uint32_t)(f.chunk_w / g.w_cls) : (num_local_trees + G - 1) / G;
+        for (uint32_t r = 0; r < G; ++r) {
+            const uint32_t lo = std::min(num_local_trees, r * per), hi = std::min(num_local_trees, (r + 1) * per);
+            if (hi == lo) return fail(e, DTE_ERR_CONFIG, "ring position %u would hold no trees (%u trees over %u devices)", r, num_local_trees, G);
+            share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
+    TRY(place_ensemble(e, g, share));
     e->g = g;
-    e->prog_partition = !e->multi() ? 0 : (e->group ? 2 : 1);
-    memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
     return DTE_OK;
@@ -1342,14 +1367,11 @@ static int infer_device_common(dte_t* e, const void* d_tuples, size_t n, float* 
     TRY(decode_geom(e, g));
     TRY(check_resident(e, g));
     Dev& d = e->devs[0];
-    d.g.K = g.K; d.g.S = g.S; d.g.missing = g.missing;
     e->g = g;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     cudaStream_t st = pick_stream(d, cuda_stream);
     CUDA_TRY(e, cudaEventRecord(d.ev_t0, st));
-    const char* why = nullptr;
-    cudaError_t rc = launch_walk(d, e->tune, e->forced_variant, d_tuples, n, d_scores, d_labels, st, accumulate, &why);
-    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
+    TRY(walk_or_fail(e, d, d_tuples, n, d_scores, d_labels, st, accumulate));
     CUDA_TRY(e, cudaEventRecord(d.ev_t1, st));
     d.timing_pending = true;
     e->tuples_in += n;
@@ -1503,20 +1525,20 @@ int dte_get_info(dte_t* e, dte_info* info) {
         d0.timing_pending = false;
     }
     memset(info, 0, sizeof *info);
-    info->num_levels = d0.d_top ? d0.g.D : e->g.D;
-    info->num_features = d0.d_top ? d0.g.F() : e->g.F();
+    info->num_levels = d0.d_top ? d0.shape.g.D : e->g.D;
+    info->num_features = d0.d_top ? d0.shape.g.F() : e->g.F();
     info->clusters = e->g.K;
     info->trees_per_pu = e->g.S;
     info->sm_count = (uint32_t)d0.sm_count;
     for (Dev& d : e->devs) {
         info->ensemble_bytes += d.ensemble_bytes;
         info->kernel_launches += d.kernel_launches;
-        if (e->group) info->num_trees += d.T;
+        if (e->part == Part::Chunked) info->num_trees += d.shape.T;
     }
-    if (!e->group) info->num_trees = d0.T;
+    if (e->part != Part::Chunked) info->num_trees = d0.shape.T;
     info->last_walk_ms = e->last_walk_ms;
     info->num_devices = (uint32_t)e->devs.size();
-    info->partition = !e->multi() ? 0u : (e->group ? 2u : 1u);
+    info->partition = info_partition(e->part);
     info->tuples_in = e->tuples_in;
     info->tuples_out = e->tuples_out;
     if (d0.d_top) {
@@ -1542,14 +1564,14 @@ int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     TRY(decode_geom(e, g));
     TRY(check_resident(e, g));
     TRY(drain_all(e));
-    const uint32_t F = d.g.F();
+    const uint32_t F = d.shape.g.F();
     n_tuples = std::max<size_t>(n_tuples, (size_t)d.sm_count * 192 * 4);
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     void* d_x = nullptr;
     float* d_s = nullptr;
     CUDA_TRY(e, cudaMalloc(&d_x, n_tuples * F * 4));
     if (cudaMalloc(&d_s, n_tuples * 4) != cudaSuccess) { cudaFree(d_x); return fail(e, DTE_ERR_NOMEM, "autotune: out of device memory"); }
-    synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n_tuples * F, 0x7091E5ull, 10000u, d.g.missing);
+    synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n_tuples * F, 0x7091E5ull, 10000u, e->g.missing);
     struct Cand { int ilp, pair, stages, phased, warps; };      // warps = 10: the 384-thread (168-register) instantiation
     const Cand cands[] = {{4, 2, 1, 1, 0}, {4, 2, 1, 0, 0}, {4, 2, 1, 1, 10}, {4, 2, 1, 0, 10}, {2, 4, 1, 1, 0}, {2, 4, 1, 0, 0}, {8, 1, 1, 0, 0},
                           {8, 1, 2, 0, 0}, {4, 1, 2, 0, 0}, {2, 2, 2, 0, 0}, {2, 2, 1, 0, 0}};
@@ -1573,7 +1595,7 @@ int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
         for (int rep_i = 0; rep_i < 2 && !rc; ++rep_i) {                     // the second launch is the measurement
             const char* why = nullptr;
             cudaEventRecord(d.ev_t0, d.s_main);
-            cudaError_t st = launch_walk(d, t, KERNEL_AUTO, d_x, n_tuples, d_s, nullptr, d.s_main, false, &why);
+            cudaError_t st = launch_walk(d, e->g, t, KERNEL_AUTO, d_x, n_tuples, d_s, nullptr, d.s_main, false, &why);
             cudaEventRecord(d.ev_t1, d.s_main);
             if (st != cudaSuccess || cudaEventSynchronize(d.ev_t1) != cudaSuccess) { rc = fail(e, DTE_ERR_CUDA, "autotune launch failed: %s", cudaGetErrorString(st)); break; }
             cudaEventElapsedTime(&ms, d.ev_t0, d.ev_t1);

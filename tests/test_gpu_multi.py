@@ -153,6 +153,89 @@ def test_multi_fast_paths_load_and_infer_host(devs):
             assert ei.value.code == -4
 
 
+def _dealt_tuples(n, bt, G, pos):
+    """Tuples ring position `pos` keeps when n tuples are dealt in batches of bt tuples over G positions, round-robin
+    from position 0 (PCIeReceiver.sv:298-307): full batches first, then the short last batch (if any)."""
+    full, rem = divmod(n, bt)
+    return (full // G + (1 if pos < full % G else 0)) * bt + (rem if full % G == pos else 0)
+
+
+def _pair(hi, lo):
+    return ((hi & 0xFFFFFFFF) << 32) | (lo & 0xFFFFFFFF)
+
+
+STATUS_CASES = [("whole", 0), ("own_batches", 0)] + [(p, d) for p in ("dealt", "chunked") for d in DEVICE_LISTS]
+
+
+@pytest.mark.parametrize("partition,devs", STATUS_CASES,
+                         ids=lambda v: v if isinstance(v, str) else "gpus" + "".join(map(str, v if isinstance(v, list) else [v])))
+def test_status_registers_and_info_per_partition(partition, devs):
+    """One line-stream job in each of the four partitions of a handle; the status registers 121-126 / 220 / 224-226
+    and the info() counters, each written as arithmetic on the job's parameters (DTInference.sv:367-372).
+      whole        single device, keeps every tuple
+      own_batches  single device standing for ring position 1 (dte_set_node) on a dealt stream: keeps its batches
+      dealt        multi-device, trees replicated, data dealt in batches over the ring
+      chunked      multi-device, trees cut in per-device chunks, data broadcast, partials ring-combined"""
+    G = len(devs) if isinstance(devs, list) else 3          # ring positions (numDevs, reg 203[39:32])
+    T, D, F, K, n, bt = 48, 6, 64, 2, 132, 8                 # 132 = 16 full batches of 8 tuples + a short batch of 4
+    assert T % G == 0 and n % 4 == 0 and bt % 4 == 0        # whole chunks, whole result lines
+    tl = F // 4                                              # lines per tuple (tuple_numcls)
+    w_cls, f_cls = L.tree_cls(D)
+    tree_lines = T * (w_cls + f_cls)
+    per = T // G                                             # trees per ring position when chunked
+    _, _, x, wl, fl, stream = _case(T, D, F, n, 151)
+    single = partition in ("whole", "own_batches")
+    if partition == "whole":
+        regs = E.csr_from_profile(T, D, 4 * F, K, L.MISSING_DEFAULT, n)
+    else:
+        regs = multi_node_regs(T, D, F, K, n, G, "ensemble" if partition == "chunked" else "data", batch_tuples=bt)
+    S = -(-(per if partition == "chunked" else T) // (8 * K))
+    n0 = n if partition in ("whole", "chunked") else _dealt_tuples(n, bt, G, 0)
+    mine = _dealt_tuples(n, bt, G, 1) if partition == "own_batches" else n    # results this handle exposes
+    if partition == "own_batches":                           # process_done counts this node's own result lines
+        regs[207] = (regs[207] & ~0xFFFFFFFF) | (mine // 4)
+    # ring position 0's tuples drive the cluster-0 counters; on a own_batches handle that is this node's device
+    nt = mine if partition == "own_batches" else n0
+    c0 = -(-nt * K // 8)                                     # tuple i uses clusters (i*K)%8 .. +K-1
+    prog_local = per * (w_cls + f_cls) if partition == "chunked" else tree_lines
+    sent = {"whole": 0,                                      # lines that left for other ring positions
+            "own_batches": (n - n0) * tl,
+            "dealt": tree_lines + (n - n0) * tl,
+            "chunked": tree_lines - prog_local + n * tl}[partition]
+    res_lines = {"whole": 0, "own_batches": 0, "dealt": (n - n0) // 4, "chunked": n // 4}[partition]
+    pk = 8                                                   # data_packet_numcls of csr_from_profile (reg 206[31:24])
+
+    def check(state, nt_now, c0_now, cum, res):
+        r = {a: e.softreg_read(a) for a in (220, 121, 122, 123, 124, 125, 126, 224, 225, 226)}
+        assert r == {220: state, 121: _pair(c0_now, cum + c0_now), 122: _pair(nt_now, (cum + c0_now) * S),
+                     123: _pair(nt_now * tl, prog_local), 124: _pair(nt_now, cum + c0_now), 125: _pair(cum + c0_now, res),
+                     126: _pair(cum + c0_now, (cum + c0_now) * tl), 224: sent, 225: -(-sent // pk), 226: sent}, partition
+
+    with ddt.Engine(devs) as e:
+        e.set_option(E.DTE_OPT_CHUNK_TUPLES, 16)             # several landing buffers per device
+        if partition == "own_batches":
+            e.set_node(1)
+        _write_regs(e, regs)
+        e.start()
+        for pos in range(0, stream.shape[0], 997):
+            e.stream_write(stream[pos:pos + 997])
+        check(3, nt, c0, 0, 0)                               # RECEIVE_DATA, nothing read yet
+        out = e.stream_read(1 << 20)
+        assert out.shape[0] == mine // 4
+        assert e.process_done()
+        check(0, 0, 0, c0, res_lines)                        # IDLE; cluster counters rolled into the cumulative ones
+        info = e.info()
+        assert {k: info[k] for k in ("partition", "num_trees", "num_devices", "tuples_in", "tuples_out")} == {
+            "partition": {"whole": 0, "own_batches": 0, "dealt": 1, "chunked": 2}[partition], "num_trees": T,
+            "num_devices": 1 if single else G, "tuples_in": n, "tuples_out": mine}
+        # a second run that is restarted before it completes: `start` rolls its cluster counters over as well
+        e.start()
+        e.stream_write(stream)
+        e.start()
+        assert e.softreg_read(220) == 1                      # RECEIVE_TREES
+        assert e.softreg_read(121) == _pair(0, 2 * c0) and e.softreg_read(126) == _pair(2 * c0, 2 * c0 * tl)
+
+
 def test_multi_handle_refuses_unsupported_partitions():
     T, D, F, K = 16, 4, 32, 2
     with ddt.Engine([0, 0]) as e:

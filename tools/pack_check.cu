@@ -31,27 +31,28 @@ int main(int argc, char** argv) {
     std::string msg;
     int rc = pack_ensemble(g, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16, 0, 0, pk, msg);
     if (rc) { fprintf(stderr, "pack_ensemble: %d %s\n", rc, msg.c_str()); return 3; }
-    if (pk.T != T) return 4;
+    const EnsembleShape& sh = pk.shape;
+    if (sh.T != T) return 4;
     const uint32_t* X = reinterpret_cast<const uint32_t*>(xs.data());
-    const int BV = pk.wide ? 4 : 2;
+    const int BV = sh.wide ? 4 : 2;
     std::vector<uint32_t> out(n * T);
     for (size_t i = 0; i < n; ++i) {
         const uint32_t* x = X + i * F;
         for (uint32_t t = 0; t < T; ++t) {
             // top: byte offset o into the tree's 8-byte heap records, child = 2o + 8 + 8*right  (step_inc in dte_kernels.cuh)
             uint32_t o = 0;
-            const uint2* tp = pk.top.data() + (size_t)t * pk.top_stride;
-            for (uint32_t lvl = 0; lvl < pk.Dtop; ++lvl) {
+            const uint2* tp = pk.top.data() + (size_t)t * sh.top_stride;
+            for (uint32_t lvl = 0; lvl < sh.Dtop; ++lvl) {
                 const uint2 nd = tp[o / 8];
                 const uint32_t xv = x[nd.y & 0xFFFFu];
                 uint32_t inc = ((int32_t)xv < (int32_t)nd.x) ? 8u : 16u;
                 if (xv == g.missing) inc = nd.y >> 16;
                 o = 2 * o + inc;
             }
-            const uint32_t j = (o >> 3) - (pk.nb - 1);
-            const uint4* rec = pk.bottom.data() + ((size_t)t * pk.nb + j) * BV;
+            const uint32_t j = (o >> 3) - (sh.nb - 1);
+            const uint4* rec = pk.bottom.data() + ((size_t)t * sh.nb + j) * BV;
             uint32_t fp, fl_, fr, mp, ml, mr; uint4 leaves;
-            if (pk.wide) {
+            if (sh.wide) {
                 fp = rec[0].w & 0xFFFFu; mp = rec[0].w >> 16; fl_ = rec[1].x & 0xFFFFu; ml = rec[1].x >> 16;
                 fr = rec[1].y & 0xFFFFu; mr = rec[1].y >> 16; leaves = rec[2];
             } else {
