@@ -127,7 +127,8 @@ def build_partition_check(force=False):
 
 def build_evidence_tools(force=False):
     """tools/racecheck_canonical (the textbook bulk-copy ring run under racecheck) and tools/pipe_microbench (cycles per
-    warp-wide access on the shared-memory / L1 pipe): the small CUDA programs behind DESIGN.md §4."""
+    warp-wide access on the shared-memory / L1 pipe, and the ring fill's L2 -> shared-memory bandwidth with and without
+    CTA-cluster multicast): the small CUDA programs behind DESIGN.md §4."""
     nvcc = nvcc_path()
     if nvcc is None:
         raise RuntimeError("nvcc not found")

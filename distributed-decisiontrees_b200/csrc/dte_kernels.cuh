@@ -100,10 +100,30 @@ __device__ __forceinline__ uint4 ldg128_nc(const void* p) {
     asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
-__device__ __forceinline__ uint4 ldg128_stream(const void* p) {   // read once: keep out of L1
+// L2 eviction priorities.  A walk streams every tuple through L2 once, while the ensemble (tree tops for the ring fill,
+// bottom records for the gather: 24 MiB at cfg3) is re-read by every tile.  Tuple lines are therefore marked
+// evict_first and ensemble lines evict_last, so the stream does not push the ensemble out of L2.
+// The policies are asm volatile so that each use makes its own and no 64-bit policy stays live across the walk.
+__device__ __forceinline__ uint64_t l2_evict_last() {
+    uint64_t q;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(q));
+    return q;
+}
+__device__ __forceinline__ uint64_t l2_evict_first() {
+    uint64_t q;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(q));
+    return q;
+}
+__device__ __forceinline__ uint4 ldg128_stream(const void* p) {   // ensemble record read once per walk: keep out of L1
     uint4 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_evict_last()));
+    return v;
+}
+__device__ __forceinline__ uint4 ldg128_tuple(const void* p) {    // tuple stream: out of L1, first out of L2
+    uint4 v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_evict_first()));
     return v;
 }
 // one 32-byte sector as two 128-bit loads (sm_90 has no 256-bit global load); both halves are issued before either
@@ -138,10 +158,11 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "DONE_%=:\n"
         "}\n" ::"r"(bar), "r"(parity) : "memory");
 }
-// bulk async copy global -> shared of this CTA, completion counted on an mbarrier (TMA bulk engine)
+// bulk async copy global -> shared of this CTA, completion counted on an mbarrier (TMA bulk engine); the source is
+// ensemble data, kept in L2 with evict_last priority
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(l2_evict_last()) : "memory");
 }
 
 // direction of one node step as a byte increment on the 8-byte heap offset: left 8, right 16
@@ -239,12 +260,22 @@ __device__ __forceinline__ void bot_load(BotRec<true>& r, const uint4* rec) {
 // record per 128-bit load, so each load touches 16 sectors instead of 32 — the gather costs what one 256-bit load
 // per lane would, which sm_90 does not have.  `recs` = this tree's records, j = this lane's record.  The halves
 // are swapped back by bot_pair_swap() when the record is consumed.
+// EVICT_LAST: load with the evict_last L2 policy (see l2_evict_last).  The ILP = 8 walks keep 8 records in flight
+// and sit at the 168-register cap, where the policy operand costs spills, so they load without it.
+template <bool EVICT_LAST>
 __device__ __forceinline__ void bot_load_pair(BotRec<false>& r, const uint4* recs, uint32_t j) {
     const uint32_t half = threadIdx.x & 1u;
     const uint32_t jp = __shfl_xor_sync(0xFFFFFFFFu, j, 1);
     const uint32_t je = half ? jp : j, jo = half ? j : jp;     // records of the even and of the odd lane
-    r.a = ldg128_stream(recs + 2 * je + half);                 // even lane: its own a; odd lane: b of the even record
-    r.b = ldg128_stream(recs + 2 * jo + half);                 // even lane: a of the odd record; odd lane: its own b
+    const uint4* pa = recs + 2 * je + half;                    // even lane: its own a; odd lane: b of the even record
+    const uint4* pb = recs + 2 * jo + half;                    // even lane: a of the odd record; odd lane: its own b
+    if constexpr (EVICT_LAST) {
+        r.a = ldg128_stream(pa);
+        r.b = ldg128_stream(pb);
+    } else {
+        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.a.x), "=r"(r.a.y), "=r"(r.a.z), "=r"(r.a.w) : "l"(pa));
+        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.b.x), "=r"(r.b.y), "=r"(r.b.z), "=r"(r.b.w) : "l"(pb));
+    }
 }
 __device__ __forceinline__ void bot_pair_swap(BotRec<false>& r) {
     const bool odd = threadIdx.x & 1u;
@@ -471,15 +502,15 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
                 sts32(a, d.x); sts32(a + row_bytes, d.y); sts32(a + 2 * row_bytes, d.z); sts32(a + 3 * row_bytes, d.w);
             };
             for (; v + 4 <= nvec; v += 4 * P) {
-                uint4 d0 = ldg128_stream(row + v), d1 = ldg128_stream(row + v + 1);
-                uint4 d2 = ldg128_stream(row + v + 2), d3 = ldg128_stream(row + v + 3);
+                uint4 d0 = ldg128_tuple(row + v), d1 = ldg128_tuple(row + v + 1);
+                uint4 d2 = ldg128_tuple(row + v + 2), d3 = ldg128_tuple(row + v + 3);
                 if (!live) { d0 = d1 = d2 = d3 = make_uint4(0, 0, 0, 0); }
                 const uint32_t a = xcol + (4 * v) * row_bytes;
                 put4(a, d0); put4(a + 4 * row_bytes, d1); put4(a + 8 * row_bytes, d2); put4(a + 12 * row_bytes, d3);
             }
             if (sub == 0) {                              // ragged tail (F/4 not a multiple of 4)
                 for (v = nvec & ~3u; v < nvec; ++v) {
-                    uint4 d0 = ldg128_stream(row + v);
+                    uint4 d0 = ldg128_tuple(row + v);
                     if (!live) d0 = make_uint4(0, 0, 0, 0);
                     put4(xcol + (4 * v) * row_bytes, d0);
                 }
@@ -628,7 +659,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
             for (int c = 0; c < ILP; ++c) {
                 const uint32_t j = (o[c] >> 3) - (p.nb - 1);
                 if constexpr (WIDE) bot_load(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
-                else bot_load_pair(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
+                else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
             }
         };
 
