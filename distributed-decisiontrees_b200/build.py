@@ -88,25 +88,33 @@ def build_model(force=False):
     return MODEL_OUT
 
 
-PACK_SRC = os.path.join(HERE, "..", "tools", "pack_check.cu")
-PACK_OUT = os.path.join(HERE, "..", "tools", "pack_check")
-
-
-def build_pack_check(force=False):
-    """Host-only checker of the ensemble repacker (tools/pack_check.cu); used by the CPU test tier."""
-    deps = [PACK_SRC] + DEPS[1:3]
-    if not force and os.path.exists(PACK_OUT) and all(os.path.getmtime(PACK_OUT) >= os.path.getmtime(d) for d in deps):
-        return PACK_OUT
+def build_host_check(name, force=False):
+    """Compile tools/<name>.cu, a host-only checker over the engine headers (runs without a GPU); CPU test tier."""
+    src = os.path.join(HERE, "..", "tools", name + ".cu")
+    out = os.path.join(HERE, "..", "tools", name)
+    deps = [src] + DEPS[1:3]
+    if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
+        return out
     nvcc = nvcc_path()
     if nvcc is None:
         raise RuntimeError("nvcc not found")
-    cmd = [nvcc, "-std=c++17", "-O2"] + GENCODE + ["-cudart", "static", "-o", PACK_OUT, PACK_SRC]
+    cmd = [nvcc, "-std=c++17", "-O2"] + GENCODE + ["-cudart", "static", "-o", out, src]
     if os.path.exists("/usr/bin/g++"):
         cmd[1:1] = ["-ccbin", "/usr/bin/g++"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)
-    return PACK_OUT
+    return out
+
+
+def build_pack_check(force=False):
+    """Host-only checker of the ensemble repacker (tools/pack_check.cu)."""
+    return build_host_check("pack_check", force)
+
+
+def build_plan_check(force=False):
+    """Host-only print of the launch planner's decisions (tools/plan_check.cu)."""
+    return build_host_check("plan_check", force)
 
 
 PART_SRC = os.path.join(HERE, "..", "tools", "partition_check.cpp")

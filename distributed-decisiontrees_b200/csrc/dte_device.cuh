@@ -6,12 +6,14 @@
 #include "dte_kernels.cuh"
 
 #include <algorithm>
+#include <array>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <deque>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace dte {
@@ -62,15 +64,15 @@ struct Geom {
 };
 
 struct Plan {               // how the next walk will be launched
-    int variant = KERNEL_GENERIC;
-    int ilp = 8, pair = 1, nstages = 0, nwarps = 0;   // nwarps = consumer warps = groups * pair
+    int row = -1;           // kTileFamilies row of a tile plan; -1: dt_walk_generic
+    int nstages = 0, nwarps = 0;                       // nwarps = consumer warps = groups * pair
     bool wide = false;
     size_t smem = 0;
-    int threads() const { return variant == KERNEL_GENERIC ? 128 : 32 * (nwarps + (variant == KERNEL_TILE_STAGED ? 1 : 0)); }
-    int thread_bound() const {                         // NT of the instantiation that will run (see dt_walk_tile)
-        const int nt_max = pair == 4 ? 672 : (ilp == 8 ? 288 : 416);
-        return (nt_max > 384 && threads() <= 384) ? 384 : nt_max;
-    }
+    const TileFamily& fam() const { return kTileFamilies[row]; }
+    int variant() const { return row < 0 ? KERNEL_GENERIC : fam().staged ? KERNEL_TILE_STAGED : KERNEL_TILE; }
+    int threads() const { return row < 0 ? 128 : 32 * (nwarps + (fam().staged ? 1 : 0)); }
+    int thread_bound() const { return tile_nt(fam().nt, threads()); }   // NT of the instantiation that will run
+    uint32_t tuples_per_cta() const { return row < 0 ? 128u : 32u * (uint32_t)(nwarps / fam().pair); }
 };
 
 // Shape of an ensemble in the device layout: what the planner and the walk read from the resident ensemble.
@@ -292,97 +294,94 @@ inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages
     return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * 8 + (size_t)F * 32 * groups * 4;
 }
 
-inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
-    Plan p;
-    p.wide = d.shape.wide;
+// The family a DTE_TUNE pin selects: the row with this ilp and pair, else the first row with this pair, else the same
+// with pair = 1.
+inline int tile_row(int ilp, int pair, bool staged) {
+    int first = -1;
+    for (int r = 0; r < kNumTileFamilies; ++r) {
+        const TileFamily& f = kTileFamilies[r];
+        if (f.staged != staged || f.pair != pair) continue;
+        if (f.ilp == ilp) return r;
+        if (first < 0) first = r;
+    }
+    return first >= 0 ? first : tile_row(ilp, 1, staged);
+}
+
+// Tuple groups (32 tuples, F*128 B of shared memory each) of family f that fit next to a ring of nstages stages, and
+// at most `warps` consumer warps when warps > 0.
+inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps) {
+    if (f.staged && d.shape.Dtop < 3) return 0;        // below that there is nothing worth staging
     const uint32_t F = d.shape.g.F();
     const size_t budget = (size_t)d.smem_optin;
-    // tuple groups (32 tuples, F*128 B of shared memory each) that fit next to the ring
-    auto max_groups = [&](int ilp, int pair, int nstages) -> int {
-        const size_t fixed = tile_smem(F, 0, ilp * pair, nstages, d.shape.top_stride);
-        if (fixed >= budget) return 0;
-        const int warp_cap = (pair == 4) ? 20 : (ilp == 8 ? 8 : 12);   // thread bound of dt_walk_tile (+1 producer warp)
-        int g = (int)std::min<size_t>((size_t)(warp_cap / pair), (budget - fixed) / ((size_t)F * 128));
-        if (tune.warps) g = std::min(g, std::max(1, tune.warps / pair));
-        return g;
+    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride);
+    if (fixed >= budget) return 0;
+    int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * 128));
+    if (warps) g = std::min(g, std::max(1, warps / f.pair));
+    return g;
+}
+
+inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
+    auto tile_plan = [&](int row, int nstages, int groups) {
+        const TileFamily& f = kTileFamilies[row];
+        Plan p;
+        p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide;
+        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride);
+        return p;
     };
-    const bool can_stage = d.shape.Dtop >= 3;          // below that there is nothing worth staging
+    Plan generic, staged;
+    generic.wide = d.shape.wide;
     // staged candidates {trees per warp, warps per tuple group, ring stages}; the candidate that fits with the most
     // walks in flight wins (dte_autotune times the alternatives on the resident ensemble).
     const int cand[6][3] = {{4, 2, 1}, {2, 4, 1}, {8, 1, 1}, {8, 1, 2}, {4, 1, 2}, {4, 1, 1}};
-    Plan staged;
-    if (can_stage) {
-        int best = 0;
-        for (auto& c : cand) {
-            int ilp = tune.ilp ? tune.ilp : c[0];
-            int pair = tune.pair ? tune.pair : c[1];
-            int st = tune.stages ? tune.stages : c[2];
-            if (pair == 4) ilp = 2; else if (pair == 2) ilp = (ilp == 2) ? 2 : 4; else { pair = 1; if (ilp != 4 && ilp != 8) ilp = 8; }
-            st = std::max(1, std::min(st, 4));
-            const int g = max_groups(ilp, pair, st);
-            const int score = g * pair * ilp * 8 + (pair == 2 ? 4 : 0) - (pair == 4 ? 4 : 0) + st;
-            if (g >= 1 && score > best) {
-                best = score;
-                staged.variant = KERNEL_TILE_STAGED;
-                staged.ilp = ilp; staged.pair = pair; staged.nstages = st; staged.nwarps = g * pair; staged.wide = d.shape.wide;
-                staged.smem = tile_smem(F, g, ilp * pair, st, d.shape.top_stride);
-            }
-            if (tune.ilp && tune.stages && tune.pair) break;
-        }
+    int best = 0;
+    for (auto& c : cand) {
+        const int row = tile_row(tune.ilp ? tune.ilp : c[0], tune.pair ? tune.pair : c[1], true);
+        const int ilp = kTileFamilies[row].ilp, pair = kTileFamilies[row].pair;
+        const int st = std::max(1, std::min(tune.stages ? tune.stages : c[2], 4));
+        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps);
+        const int score = g * pair * ilp * 8 + (pair == 2 ? 4 : 0) - (pair == 4 ? 4 : 0) + st;
+        if (g >= 1 && score > best) { best = score; staged = tile_plan(row, st, g); }
+        if (tune.ilp && tune.stages && tune.pair) break;
     }
-    Plan tile;
-    {
-        const int ilp = (tune.ilp == 4) ? 4 : 8;
-        const int g = max_groups(ilp, 1, 0);
-        if (g >= 1) {
-            tile.variant = KERNEL_TILE; tile.ilp = ilp; tile.pair = 1; tile.nstages = 0; tile.nwarps = g; tile.wide = d.shape.wide;
-            tile.smem = tile_smem(F, g, ilp, 0, d.shape.top_stride);
-        }
-    }
+    const int tile_r = tile_row(tune.ilp, 1, false);
+    const int tile_g = tile_groups(d, kTileFamilies[tile_r], 0, tune.warps);
+    const Plan tile = tile_g >= 1 ? tile_plan(tile_r, 0, tile_g) : generic;
     if (want == KERNEL_TILE_STAGED && staged.nwarps >= 1) return staged;
     if (want == KERNEL_TILE && tile.nwarps >= 1) return tile;
-    if (want == KERNEL_GENERIC) return p;
+    if (want == KERNEL_GENERIC) return generic;
     // AUTO (or a forced variant that does not fit): staged > tile > generic
     if (staged.nwarps >= 2) return staged;
     if (tile.nwarps >= 1) return tile;
-    return p;
+    return generic;
 }
 
 // phased ring refill needs >= 3 staged levels and at most 4 ring stages (16 mbarriers in the header).
 // On by default from D = 12 (64 KiB stage); at D <= 10 (<= 16 KiB stage) the refill is already cheap and the extra
 // barrier hand-offs cost more than they hide.
 inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
-    if (pl.variant != KERNEL_TILE_STAGED) return 0xFFFFFFFFu;
+    if (pl.variant() != KERNEL_TILE_STAGED) return 0xFFFFFFFFu;
     const bool phased = tune.phased >= 1 || (tune.phased == -1 && d.shape.Dtop >= 10);
     // part A = levels 0..Lw; DTE_TUNE phased=k moves the split k-1 levels further up (smaller part A)
     const uint32_t up = tune.phased > 1 ? (uint32_t)tune.phased - 1 : 0;
     return (phased && d.shape.Dtop >= 3 + up && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
-template <int ILP, int P, bool STAGED, bool WIDE, int NT, bool MC>
-cudaError_t launch_tile_nt(const WalkParams& wp, int grid, int threads, size_t smem, cudaStream_t st) {
-    auto k = dt_walk_tile<ILP, P, STAGED, WIDE, NT, MC>;
-    cudaError_t rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (rc != cudaSuccess) return rc;
-    k<<<grid, threads, smem, st>>>(wp);
-    return cudaGetLastError();
+using WalkKernel = void (*)(WalkParams);
+// The instantiation of family R with the given WIDE and MC flags and thread bound nt (Plan::thread_bound)
+template <int R, bool WIDE, bool MC>
+WalkKernel tile_kernel(int nt) {
+    constexpr TileFamily f = kTileFamilies[R];
+    return nt == f.nt ? dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, f.nt, MC>
+                      : dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, std::min(f.nt, 384), MC>;
 }
-// thread-bound classes (see dt_walk_tile): <= 12 warps -> the 168-register instantiation, else the wide one
-template <int ILP, int P, bool STAGED, bool WIDE, bool MC>
-cudaError_t launch_tile(const WalkParams& wp, int grid, int threads, size_t smem, cudaStream_t st) {
-    constexpr int NT_MAX = P == 4 ? 672 : (ILP == 8 ? 288 : 416);
-    if constexpr (NT_MAX > 384) {
-        if (threads <= 384) return launch_tile_nt<ILP, P, STAGED, WIDE, 384, MC>(wp, grid, threads, smem, st);
-    }
-    return launch_tile_nt<ILP, P, STAGED, WIDE, NT_MAX, MC>(wp, grid, threads, smem, st);
+// [row][2 * WIDE + MC]: every tile kernel, one entry per row of kTileFamilies
+template <size_t... R>
+constexpr auto tile_kernel_table(std::index_sequence<R...>) {
+    using Pick = WalkKernel (*)(int);
+    return std::array<std::array<Pick, 4>, sizeof...(R)>{
+        {{tile_kernel<R, false, false>, tile_kernel<R, false, true>, tile_kernel<R, true, false>, tile_kernel<R, true, true>}...}};
 }
-template <int ILP, int P, bool STAGED>
-cudaError_t launch_tile_any(const WalkParams& wp, bool wide, bool mc, int grid, int threads, size_t smem, cudaStream_t st) {
-    if (mc) return wide ? launch_tile<ILP, P, STAGED, true, true>(wp, grid, threads, smem, st)
-                        : launch_tile<ILP, P, STAGED, false, true>(wp, grid, threads, smem, st);
-    return wide ? launch_tile<ILP, P, STAGED, true, false>(wp, grid, threads, smem, st)
-                : launch_tile<ILP, P, STAGED, false, false>(wp, grid, threads, smem, st);
-}
+inline constexpr auto kTileKernels = tile_kernel_table(std::make_index_sequence<kNumTileFamilies>());
 
 // Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
 // `run`; the layout comes from the resident ensemble.  Returns a cudaError_t.
@@ -417,7 +416,7 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     wp.Lw = phased_level(d, tune, pl);
     wp.tiles = 0;
     cudaError_t rc;
-    if (pl.variant == KERNEL_GENERIC) {
+    if (pl.row < 0) {
         const int threads = 128;
         const unsigned long long blocks = (n + threads - 1) / threads;
         if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
@@ -430,26 +429,16 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
         }
         rc = cudaGetLastError();
     } else {
-        const size_t M = 32ull * (pl.nwarps / pl.pair);
+        const size_t M = pl.tuples_per_cta();
         const unsigned long long tiles = (n + M - 1) / M;
         if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
         wp.tiles = (uint32_t)tiles;
         const int grid = (int)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count);
-        const bool staged = pl.variant == KERNEL_TILE_STAGED;
-        const int threads = pl.threads();
-        const size_t sm = pl.smem;
-#define DTE_LAUNCH(ILP_, P_, ST_) launch_tile_any<ILP_, P_, ST_>(wp, pl.wide, mc, grid, threads, sm, st)
-        if (staged) {
-            if (pl.ilp == 8) rc = DTE_LAUNCH(8, 1, true);
-            else if (pl.pair == 4) rc = DTE_LAUNCH(2, 4, true);
-            else if (pl.pair == 2 && pl.ilp == 2) rc = DTE_LAUNCH(2, 2, true);
-            else if (pl.pair == 2) rc = DTE_LAUNCH(4, 2, true);
-            else rc = DTE_LAUNCH(4, 1, true);
-        } else {
-            if (pl.ilp == 8) rc = DTE_LAUNCH(8, 1, false);
-            else rc = DTE_LAUNCH(4, 1, false);
-        }
-#undef DTE_LAUNCH
+        const WalkKernel k = kTileKernels[pl.row][2 * pl.wide + mc](pl.thread_bound());
+        rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+        if (rc != cudaSuccess) return rc;
+        k<<<grid, pl.threads(), pl.smem, st>>>(wp);
+        rc = cudaGetLastError();
     }
     if (rc == cudaSuccess) d.kernel_launches++;
     return rc;
@@ -457,12 +446,12 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
 
 inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len) {
     const Plan pl = make_plan(d, tune, want);
-    if (pl.variant == KERNEL_GENERIC) {
+    if (pl.row < 0) {
         snprintf(buf, len, "dt_walk_generic<%d>", pl.wide ? 1 : 0);
     } else {
-        const bool staged = pl.variant == KERNEL_TILE_STAGED;
+        const TileFamily& f = pl.fam();
         snprintf(buf, len, "dt_walk_tile<%d, %d, %d, %d, %d> warps=%d stages=%d phased=%d threads=%d smem=%zu",
-                 pl.ilp, pl.pair, staged ? 1 : 0, pl.wide ? 1 : 0, pl.thread_bound(), pl.nwarps, pl.nstages,
+                 f.ilp, f.pair, f.staged ? 1 : 0, pl.wide ? 1 : 0, pl.thread_bound(), pl.nwarps, pl.nstages,
                  phased_level(d, tune, pl) != 0xFFFFFFFFu ? 1 : 0, pl.threads(), pl.smem);
     }
     if (d.shape.C >= 2) {

@@ -1594,9 +1594,9 @@ int dte_get_info(dte_t* e, dte_info* info) {
     info->tuples_out = e->tuples_out;
     info->num_classes = d0.d_top ? d0.shape.C : 0;
     if (d0.d_top) {
-        Plan pl = make_plan(d0, e->tune, e->forced_variant);
-        info->kernel_variant = (uint32_t)pl.variant;
-        info->tuples_per_cta = pl.variant == KERNEL_GENERIC ? 128u : 32u * (uint32_t)(pl.nwarps / pl.pair);
+        const Plan pl = make_plan(d0, e->tune, e->forced_variant);
+        info->kernel_variant = (uint32_t)pl.variant();
+        info->tuples_per_cta = pl.tuples_per_cta();
     }
     return DTE_OK;
 }
@@ -1624,9 +1624,11 @@ int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     CUDA_TRY(e, cudaMalloc(&d_x, n_tuples * F * 4));
     if (cudaMalloc(&d_s, n_tuples * d.shape.C * 4) != cudaSuccess) { cudaFree(d_x); return fail(e, DTE_ERR_NOMEM, "autotune: out of device memory"); }
     synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n_tuples * F, 0x7091E5ull, 10000u, e->g.missing);
-    struct Cand { int ilp, pair, stages, phased, warps; };      // warps = 10: the 384-thread (168-register) instantiation
-    const Cand cands[] = {{4, 2, 1, 1, 0}, {4, 2, 1, 0, 0}, {4, 2, 1, 1, 10}, {4, 2, 1, 0, 10}, {2, 4, 1, 1, 0}, {2, 4, 1, 0, 0}, {8, 1, 1, 0, 0},
-                          {8, 1, 2, 0, 0}, {4, 1, 2, 0, 0}, {2, 2, 2, 0, 0}, {2, 2, 1, 0, 0}};
+    struct Cand { int row, stages, phased, warps; };            // warps = 10: the 384-thread (168-register) instantiation
+    const int r42 = tile_row(4, 2, true), r24 = tile_row(2, 4, true), r81 = tile_row(8, 1, true), r41 = tile_row(4, 1, true),
+              r22 = tile_row(2, 2, true);
+    const Cand cands[] = {{r42, 1, 1, 0}, {r42, 1, 0, 0}, {r42, 1, 1, 10}, {r42, 1, 0, 10}, {r24, 1, 1, 0}, {r24, 1, 0, 0}, {r81, 1, 0, 0},
+                          {r81, 2, 0, 0}, {r41, 2, 0, 0}, {r22, 2, 0, 0}, {r22, 1, 0, 0}};
     const Tune saved = e->tune;
     Tune best = saved;
     float best_ms = 1e30f;
@@ -1634,15 +1636,13 @@ int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     char name[256], line[400];
     int rc = DTE_OK;
     for (const Cand& c : cands) {
+        const TileFamily& f = kTileFamilies[c.row];
+        // the planner stages a pinned family only with >= 2 consumer warps, and a cap is only worth timing when it
+        // removes a tuple group; a plan that stages can always refill phased (Dtop >= 3, at most 4 stages)
+        const int groups = tile_groups(d, f, c.stages, c.warps);
+        if (groups * f.pair < 2 || (c.warps && tile_groups(d, f, c.stages, 0) * f.pair <= c.warps)) continue;
         Tune t = saved;
-        t.ilp = c.ilp; t.pair = c.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps;
-        const Plan pl = make_plan(d, t, KERNEL_AUTO);
-        if (pl.variant != KERNEL_TILE_STAGED || pl.ilp != c.ilp || pl.pair != c.pair || pl.nstages != c.stages) continue;   // does not fit
-        if (c.warps) {                               // only meaningful when the cap actually removes a tuple group
-            Tune u = t; u.warps = 0;
-            if (make_plan(d, u, KERNEL_AUTO).nwarps <= c.warps) continue;
-        }
-        if (c.phased && phased_level(d, t, pl) == 0xFFFFFFFFu) continue;
+        t.ilp = f.ilp; t.pair = f.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps;
         float ms = 0;
         for (int rep_i = 0; rep_i < 2 && !rc; ++rep_i) {                     // the second launch is the measurement
             const char* why = nullptr;

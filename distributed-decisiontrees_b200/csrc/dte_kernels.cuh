@@ -396,6 +396,25 @@ __device__ __forceinline__ void group_barrier(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// The tile families the library instantiates, one row per (ILP, P, STAGED).  The host planner, launcher and kernel
+// names are built from this table (dte_device.cuh), so a row added or removed here leaves no dispatch site behind.
+// The planner takes the first row of a P for a DTE_TUNE pin that names no listed ILP, so row order matters.
+struct TileFamily {
+    int ilp, pair;          // trees per warp, consumer warps per tuple group
+    bool staged;            // a producer warp streams the tree tops through a shared-memory ring
+    int nt;                 // thread bound; a family with nt > 384 is also instantiated for 384 threads (tile_nt)
+};
+constexpr TileFamily kTileFamilies[] = {
+    {8, 1, true, 288}, {4, 1, true, 416}, {4, 2, true, 416}, {2, 2, true, 416}, {2, 4, true, 672},
+    {8, 1, false, 288}, {4, 1, false, 416},
+};
+constexpr int kNumTileFamilies = sizeof(kTileFamilies) / sizeof(kTileFamilies[0]);
+// The planner's consumer-warp cap for thread bound nt: the bound less the producer warp (the non-staged families keep
+// the same cap).  A staged plan that runs the 384-thread instantiation therefore has at most tile_warp_cap(384) warps.
+__host__ __device__ constexpr int tile_warp_cap(int nt) { return nt / 32 - 1; }
+// NT of the instantiation that runs a plan of `threads` threads of a family with thread bound nt
+__host__ __device__ constexpr int tile_nt(int nt, int threads) { return (nt > 384 && threads <= 384) ? 384 : nt; }
+
 // NT = thread bound of the instantiation.  Registers are allocated per SM sub-partition (16 K each), so the
 // per-thread limit is set by ceil(warps / 4): 9..12 warps -> 168 registers, 13..16 warps -> 128.  The planner
 // picks the 384-thread instantiation whenever the plan fits in 12 warps (cfg3: 5 tuple groups x 2 + producer).
@@ -482,8 +501,8 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
     const uint32_t col = grp * 32u + lane;
     const uint32_t xcol = xs_base + col * 4u;
     // exchange slots: P=2: 2 x 128 B per group (step parity); P=4: 3 x 128 B per group (sender sub-1).
-    // 6 groups x 256 B or 5 groups x 384 B both stay inside kXchBytes.
-    static_assert(6 * 256 <= kXchBytes && 5 * 384 <= kXchBytes, "exchange area too small");
+    // P > 1 only in staged families, whose plans give this instantiation at most tile_warp_cap(NT) / P groups.
+    static_assert(P == 1 || tile_warp_cap(NT) / P * (P == 4 ? 384u : 256u) <= kXchBytes, "exchange area too small");
     const uint32_t xch = sbase + kBarBytes + grp * (P == 4 ? 384u : 256u) + lane * 4u;
     auto feat = [&](uint32_t f) { return lds32(xcol + f * row_bytes); };
     uint32_t slot = 0, par = 0;
