@@ -1401,6 +1401,11 @@ int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, con
 
 static int infer_device_common(dte_t* e, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream,
                                bool accumulate, const char* what) {
+    // the tile kernels read tuple rows as 16-byte vectors and every kernel stores 4-byte score words: a misaligned
+    // pointer would fault the walk and leave the caller's CUDA context unusable, so it is refused here
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "%s: d_tuples not 16-byte aligned", what);
+    if (reinterpret_cast<uintptr_t>(d_scores) & 3u)
+        return fail(e, DTE_ERR_ARG, "%s: %s not 4-byte aligned", what, accumulate ? "d_scores_accum" : "d_scores");
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));

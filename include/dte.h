@@ -149,7 +149,9 @@ int dte_load_ensemble_classes(dte_t* engine, const void* weight_cls, size_t n_we
  * (a cudaStream_t passed as void*; NULL = the engine's own stream, then the call synchronises).
  * The CUDA legacy default stream has the handle value 0 in the runtime API; pass DTE_STREAM_LEGACY
  * (= cudaStreamLegacy) or DTE_STREAM_PER_THREAD (= cudaStreamPerThread) to name it explicitly.
- * Single-device handles only (a multi-device handle takes host buffers: dte_infer_host / the line stream). */
+ * Single-device handles only (a multi-device handle takes host buffers: dte_infer_host / the line stream).
+ * d_tuples must be 16-byte aligned (tuple rows are read as 128-bit vectors) and d_scores 4-byte aligned; any other
+ * pointer returns DTE_ERR_ARG before a kernel is launched.  cudaMalloc'd buffers satisfy both. */
 #define DTE_STREAM_LEGACY ((void*)0x1)
 #define DTE_STREAM_PER_THREAD ((void*)0x2)
 int dte_infer_device(dte_t* engine, const void* d_tuples, size_t n, float* d_scores,
@@ -160,7 +162,8 @@ int dte_infer_device(dte_t* engine, const void* d_tuples, size_t n, float* d_sco
  * kernel's own epilogue — d_scores_accum may be a buffer of a PEER GPU (opened with dte_ipc_open),
  * so the ResultsCombiner hop (ResultsCombiner.sv:292-311) rides NVLink with no separate collective.
  * The target must be zeroed before the first contributor starts; the order of the adds is not the
- * ring order, so scores agree with the ring to ~1 ulp per device (north_star's 1e-5), not bit-exactly. */
+ * ring order, so scores agree with the ring to ~1 ulp per device (north_star's 1e-5), not bit-exactly.
+ * Alignment as dte_infer_device: d_tuples 16-byte, d_scores_accum 4-byte, else DTE_ERR_ARG. */
 int dte_infer_device_accumulate(dte_t* engine, const void* d_tuples, size_t n, float* d_scores_accum, void* cuda_stream);
 
 /* Peer-visible device buffers for the call above (cudaIpc*): the owner allocates and publishes the

@@ -22,7 +22,7 @@
 /* Model A is exactly what the GPU executes with add.rn.ftz.f32: subnormal operands read as     */
 /* signed zero, IEEE RNE add, subnormal results flushed to signed zero.  It coincides with the  */
 /* netlist (model B below) on the contract domain: operands are +0 or normal finite, the result */
-/* is exactly zero or normal finite.  tests/test_oracle_adder.py diffs A against B.             */
+/* is exactly zero or normal finite.  tests/test_oracle_selfcheck.py diffs A against B.         */
 /* ------------------------------------------------------------------------------------------ */
 static inline float u2f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 static inline uint32_t f2u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }

@@ -2,8 +2,9 @@
 # compute-sanitizer over the walk kernel that SHIPS for the headline geometry (D = 12, F = 256, AUTO plan =
 # dt_walk_tile<4,2,1,0,384>, phased ring refill, CTAs with two tiles) and over the planner's alternatives.
 # Logs (with the kernel name printed by the test) go to <logdir>/sanitizer_<tool>_<plan>.log.
-#   bash tools/gpu_sanitize.sh [logdir=sanitizer_logs]   memcheck + synccheck over four launch plans and a 3-class
-#                                                        ensemble, racecheck once (AUTO)
+#   bash tools/gpu_sanitize.sh [logdir=sanitizer_logs]   memcheck + synccheck over four launch plans, a 3-class
+#                                                        ensemble and seven kernel-matrix instantiations, racecheck
+#                                                        once (AUTO)
 # racecheck does not model the mbarrier / cp.async.bulk (async-proxy) hand-off: tools/racecheck_canonical.cu is the
 # textbook producer/consumer ring with exactly that synchronisation, run under the same tool for comparison.
 set -u
@@ -24,6 +25,17 @@ done
 # the multi-class epilogue (C = 3, class-boundary stores and the argmax read-back) in the same geometry
 T=tests/test_gpu_multiclass.py::test_multiclass_headline_geometry_multi_tile
 for tool in memcheck synccheck; do run $tool "" "" ; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_multiclass.log"; done
+# instantiations no other test launches, from the kernel matrix (each case pins its own DTE_TUNE; one wave of CTAs
+# + 33 tuples here): the wide-record staged kernels but <4,2,1,1,384>, the P = 4 compact <2,4,1,0,384> and the
+# non-staged wide <4,1,0,1,384>
+for id in "dt_walk_tile<8,1,1,1,288>-C1-typical-D10-F516" "dt_walk_tile<4,1,1,1,384>-C1-typical-D10-F516" \
+          "dt_walk_tile<2,2,1,1,384>-C1-typical-D10-F516" "dt_walk_tile<2,4,1,1,384>-C1-typical-D10-F516" \
+          "dt_walk_tile<2,4,1,1,672>-C1-typical-D10-F516" "dt_walk_tile<2,4,1,0,384>-C1-typical-D11-F512" \
+          "dt_walk_tile<4,1,0,1,384>-C1-typical-D10-F516"; do
+  T="tests/test_gpu_kernel_matrix.py::test_reachable_instantiation_bit_exact[$id]"
+  ktag=$(echo "$id" | cut -d- -f1 | tr -c 'A-Za-z0-9\n' '_')      # run() sets its own $tag
+  for tool in memcheck synccheck; do run $tool "" ""; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_matrix_${ktag}.log"; done
+done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1
 echo "racecheck [canonical textbook pipeline] rc=$? $(grep -E 'canonical|RACECHECK SUMMARY' $OUT/sanitizer_racecheck_canonical.log | tr '\n' ' ' | cut -c1-300)"
