@@ -117,6 +117,11 @@ def build_plan_check(force=False):
     return build_host_check("plan_check", force)
 
 
+def build_bin_check(force=False):
+    """Host-only checker of the binned layout (tools/bin_check.cu)."""
+    return build_host_check("bin_check", force)
+
+
 PART_SRC = os.path.join(HERE, "..", "tools", "partition_check.cpp")
 PART_OUT = os.path.join(HERE, "..", "tools", "partition_check")
 

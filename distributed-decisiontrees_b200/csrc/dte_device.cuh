@@ -67,6 +67,7 @@ struct Plan {               // how the next walk will be launched
     int row = -1;           // kTileFamilies row of a tile plan; -1: dt_walk_generic
     int nstages = 0, nwarps = 0;                       // nwarps = consumer warps = groups * pair
     bool wide = false;
+    bool bin = false;       // binned walk (u8 tile, 4-byte tree tops)
     size_t smem = 0;
     const TileFamily& fam() const { return kTileFamilies[row]; }
     int variant() const { return row < 0 ? KERNEL_GENERIC : fam().staged ? KERNEL_TILE_STAGED : KERNEL_TILE; }
@@ -91,18 +92,91 @@ struct EnsembleShape {
 //                      32 bytes (= one L2 sector) when every feature index < 512, 64 bytes otherwise
 // Source layout (SURVEY R1): per tree W = heap array of 2^(D+1)-1 fp32 words padded to w_cls lines, FI = 2^D-1
 // u16 padded to f_cls lines (DTPU.sv:282-338,579-596).
+//   binned layout (DESIGN.md §9), built only when pack_ensemble is given the edge table:
+//   top_b[t][2^(D-2)]     4-byte heap records rank | fidx << 8 | missing_right << 20
+//   bottom_b              the bottom records with the rank of each node in its threshold word
 struct PackedEnsemble {
     EnsembleShape shape;
     std::vector<uint2> top;
     std::vector<uint4> bottom;
+    std::vector<uint32_t> top_b;
+    std::vector<uint4> bottom_b;
 };
+
+// Per-feature edge table of the binned layout: feature f's distinct live threshold words, sorted as int32, are
+// edges[offsets[f] .. offsets[f+1]).  A live node of f with threshold edges[offsets[f] + r] stores rank r + 1.
+constexpr uint32_t kMaxBinEdges = 254;        // bins 0..254 for values, 255 for the missing pattern
+struct BinEdges {
+    std::vector<uint32_t> offsets;            // F + 1
+    std::vector<uint32_t> edges;
+    uint32_t rank(uint32_t f, uint32_t thr) const {
+        const uint32_t* b = edges.data() + offsets[f];
+        const uint32_t* e = edges.data() + offsets[f + 1];
+        return (uint32_t)(std::lower_bound(b, e, thr, [](uint32_t a, uint32_t v) { return (int32_t)a < (int32_t)v; }) - b) + 1u;
+    }
+};
+
+// Live nodes of one stream tree: not below an early leaf (those are unreachable; the node with bit 14 itself is live).
+// live[i] for the 2^D - 1 internal nodes of fi.
+inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& live) {
+    const uint32_t n_int = (1u << D) - 1;
+    live.assign(n_int, 1);
+    for (uint32_t i = 0; i < n_int; ++i)
+        if ((!live[i] || (fi[i] & 0x4000u)) && 2 * i + 2 < n_int) live[2 * i + 1] = live[2 * i + 2] = 0;
+}
+
+// The edge table over EVERY tree of the streams (not one chunk), so that engines holding different tree chunks of one
+// ensemble bin tuples identically.  Returns 0, -1 (malformed streams) or -4 (a feature index >= F, or a feature with
+// more than kMaxBinEdges distinct live thresholds; nothing is built).
+inline int bin_edges(const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl, BinEdges& out,
+                     std::string& msg) {
+    char buf[256];
+    if (n_wl % g.w_cls || n_fl != (n_wl / g.w_cls) * g.f_cls) { msg = "tree streams: line counts do not match the geometry"; return -1; }
+    const size_t T_all = n_wl / g.w_cls;
+    const uint32_t D = g.D, F = g.F(), n_int = (1u << D) - 1;
+    const size_t wstride = (size_t)g.w_cls * 4, fstride = (size_t)g.f_cls * 8;
+    const uint32_t* Wall = reinterpret_cast<const uint32_t*>(wl);
+    const uint16_t* Fall = reinterpret_cast<const uint16_t*>(fl);
+    std::vector<std::vector<uint32_t>> per(F);
+    std::vector<uint8_t> live;
+    for (size_t t = 0; t < T_all; ++t) {
+        const uint16_t* fi = Fall + t * fstride;
+        live_nodes(fi, D, live);
+        for (uint32_t i = 0; i < n_int; ++i) {
+            if (!live[i]) continue;
+            const uint32_t f = fi[i] & 0x7FFu;
+            if (f >= F) {
+                snprintf(buf, sizeof buf, "tree %zu node %u: feature index %u >= %u features", t, i, f, F);
+                msg = buf; return -4;
+            }
+            per[f].push_back(Wall[t * wstride + i]);
+        }
+    }
+    out.offsets.assign(F + 1, 0);
+    out.edges.clear();
+    for (uint32_t f = 0; f < F; ++f) {
+        std::vector<uint32_t>& v = per[f];
+        std::sort(v.begin(), v.end(), [](uint32_t a, uint32_t b) { return (int32_t)a < (int32_t)b; });
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+        if (v.size() > kMaxBinEdges) {
+            snprintf(buf, sizeof buf, "feature %u has %zu distinct thresholds: a binned layout holds at most %u per feature",
+                     f, v.size(), kMaxBinEdges);
+            msg = buf; return -4;
+        }
+        out.edges.insert(out.edges.end(), v.begin(), v.end());
+        out.offsets[f + 1] = (uint32_t)out.edges.size();
+    }
+    return 0;
+}
 
 // Packs trees [first, first + count) of the streams; `first` is the global stream index of the first packed tree, so
 // with `classes` = C >= 2 tree first + t belongs to class (first + t) % C.  The trees are then stored class-major:
 // class c occupies tree slots [c * gpc * 8, (c + 1) * gpc * 8) in stream order, gpc = ceil(largest class / 8).
+// With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well.
 // Returns 0 or a negative dte_status; *msg receives the reason.
 inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl,
-                         uint32_t first, uint32_t count, uint32_t classes, PackedEnsemble& out, std::string& msg) {
+                         uint32_t first, uint32_t count, uint32_t classes, PackedEnsemble& out, std::string& msg,
+                         const BinEdges* bins = nullptr) {
     char buf[256];
     if (classes < 1) { msg = "class count 0"; return -1; }
     if (n_wl % g.w_cls) {
@@ -171,6 +245,8 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     out.shape = {g, count, Tpad, Dtop, top_stride, nb, wide, classes, gpc, cls_max};
     out.top.assign((size_t)Tpad * top_stride, make_uint2(0u, 8u << 16));
     out.bottom.assign((size_t)Tpad * nb * BV, make_uint4(0, 0, 0, 0));
+    out.top_b.assign(bins ? (size_t)Tpad * top_stride : 0, 0u);
+    out.bottom_b.assign(bins ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
     std::vector<uint32_t> Wk((2u << Dk) - 1);
     std::vector<uint16_t> Fk((1u << Dk) - 1);
     for (uint32_t t = 0; t < count; ++t) {
@@ -226,6 +302,24 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                 bp[j * 2 + 1] = leaves;
             }
         }
+        if (bins) {
+            // Don't-care nodes (the dummy level of D = 1, the constant nodes of an expanded early leaf) store rank 0:
+            // both children hold the same value, so the direction does not matter.  Every other node is a live node of
+            // the stream tree and its threshold is one of its feature's edges.
+            auto rank = [&](uint32_t n) -> uint32_t {
+                const bool dont_care = D == 1 ? n != 0 : (any_early && dead[n]);
+                return dont_care ? 0u : bins->rank(Fk[n] & 0x7FFu, Wk[n]);
+            };
+            uint32_t* tb = out.top_b.data() + (size_t)slot_of[t] * top_stride;
+            for (uint32_t n = 0; n + 1 < (1u << Dtop); ++n)
+                tb[n] = rank(n) | (uint32_t)(Fk[n] & 0x7FFu) << 8 | (uint32_t)((Fk[n] >> 13) & 1u) << 20;
+            uint4* bb = out.bottom_b.data() + (size_t)slot_of[t] * nb * BV;
+            std::copy(bp, bp + (size_t)nb * BV, bb);
+            for (uint32_t j = 0; j < nb; ++j) {
+                const uint32_t n = nb - 1 + j;
+                bb[j * BV].x = rank(n); bb[j * BV].y = rank(2 * n + 1); bb[j * BV].z = rank(2 * n + 2);
+            }
+        }
     }
     return 0;
 }
@@ -260,6 +354,13 @@ struct Dev {
     uint2* d_top = nullptr;
     uint4* d_bottom = nullptr;
     uint64_t ensemble_bytes = 0;
+    // binned layout (dte_load_ensemble_binned only): 4-byte tops, binned bottom records, the edge table (CSR)
+    uint32_t* d_top_b = nullptr;
+    uint4* d_bottom_b = nullptr;
+    uint32_t* d_bin_off = nullptr;
+    uint32_t* d_bin_edges = nullptr;
+    bool run_bin = false;             // the landing slots carry u8 bins (F bytes per tuple) during dte_infer_host_binned
+    size_t run_tuple_bytes() const { return run_bin ? shape.g.F() : shape.g.tuple_bytes(); }
 
     // ---- landing slots ----
     Slot slot[kNumSlots];
@@ -290,8 +391,9 @@ struct Dev {
 };
 
 // ---- launch planning ---------------------------------------------------------------------------
-inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride) {
-    return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * 8 + (size_t)F * 32 * groups * 4;
+// bin: the binned walk's 4-byte tree tops and one byte per feature in the tile
+inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride, bool bin = false) {
+    return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * (bin ? 4 : 8) + (size_t)F * 32 * groups * (bin ? 1 : 4);
 }
 
 // The family a DTE_TUNE pin selects: the row with this ilp and pair, else the first row with this pair, else the same
@@ -307,29 +409,31 @@ inline int tile_row(int ilp, int pair, bool staged) {
     return first >= 0 ? first : tile_row(ilp, 1, staged);
 }
 
-// Tuple groups (32 tuples, F*128 B of shared memory each) of family f that fit next to a ring of nstages stages, and
-// at most `warps` consumer warps when warps > 0.
-inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps) {
+// Tuple groups (32 tuples, F*128 B of shared memory each, F*32 B binned) of family f that fit next to a ring of nstages
+// stages, and at most `warps` consumer warps when warps > 0.
+inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps, bool bin = false) {
     if (f.staged && d.shape.Dtop < 3) return 0;        // below that there is nothing worth staging
     const uint32_t F = d.shape.g.F();
     const size_t budget = (size_t)d.smem_optin;
-    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride);
+    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride, bin);
     if (fixed >= budget) return 0;
-    int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * 128));
+    int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * (bin ? 32 : 128)));
     if (warps) g = std::min(g, std::max(1, warps / f.pair));
     return g;
 }
 
-inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
+// bin: plan the binned walk of the resident binned layout (same candidates and rules, binned tile and top sizes)
+inline Plan make_plan(const Dev& d, const Tune& tune, int want, bool bin = false) {
     auto tile_plan = [&](int row, int nstages, int groups) {
         const TileFamily& f = kTileFamilies[row];
         Plan p;
-        p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide;
-        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride);
+        p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide; p.bin = bin;
+        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride, bin);
         return p;
     };
     Plan generic, staged;
     generic.wide = d.shape.wide;
+    generic.bin = bin;
     // staged candidates {trees per warp, warps per tuple group, ring stages}; the candidate that fits with the most
     // walks in flight wins (dte_autotune times the alternatives on the resident ensemble).
     const int cand[6][3] = {{4, 2, 1}, {2, 4, 1}, {8, 1, 1}, {8, 1, 2}, {4, 1, 2}, {4, 1, 1}};
@@ -338,13 +442,13 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want) {
         const int row = tile_row(tune.ilp ? tune.ilp : c[0], tune.pair ? tune.pair : c[1], true);
         const int ilp = kTileFamilies[row].ilp, pair = kTileFamilies[row].pair;
         const int st = std::max(1, std::min(tune.stages ? tune.stages : c[2], 4));
-        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps);
+        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps, bin);
         const int score = g * pair * ilp * 8 + (pair == 2 ? 4 : 0) - (pair == 4 ? 4 : 0) + st;
         if (g >= 1 && score > best) { best = score; staged = tile_plan(row, st, g); }
         if (tune.ilp && tune.stages && tune.pair) break;
     }
     const int tile_r = tile_row(tune.ilp, 1, false);
-    const int tile_g = tile_groups(d, kTileFamilies[tile_r], 0, tune.warps);
+    const int tile_g = tile_groups(d, kTileFamilies[tile_r], 0, tune.warps, bin);
     const Plan tile = tile_g >= 1 ? tile_plan(tile_r, 0, tile_g) : generic;
     if (want == KERNEL_TILE_STAGED && staged.nwarps >= 1) return staged;
     if (want == KERNEL_TILE && tile.nwarps >= 1) return tile;
@@ -363,37 +467,54 @@ inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
     const bool phased = tune.phased >= 1 || (tune.phased == -1 && d.shape.Dtop >= 10);
     // part A = levels 0..Lw; DTE_TUNE phased=k moves the split k-1 levels further up (smaller part A)
     const uint32_t up = tune.phased > 1 ? (uint32_t)tune.phased - 1 : 0;
-    return (phased && d.shape.Dtop >= 3 + up && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
+    // a binned part A of 8 << Lw bytes is no whole number of 16-byte bulk-copy units at Lw = 0
+    const bool fits = d.shape.Dtop >= 3 + up + (pl.bin ? 1 : 0);
+    return (phased && fits && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
 using WalkKernel = void (*)(WalkParams);
-// The instantiation of family R with the given WIDE and MC flags and thread bound nt (Plan::thread_bound)
-template <int R, bool WIDE, bool MC>
+// The instantiation of family R with the given WIDE, MC and BIN flags and thread bound nt (Plan::thread_bound)
+template <int R, bool WIDE, bool MC, bool BIN>
 WalkKernel tile_kernel(int nt) {
     constexpr TileFamily f = kTileFamilies[R];
-    return nt == f.nt ? dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, f.nt, MC>
-                      : dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, std::min(f.nt, 384), MC>;
+    if constexpr (BIN)
+        return nt == f.nt ? dt_walk_tile_u8<f.ilp, f.pair, f.staged, WIDE, f.nt, MC>
+                          : dt_walk_tile_u8<f.ilp, f.pair, f.staged, WIDE, std::min(f.nt, 384), MC>;
+    else
+        return nt == f.nt ? dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, f.nt, MC>
+                          : dt_walk_tile<f.ilp, f.pair, f.staged, WIDE, std::min(f.nt, 384), MC>;
 }
-// [row][2 * WIDE + MC]: every tile kernel, one entry per row of kTileFamilies
+// [row][4 * BIN + 2 * WIDE + MC]: every tile kernel, one entry per row of kTileFamilies
 template <size_t... R>
 constexpr auto tile_kernel_table(std::index_sequence<R...>) {
     using Pick = WalkKernel (*)(int);
-    return std::array<std::array<Pick, 4>, sizeof...(R)>{
-        {{tile_kernel<R, false, false>, tile_kernel<R, false, true>, tile_kernel<R, true, false>, tile_kernel<R, true, true>}...}};
+    return std::array<std::array<Pick, 8>, sizeof...(R)>{
+        {{tile_kernel<R, false, false, false>, tile_kernel<R, false, true, false>, tile_kernel<R, true, false, false>,
+          tile_kernel<R, true, true, false>, tile_kernel<R, false, false, true>, tile_kernel<R, false, true, true>,
+          tile_kernel<R, true, false, true>, tile_kernel<R, true, true, true>}...}};
 }
 inline constexpr auto kTileKernels = tile_kernel_table(std::make_index_sequence<kNumTileFamilies>());
+// [4 * BIN + 2 * WIDE + MC]
+inline constexpr WalkKernel kGenericKernels[8] = {
+    dt_walk_generic<false, false, false>, dt_walk_generic<false, true, false>, dt_walk_generic<true, false, false>,
+    dt_walk_generic<true, true, false>, dt_walk_generic<false, false, true>, dt_walk_generic<false, true, true>,
+    dt_walk_generic<true, false, true>, dt_walk_generic<true, true, true>};
 
 // Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
-// `run`; the layout comes from the resident ensemble.  Returns a cudaError_t.
+// `run`; the layout comes from the resident ensemble.  bin: d_tuples are u8 bins [n][F], walked against the resident
+// binned layout.  Returns a cudaError_t.
 inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int want_variant, const void* d_tuples, size_t n,
-                               float* d_scores, uint8_t* d_labels, cudaStream_t st, bool accumulate, const char** why) {
+                               float* d_scores, uint8_t* d_labels, cudaStream_t st, bool accumulate, const char** why,
+                               bool bin = false) {
     *why = nullptr;
     if (n == 0) return cudaSuccess;
-    const Plan pl = make_plan(d, tune, want_variant);
+    const Plan pl = make_plan(d, tune, want_variant, bin);
     WalkParams wp;
     wp.top = d.d_top;
-    wp.bottom = d.d_bottom;
-    wp.tuples = static_cast<const float*>(d_tuples);
+    wp.bottom = bin ? d.d_bottom_b : d.d_bottom;
+    wp.tuples = bin ? nullptr : static_cast<const float*>(d_tuples);
+    wp.top4 = bin ? d.d_top_b : nullptr;
+    wp.bins = bin ? static_cast<const uint8_t*>(d_tuples) : nullptr;
     wp.scores = d_scores;
     wp.labels = d_labels;
     wp.n = n;
@@ -408,7 +529,7 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     wp.classes = d.shape.C;
     wp.groups_per_class = d.shape.gpc;
     wp.K = run.K;
-    wp.missing = run.missing;
+    wp.missing = bin ? 255u : run.missing;           // the bin of the missing pattern
     wp.nwarps = (uint32_t)pl.nwarps;
     wp.nstages = (uint32_t)pl.nstages;
     wp.accumulate = accumulate ? 1u : 0u;
@@ -420,13 +541,7 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
         const int threads = 128;
         const unsigned long long blocks = (n + threads - 1) / threads;
         if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
-        if (mc) {
-            if (pl.wide) dt_walk_generic<true, true><<<(unsigned)blocks, threads, 0, st>>>(wp);
-            else dt_walk_generic<false, true><<<(unsigned)blocks, threads, 0, st>>>(wp);
-        } else {
-            if (pl.wide) dt_walk_generic<true, false><<<(unsigned)blocks, threads, 0, st>>>(wp);
-            else dt_walk_generic<false, false><<<(unsigned)blocks, threads, 0, st>>>(wp);
-        }
+        kGenericKernels[4 * bin + 2 * pl.wide + mc]<<<(unsigned)blocks, threads, 0, st>>>(wp);
         rc = cudaGetLastError();
     } else {
         const size_t M = pl.tuples_per_cta();
@@ -434,7 +549,7 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
         if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
         wp.tiles = (uint32_t)tiles;
         const int grid = (int)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count);
-        const WalkKernel k = kTileKernels[pl.row][2 * pl.wide + mc](pl.thread_bound());
+        const WalkKernel k = kTileKernels[pl.row][4 * bin + 2 * pl.wide + mc](pl.thread_bound());
         rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
         if (rc != cudaSuccess) return rc;
         k<<<grid, pl.threads(), pl.smem, st>>>(wp);
@@ -444,14 +559,16 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     return rc;
 }
 
-inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len) {
-    const Plan pl = make_plan(d, tune, want);
+// bin: the binned walk's plan, named dt_walk_generic_u8 / dt_walk_tile_u8
+inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len, bool bin = false) {
+    const Plan pl = make_plan(d, tune, want, bin);
+    const char* sfx = bin ? "_u8" : "";
     if (pl.row < 0) {
-        snprintf(buf, len, "dt_walk_generic<%d>", pl.wide ? 1 : 0);
+        snprintf(buf, len, "dt_walk_generic%s<%d>", sfx, pl.wide ? 1 : 0);
     } else {
         const TileFamily& f = pl.fam();
-        snprintf(buf, len, "dt_walk_tile<%d, %d, %d, %d, %d> warps=%d stages=%d phased=%d threads=%d smem=%zu",
-                 f.ilp, f.pair, f.staged ? 1 : 0, pl.wide ? 1 : 0, pl.thread_bound(), pl.nwarps, pl.nstages,
+        snprintf(buf, len, "dt_walk_tile%s<%d, %d, %d, %d, %d> warps=%d stages=%d phased=%d threads=%d smem=%zu",
+                 sfx, f.ilp, f.pair, f.staged ? 1 : 0, pl.wide ? 1 : 0, pl.thread_bound(), pl.nwarps, pl.nstages,
                  phased_level(d, tune, pl) != 0xFFFFFFFFu ? 1 : 0, pl.threads(), pl.smem);
     }
     if (d.shape.C >= 2) {

@@ -101,6 +101,7 @@ struct dte_engine {
     uint32_t ndev_ring = 1;           // numDevs (reg 203[39:32])
     uint64_t deal_lines = 0;          // Dealt / OwnBatches: data lines per dealt batch
     std::optional<Part> placed;       // how the RESIDENT ensemble was placed (none until a placement completes)
+    BinEdges bins;                    // edge table of the resident binned layout (empty offsets: none resident)
     int prog_pos2dev[kMaxRing];       // ... and on which devices (a run must use the same placement)
 
     // ---- data / result accounting since `start` ----
@@ -268,8 +269,9 @@ int decide_partition(dte_engine* e, const Geom& g) {
 }
 
 // A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
-// layout and the validated feature-index range; K, S and the missing pattern are free to change).
-int check_resident(dte_engine* e, const Geom& g) {
+// layout and the validated feature-index range; K, S and the missing pattern are free to change).  bin: the run walks
+// u8 bins and needs the binned layout as well.
+int check_resident(dte_engine* e, const Geom& g, bool bin = false) {
     if (e->multi() && e->placed) {
         if (e->part != *e->placed)
             return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
@@ -279,6 +281,7 @@ int check_resident(dte_engine* e, const Geom& g) {
     }
     for (Dev& d : e->devs) {
         if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
+        if (bin && !d.d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
                         g.F(), g.D, d.shape.g.F(), d.shape.g.D);
@@ -296,24 +299,40 @@ uint32_t classes_of(const dte_engine* e) { return host_dev(e).shape.C; }
 // ---- placement of the ensemble on the devices ---------------------------------------------------------
 void free_ensemble(Dev& d) {
     cudaSetDevice(d.ordinal);
-    if (d.d_top) cudaFree(d.d_top);
-    if (d.d_bottom) cudaFree(d.d_bottom);
+    for (void* p : {(void*)d.d_top, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges})
+        if (p) cudaFree(p);
     d.d_top = nullptr;
     d.d_bottom = nullptr;
+    d.d_top_b = nullptr;
+    d.d_bottom_b = nullptr;
+    d.d_bin_off = d.d_bin_edges = nullptr;
     d.shape.T = d.shape.Tpad = 0;    // the geometry stays: the landing slots of a run in progress are cut by it
     d.ensemble_bytes = 0;
 }
 
-int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk) {
+template <class T>
+int upload(dte_engine* e, T*& dst, const std::vector<T>& src) {
+    CUDA_TRY(e, cudaMalloc(&dst, std::max<size_t>(1, src.size()) * sizeof(T)));
+    if (!src.empty()) CUDA_TRY(e, cudaMemcpy(dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return DTE_OK;
+}
+
+// `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr
+int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins) {
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
     free_ensemble(d);
-    CUDA_TRY(e, cudaMalloc(&d.d_top, pk.top.size() * sizeof(uint2)));
-    CUDA_TRY(e, cudaMalloc(&d.d_bottom, pk.bottom.size() * sizeof(uint4)));
-    CUDA_TRY(e, cudaMemcpy(d.d_top, pk.top.data(), pk.top.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    CUDA_TRY(e, cudaMemcpy(d.d_bottom, pk.bottom.data(), pk.bottom.size() * sizeof(uint4), cudaMemcpyHostToDevice));
+    TRY(upload(e, d.d_top, pk.top));
+    TRY(upload(e, d.d_bottom, pk.bottom));
     d.shape = pk.shape;
     d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.bottom.size() * sizeof(uint4);
+    if (bins) {
+        TRY(upload(e, d.d_top_b, pk.top_b));
+        TRY(upload(e, d.d_bottom_b, pk.bottom_b));
+        TRY(upload(e, d.d_bin_off, bins->offsets));
+        TRY(upload(e, d.d_bin_edges, bins->edges));
+        d.ensemble_bytes += pk.top_b.size() * sizeof(uint32_t) + pk.bottom_b.size() * sizeof(uint4);
+    }
     return DTE_OK;
 }
 
@@ -327,19 +346,21 @@ struct TreeShare {
 // Place the ensemble for the run's partition: Chunked puts share[r] on the device of ring position r; every other
 // partition packs share[0] once and replicates it.  Records the placement for check_resident.  `classes` >= 2: every
 // share is packed class-major, the class of a tree taken from its global stream index (share.first counts from the
-// start of the stream).
-int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes) {
+// start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
+// binned layout is dropped.
+int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr) {
     const bool chunked = e->part == Part::Chunked;
     PackedEnsemble pk;
     for (size_t r = 0; r < e->devs.size(); ++r) {
         if (chunked || r == 0) {
             const TreeShare& s = share[r];
             std::string msg;
-            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg);
+            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg, bins);
             if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
         }
-        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk));
+        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins));
     }
+    e->bins = bins ? *bins : BinEdges();
     e->placed = e->part;
     memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
     return DTE_OK;
@@ -468,10 +489,11 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
 }
 
 // Launch the walk of n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.
+// bin: `tuples` are u8 bins walked against the binned layout.
 int walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, float* scores, uint8_t* labels, cudaStream_t st,
-                 bool accumulate) {
+                 bool accumulate, bool bin) {
     const char* why = nullptr;
-    const cudaError_t rc = launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, scores, labels, st, accumulate, &why);
+    const cudaError_t rc = launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, scores, labels, st, accumulate, &why, bin);
     if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
@@ -479,7 +501,7 @@ int walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, float* sco
 // Walk the whole tuples that have landed in slot b of device d since the last submit and queue their results.
 int submit_dev(dte_engine* e, Dev& d, int b) {
     Slot& s = d.slot[b];
-    const size_t tb = d.shape.g.tuple_bytes();
+    const size_t tb = d.run_tuple_bytes();
     if (!d.cap_tuples || !tb) return DTE_OK;
     const size_t whole = s.fill / tb, cnt = whole - s.walked;
     if (!cnt) return DTE_OK;
@@ -490,7 +512,7 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // score buffer of this slot drained
     const bool labels = d.sink_sc && d.sink_lb;
-    TRY(walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked * d.slot_C, labels ? s.d_lb + s.walked : nullptr, d.s_main, false));
+    TRY(walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked * d.slot_C, labels ? s.d_lb + s.walked : nullptr, d.s_main, false, d.run_bin));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
     TRY(enqueue_results(e, d, s, s.walked, cnt, labels));
     s.walked = whole;
@@ -556,7 +578,7 @@ void advance_slot(Dev& d) {
 // Land `bytes` of the tuple stream on device d (pinned memory is DMA'd in place, pageable memory goes through the
 // engine's staging ring, h2d_piece).  Full slots are submitted as they fill.
 int land_dev(dte_engine* e, Dev& d, const unsigned char* src, size_t bytes) {
-    const size_t cap_bytes = d.cap_tuples * d.shape.g.tuple_bytes();
+    const size_t cap_bytes = d.cap_tuples * d.run_tuple_bytes();
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     const bool pageable = bytes >= (256u << 10) && is_pageable(src);
     while (bytes) {
@@ -637,7 +659,7 @@ int nccl_combine(dte_engine* e, int b, size_t walked, size_t cnt, bool labels) {
 int submit_group(dte_engine* e, int b) {
     const size_t G = e->devs.size();
     Dev& h = host_dev(e);
-    const size_t tb = h.shape.g.tuple_bytes();
+    const size_t tb = h.run_tuple_bytes();
     if (!h.cap_tuples || !tb) return DTE_OK;
     const size_t whole = h.slot[b].fill / tb, walked = h.slot[b].walked, cnt = whole - walked;
     if (!cnt) return DTE_OK;
@@ -654,7 +676,7 @@ int submit_group(dte_engine* e, int b) {
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));   // every piece has landed here
         CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, h.slot[b].ev_comb, 0));    // the previous combine is done with our partials
-        TRY(walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_part + walked * C, nullptr, d.s_main, false));
+        TRY(walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_part + walked * C, nullptr, d.s_main, false, d.run_bin));
         CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
         s.walked = whole;
     }
@@ -686,7 +708,7 @@ int submit_group(dte_engine* e, int b) {
 int land_group(dte_engine* e, const unsigned char* src, size_t bytes) {
     const size_t G = e->devs.size();
     Dev& h = host_dev(e);
-    const size_t cap_bytes = h.cap_tuples * h.shape.g.tuple_bytes();
+    const size_t cap_bytes = h.cap_tuples * h.run_tuple_bytes();
     static const size_t kMinPiece = 256u << 10;
     uint32_t rot = 0;
     const bool pageable = bytes >= kMinPiece && is_pageable(src);
@@ -759,7 +781,7 @@ int drain_all(dte_engine* e) {
 
 bool fragment_pending(const dte_engine* e) {
     for (const Dev& d : e->devs)
-        if (d.cap_tuples && d.shape.g.tuple_cls && d.slot[d.cur].fill % d.shape.g.tuple_bytes()) return true;
+        if (d.cap_tuples && d.shape.g.tuple_cls && d.slot[d.cur].fill % d.run_tuple_bytes()) return true;
     return false;
 }
 
@@ -817,23 +839,38 @@ int prepare_data_phase(dte_engine* e, bool need_ring) {
     return DTE_OK;
 }
 
+int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels);
+
 // Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
 // score buffer as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every
-// chunk broadcast to all of them (tree chunks + ring combine).
-int infer_host(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
+// chunk broadcast to all of them (tree chunks + ring combine).  bin: h_tuples are u8 bins [n][F] (F bytes per tuple
+// through the same landing slots), walked against the binned layout.
+int infer_host(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels, bool bin) {
     Geom g;
     TRY(decode_geom(e, g));
     if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "infer_host while the tree stream is being received");
     if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
-    TRY(check_resident(e, g));
+    TRY(check_resident(e, g, bin));
     if (n == 0) return DTE_OK;
     e->g = g;
     for (Dev& d : e->devs)                           // every chunk of this call starts on a fresh landing buffer
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
     TRY(prepare_data_phase(e, false));
-    const size_t tb = g.tuple_bytes();
+    if (!bin) return infer_host_run(e, h_tuples, n, h_scores, h_labels);
+    for (Dev& d : e->devs) d.run_bin = true;
+    const int rc = infer_host_run(e, h_tuples, n, h_scores, h_labels);
+    for (Dev& d : e->devs) {                         // the slots carry fp32 tuples again: leave none partly filled
+        if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
+        d.run_bin = false;
+    }
+    return rc;
+}
+
+// The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.
+int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
+    const size_t tb = e->devs[0].run_tuple_bytes();
     std::vector<uint64_t> enq0(e->devs.size());
     for (size_t i = 0; i < e->devs.size(); ++i) {
         Dev& d = e->devs[i];
@@ -1358,8 +1395,10 @@ int dte_process_done(dte_t* e, int* done) {
     return DTE_OK;
 }
 
-int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
-                              size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
+// dte_load_ensemble_classes, and with `binned` dte_load_ensemble_binned: the edge table over every tree of the streams
+// is built, and refused, before anything is packed or uploaded.
+static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
+                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool binned) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1369,6 +1408,12 @@ int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_
     if (e->multi()) TRY(decide_partition(e, g));
     const unsigned char* wl = static_cast<const unsigned char*>(weight_cls);
     const unsigned char* fl = static_cast<const unsigned char*>(findex_cls);
+    BinEdges bins;
+    if (binned) {
+        std::string msg;
+        const int rc = bin_edges(g, wl, n_weight_cls, fl, n_findex_cls, bins, msg);
+        if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
+    }
     TreeShare share[kMaxRing];
     share[0] = {wl, fl, n_weight_cls, n_findex_cls, first_tree, num_local_trees};
     if (e->part == Part::Chunked) {
@@ -1387,11 +1432,21 @@ int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes));
+    TRY(place_ensemble(e, g, share, num_classes, binned ? &bins : nullptr));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
     return DTE_OK;
+}
+
+int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                              size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false);
+}
+
+int dte_load_ensemble_binned(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                             size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, true);
 }
 
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1400,22 +1455,22 @@ int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, con
 }
 
 static int infer_device_common(dte_t* e, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream,
-                               bool accumulate, const char* what) {
+                               bool accumulate, const char* what, bool bin = false) {
     // the tile kernels read tuple rows as 16-byte vectors and every kernel stores 4-byte score words: a misaligned
     // pointer would fault the walk and leave the caller's CUDA context unusable, so it is refused here
-    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "%s: d_tuples not 16-byte aligned", what);
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "%s: %s not 16-byte aligned", what, bin ? "d_bins" : "d_tuples");
     if (reinterpret_cast<uintptr_t>(d_scores) & 3u)
         return fail(e, DTE_ERR_ARG, "%s: %s not 4-byte aligned", what, accumulate ? "d_scores_accum" : "d_scores");
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));
-    TRY(check_resident(e, g));
+    TRY(check_resident(e, g, bin));
     Dev& d = e->devs[0];
     e->g = g;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     cudaStream_t st = pick_stream(d, cuda_stream);
     CUDA_TRY(e, cudaEventRecord(d.ev_t0, st));
-    TRY(walk_or_fail(e, d, d_tuples, n, d_scores, d_labels, st, accumulate));
+    TRY(walk_or_fail(e, d, d_tuples, n, d_scores, d_labels, st, accumulate, bin));
     CUDA_TRY(e, cudaEventRecord(d.ev_t1, st));
     d.timing_pending = true;
     e->tuples_in += n;
@@ -1470,7 +1525,59 @@ int dte_ipc_close(dte_t* e, void* d_ptr, int owner) {
 
 int dte_infer_host(dte_t* e, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
     if (!e || (n && (!h_tuples || !h_scores))) return DTE_ERR_ARG;
-    return infer_host(e, static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels);
+    return infer_host(e, static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels, false);
+}
+
+// ---- binned inference (DESIGN.md §9) ----
+int dte_infer_host_binned(dte_t* e, const void* h_bins, size_t n, float* h_scores, uint8_t* h_labels) {
+    if (!e || (n && (!h_bins || !h_scores))) return DTE_ERR_ARG;
+    return infer_host(e, static_cast<const unsigned char*>(h_bins), n, h_scores, h_labels, true);
+}
+
+int dte_infer_device_binned(dte_t* e, const void* d_bins, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream) {
+    if (!e || (n && (!d_bins || !d_scores))) return DTE_ERR_ARG;
+    return infer_device_common(e, d_bins, n, d_scores, d_labels, cuda_stream, false, "dte_infer_device_binned", true);
+}
+
+int dte_bin_tuples_device(dte_t* e, const void* d_tuples, size_t n, uint8_t* d_bins, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_bins))) return DTE_ERR_ARG;
+    // one 128-bit load of four features per thread
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "dte_bin_tuples_device: d_tuples not 16-byte aligned");
+    if (reinterpret_cast<uintptr_t>(d_bins) & 15u) return fail(e, DTE_ERR_ARG, "dte_bin_tuples_device: d_bins not 16-byte aligned");
+    TRY(single_only(e, "dte_bin_tuples_device"));
+    Geom g;
+    TRY(decode_geom(e, g));
+    TRY(check_resident(e, g, true));
+    if (!n) return DTE_OK;
+    Dev& d = e->devs[0];
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    cudaStream_t st = pick_stream(d, cuda_stream);
+    const unsigned long long nq = (unsigned long long)n * g.F() / 4;
+    const unsigned blocks = (unsigned)std::min<unsigned long long>((nq + 255) / 256, (unsigned long long)d.sm_count * 16);
+    bin_tuples_kernel<<<blocks, 256, 0, st>>>(static_cast<const uint4*>(d_tuples), reinterpret_cast<uint32_t*>(d_bins), nq,
+                                              g.F(), d.d_bin_off, d.d_bin_edges, g.missing);
+    CUDA_TRY(e, cudaGetLastError());
+    if (!cuda_stream) CUDA_TRY(e, cudaStreamSynchronize(st));
+    return DTE_OK;
+}
+
+int dte_bin_edges(dte_t* e, uint32_t* offsets, uint32_t* edges, size_t cap, size_t* total) {
+    if (!e || !offsets || !total) return DTE_ERR_ARG;
+    if (e->bins.offsets.empty()) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
+    const std::vector<uint32_t>& o = e->bins.offsets;
+    *total = e->bins.edges.size();
+    std::copy(o.begin(), o.end(), offsets);
+    if (!edges) return DTE_OK;
+    if (cap < *total) return fail(e, DTE_ERR_ARG, "dte_bin_edges: %zu edges do not fit a buffer of %zu", *total, cap);
+    std::copy(e->bins.edges.begin(), e->bins.edges.end(), edges);
+    return DTE_OK;
+}
+
+int dte_kernel_name_binned(dte_t* e, char* buf, size_t len) {
+    if (!e || !buf || !len) return DTE_ERR_ARG;
+    if (!e->devs[0].d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
+    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, true);
+    return DTE_OK;
 }
 
 int dte_host_alloc(dte_t* e, size_t bytes, void** h_ptr) {

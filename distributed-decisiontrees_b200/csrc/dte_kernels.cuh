@@ -59,6 +59,10 @@ struct WalkParams {
     // see the parameter block they always saw.
     uint32_t classes;
     uint32_t groups_per_class;  // gpc: group g belongs to class g / gpc and accumulates into partial (g % gpc) % K
+    // binned walks (dt_walk_tile_u8, dt_walk_generic<..., BIN>; DESIGN.md §9): u8 bins [n][F] instead of `tuples`, 4-byte tree tops instead of
+    // `top`; `bottom` then holds the binned bottom records (ranks in the threshold words) and `missing` is 255
+    const uint32_t* top4;       // [trees_padded][top_stride] rank | fidx << 8 | missing_right << 20
+    const uint8_t* bins;        // [n][F] row-major
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -80,6 +84,11 @@ __device__ __forceinline__ void red_add_sys(float* addr, float v) {
 __device__ __forceinline__ uint2 lds64(uint32_t addr) {
     uint2 v;
     asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint32_t lds8(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
 __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
@@ -124,6 +133,16 @@ __device__ __forceinline__ uint4 ldg128_tuple(const void* p) {    // tuple strea
     uint4 v;
     asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
                  : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_evict_first()));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg32_tuple(const void* p) {  // binned rows with F % 16 != 0
+    uint32_t v;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(l2_evict_first()));
+    return v;
+}
+__device__ __forceinline__ uint32_t ldg32_nc(const void* p) {
+    uint32_t v;
+    asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(v) : "l"(p));
     return v;
 }
 // one 32-byte sector as two 128-bit loads (sm_90 has no 256-bit global load); both halves are issued before either
@@ -192,6 +211,13 @@ __device__ __forceinline__ uint32_t step_select(uint32_t x, uint32_t thr, uint32
         : "=r"(r) : "r"(x), "r"(thr), "r"(missing), "r"(meta), "r"(a_left), "r"(a_right));
     return r;
 }
+
+// Fields of a tree-top record as step_select() takes them.  fp32 (8 bytes): {thr bits, fidx | (8 + 8*missing_right) << 16}.
+// Binned (4 bytes, in .x): rank | fidx << 8 | missing_right << 20, so the word itself is the meta operand (>= 2^20 exactly
+// when missing goes right), compared against a bin with missing = 255.
+template <bool BIN> __device__ __forceinline__ uint32_t node_thr(uint2 nd) { return BIN ? nd.x & 0xFFu : nd.x; }
+template <bool BIN> __device__ __forceinline__ uint32_t node_fidx(uint2 nd) { return BIN ? (nd.x >> 8) & 0x7FFu : nd.y & 0xFFFFu; }
+template <bool BIN> __device__ __forceinline__ uint32_t node_meta(uint2 nd) { return BIN ? nd.x : nd.y; }
 
 // select partial `j` out of a register file of 8 (j is warp-uniform)
 __device__ __forceinline__ float acc_get(const float (&a)[8], uint32_t j) {
@@ -319,14 +345,19 @@ __device__ __forceinline__ float bot_finish(const BotRec<WIDE>& r, uint32_t miss
 // Any F (up to 2047) and any D; used when the feature-major tile does not fit shared memory and as
 // an independent cross-check of the tile kernels in the tests.
 // MC = multi-class walk (WalkParams::classes >= 2); the MC = false instantiations are the single-class kernels.
+// BIN = binned walk: u8 bins and 4-byte tree tops (WalkParams::bins / top4).
 // ---------------------------------------------------------------------------------------------
-template <bool WIDE, bool MC>
+template <bool WIDE, bool MC, bool BIN = false>
 __global__ void __launch_bounds__(128) dt_walk_generic(const WalkParams p) {
     constexpr int BV = WIDE ? 4 : 2;
     unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
     const uint32_t* x = reinterpret_cast<const uint32_t*>(p.tuples) + i * p.F;
-    auto feat = [&](uint32_t f) { return __ldg(x + f); };
+    const uint8_t* xb = p.bins + i * p.F;
+    auto feat = [&](uint32_t f) -> uint32_t {
+        if constexpr (BIN) return __ldg(xb + f);
+        else return __ldg(x + f);
+    };
     float acc[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) acc[k] = 0.0f;
@@ -337,12 +368,22 @@ __global__ void __launch_bounds__(128) dt_walk_generic(const WalkParams p) {
 #pragma unroll 1
         for (int q = 0; q < 8; ++q) {
             const uint32_t t = g * 8 + q;
-            const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
             uint32_t o = 0;
-            for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
-                uint2 nd = ldg64_nc(tp + o);
-                uint32_t xv = feat(nd.y & 0xFFFFu);
-                o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
+            if constexpr (BIN) {
+                const char* tp = reinterpret_cast<const char*>(p.top4 + (size_t)t * p.top_stride);
+                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+                    const uint2 nd = make_uint2(ldg32_nc(tp + o), 0u);
+                    const uint32_t xv = feat(node_fidx<true>(nd));
+                    o = 2 * o + step_select(xv, node_thr<true>(nd), node_meta<true>(nd), p.missing, 4u, 8u);
+                }
+                o *= 2;                                          // as a byte offset into 8-byte records
+            } else {
+                const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
+                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+                    uint2 nd = ldg64_nc(tp + o);
+                    uint32_t xv = feat(nd.y & 0xFFFFu);
+                    o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
+                }
             }
             const uint32_t j = (o >> 3) - (p.nb - 1);
             BotRec<WIDE> br;
@@ -722,6 +763,319 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
     }
 }
 
+// The binned tile walk (DESIGN.md §9): dt_walk_tile on u8 bins (WalkParams::bins) and 4-byte tree tops (top4), with
+// `bottom` holding the rank-coded records and missing = 255.  The tile word (f/4, column) holds the bins of features
+// 4*(f/4)..+3 of one tuple, and feat(f) is a byte load from it: the same bank as the word, so the per-lane fetch stays
+// at bank = lane.  It is a separate kernel rather than a flag on dt_walk_tile: instantiating the fp32 walk from a
+// shared body changed the code ptxas emits for its ILP = 4 staged kernels and cost the cfg4 shard 2 %.
+template <int ILP, int P, bool STAGED, bool WIDE, int NT, bool MC>
+__global__ void __launch_bounds__(NT, 1) dt_walk_tile_u8(const WalkParams p) {
+    static_assert(ILP * P == 8 || ILP * P == 4, "a step covers a tree8 group or half of one");
+    constexpr int BV = WIDE ? 4 : 2;
+    constexpr int SP = ILP * P;                         // trees per ring stage / per step
+    constexpr uint32_t REC = 4u;                        // bytes per tree-top record
+    constexpr uint32_t kMissingBin = 255u;              // the bin of the missing pattern (an immediate, not p.missing)
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const uint32_t sbase = smem_u32(smem_raw);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t G = p.nwarps / P;                    // tuple groups per CTA
+    const uint32_t M = 32u * G;
+    const uint32_t tree_bytes = p.top_stride * REC;
+    const uint32_t stage_bytes = (uint32_t)SP * tree_bytes;
+    const uint32_t ring_bytes = STAGED ? p.nstages * stage_bytes : 0u;
+    const uint32_t xs_base = sbase + kHdrBytes + ring_bytes;
+    const uint32_t row_bytes = M * 4u;
+    const uint32_t steps = p.groups * (8 / SP);         // SP trees per step
+    const uint32_t my_tiles = (p.tiles > blockIdx.x) ? (p.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+
+    if (STAGED) {
+        if (threadIdx.x == 0) {
+            for (uint32_t s = 0; s < p.nstages; ++s) {
+                mbar_init(sbase + 8 * s, 1);                        // full (part A): producer's arrive + tx bytes
+                mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);   // empty (part A): one arrive per consumer warp
+                mbar_init(sbase + 8 * (2 * p.nstages + s), 1);      // full, part B  (phased refill only)
+                mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);   // empty, part B
+            }
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        }
+        __syncthreads();
+        if (warp == p.nwarps) {
+            // ---------------- producer: stream tree tops through the ring ----------------
+            if (lane == 0) {
+                const uint64_t total = (uint64_t)my_tiles * steps;
+                const char* src0 = reinterpret_cast<const char*>(p.top4);
+                uint32_t slot = 0, par = 1;                          // fresh barrier: parity-1 wait passes
+                uint32_t q = 0;
+                // Phased refill (p.Lw set): a stage is refilled in two parts with their own barriers.
+                //   part A = the first 4*2^(Lw+1) bytes of every tree top (levels 0..Lw and the first record of
+                //   level Lw+1), part B = the rest (75 % of the bytes).  The consumers hand part A back before
+                //   their last level and part B after it, and need part B only from level iteration Lw on, so
+                //   ONE stage overlaps copy and walk: B of step q+1 streams in under levels 0..Lw of step q+1,
+                //   A of step q+1 under the last level + bottom records + leaf sums of step q.  Bulk copies move
+                //   multiples of 16 bytes, so the planner does not phase a binned walk at Lw = 0.
+                const bool phased = p.Lw != 0xFFFFFFFFu;
+                const uint32_t bytesA = phased ? (8u << p.Lw) : tree_bytes;
+                const uint32_t bytesB = tree_bytes - bytesA;
+                for (uint64_t it = 0; it < total; ++it) {
+                    const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
+                    const char* src = src0 + (size_t)q * stage_bytes;
+                    mbar_wait(sbase + 8 * (p.nstages + slot), par);
+                    const uint32_t full = sbase + 8 * slot;
+                    if (!phased) {
+                        mbar_arrive_expect_tx(full, stage_bytes);
+                        if (p.fill_split == 0) {
+                            bulk_g2s(dst, src, stage_bytes, full);                 // the SP tree tops are contiguous: one copy
+                        } else {
+#pragma unroll
+                            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
+                        }
+                    } else {
+                        mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
+#pragma unroll
+                        for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
+                        mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
+                        const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
+                        mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
+#pragma unroll
+                        for (int c = 0; c < SP; ++c)
+                            bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
+                    }
+                    if (++q == steps) q = 0;
+                    if (++slot == p.nstages) { slot = 0; par ^= 1; }
+                }
+            }
+            return;
+        }
+    }
+
+    // ---------------- consumers ----------------
+    const uint32_t grp = warp / P, sub = warp % P;      // tuple group, position inside the warp pair
+    const uint32_t col = grp * 32u + lane;
+    const uint32_t xcol = xs_base + col * 4u;
+    // exchange slots: P=2: 2 x 128 B per group (step parity); P=4: 3 x 128 B per group (sender sub-1).
+    // P > 1 only in staged families, whose plans give this instantiation at most tile_warp_cap(NT) / P groups.
+    static_assert(P == 1 || tile_warp_cap(NT) / P * (P == 4 ? 384u : 256u) <= kXchBytes, "exchange area too small");
+    const uint32_t xch = sbase + kBarBytes + grp * (P == 4 ? 384u : 256u) + lane * 4u;
+    auto feat = [&](uint32_t f) { return lds8(xcol + (f >> 2) * row_bytes + (f & 3u)); };
+    uint32_t slot = 0, par = 0;
+
+    for (uint32_t tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        // ---- load this group's 32 tuples, transposing row-major global -> feature-major shared;
+        //      the P warps of the group take alternate blocks of 16 tile words (64 bins) ----
+        __syncwarp();
+        {
+            const unsigned long long m = (unsigned long long)tile * M + col;
+            const bool live = m < p.n;
+            const uint4* row = reinterpret_cast<const uint4*>(p.bins + (live ? m : 0ull) * p.F);
+            const uint32_t nvec = (p.F & 15u) ? 0u : p.F >> 4;     // 128-bit vectors per row; F % 16 != 0: 32-bit loads
+            if (p.F & 15u) {
+                const uint32_t* roww = reinterpret_cast<const uint32_t*>(row);
+                for (uint32_t w = sub; w < (p.F >> 2); w += P) {
+                    uint32_t d = ldg32_tuple(roww + w);
+                    if (!live) d = 0;
+                    sts32(xcol + w * row_bytes, d);
+                }
+            }
+            uint32_t v = 4 * sub;
+            auto put4 = [&](uint32_t a, const uint4& d) {
+                sts32(a, d.x); sts32(a + row_bytes, d.y); sts32(a + 2 * row_bytes, d.z); sts32(a + 3 * row_bytes, d.w);
+            };
+            for (; v + 4 <= nvec; v += 4 * P) {
+                uint4 d0 = ldg128_tuple(row + v), d1 = ldg128_tuple(row + v + 1);
+                uint4 d2 = ldg128_tuple(row + v + 2), d3 = ldg128_tuple(row + v + 3);
+                if (!live) { d0 = d1 = d2 = d3 = make_uint4(0, 0, 0, 0); }
+                const uint32_t a = xcol + (4 * v) * row_bytes;
+                put4(a, d0); put4(a + 4 * row_bytes, d1); put4(a + 8 * row_bytes, d2); put4(a + 12 * row_bytes, d3);
+            }
+            if (sub == 0) {                              // ragged tail (F/4 not a multiple of 4)
+                for (v = nvec & ~3u; v < nvec; ++v) {
+                    uint4 d0 = ldg128_tuple(row + v);
+                    if (!live) d0 = make_uint4(0, 0, 0, 0);
+                    put4(xcol + (4 * v) * row_bytes, d0);
+                }
+            }
+        }
+        if (P > 1) group_barrier(1 + grp, 32 * P); else __syncwarp();
+
+        float acc[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) acc[k] = 0.0f;
+        float half0 = 0.0f;
+
+        // finish one step: resolve the ILP bottom records into leaves, tree8-reduce, accumulate in the
+        // reference's order.  Called one step late so the record fetch overlaps the next top walk.
+        auto finish = [&](const BotRec<WIDE> (&rec)[ILP], uint32_t qf) {
+            float l[ILP];
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) {
+                BotRec<WIDE> r = rec[c];
+                if constexpr (!WIDE) bot_pair_swap(r);
+                l[c] = bot_finish<WIDE>(r, kMissingBin, feat);
+            }
+            // (1) this warp's share of the tree8 pairing ((l0+l1)+(l2+l3))+((l4+l5)+(l6+l7))
+            float h;
+            if constexpr (ILP == 8)
+                h = fadd_ref(fadd_ref(fadd_ref(l[0], l[1]), fadd_ref(l[2], l[3])),
+                             fadd_ref(fadd_ref(l[4], l[5]), fadd_ref(l[6], l[7])));
+            else if constexpr (ILP == 4)
+                h = fadd_ref(fadd_ref(l[0], l[1]), fadd_ref(l[2], l[3]));
+            else
+                h = fadd_ref(l[0], l[1]);
+            // (2) combine the P warps of the group in pairing order; only sub 0 continues
+            if constexpr (P == 2) {
+                const uint32_t slot_x = xch + 128u * (qf & 1u);              // double-buffered by step parity
+                if (sub == 1) sts32(slot_x, __float_as_uint(h));
+                group_barrier(1 + grp, 64);
+                if (sub == 0) h = fadd_ref(h, __uint_as_float(lds32(slot_x)));
+            } else if constexpr (P == 4) {
+                if (sub != 0) sts32(xch + 128u * (sub - 1u), __float_as_uint(h));
+                group_barrier(1 + grp, 128);
+                if (sub == 0) {
+                    const float s1 = __uint_as_float(lds32(xch)), s2 = __uint_as_float(lds32(xch + 128u));
+                    const float s3 = __uint_as_float(lds32(xch + 256u));
+                    h = fadd_ref(fadd_ref(h, s1), fadd_ref(s2, s3));
+                }
+                group_barrier(1 + grp, 128);             // single exchange buffer: readers done before the next write
+            }
+            // (3) a step covers SP = ILP*P trees: a whole tree8 group, or half of one
+            float r;
+            bool group_done;
+            if constexpr (SP == 8) {
+                r = h;
+                group_done = (sub == 0);
+            } else {
+                group_done = (sub == 0) && (qf & 1u) != 0;
+                r = fadd_ref(half0, h);
+                half0 = h;
+            }
+            if (group_done) {
+                const uint32_t g = qf / (8 / SP);
+                const uint32_t gi = MC ? g % p.groups_per_class : g;     // group index inside its class
+                const uint32_t j = gi % p.K;
+                acc_set(acc, j, fadd_ref(r, acc_get(acc, j)));
+                if constexpr (MC) {
+                    if (gi + 1 == p.groups_per_class) {
+                        const unsigned long long m = (unsigned long long)tile * M + col;
+                        class_boundary(acc, p, m, m < p.n, g / p.groups_per_class);
+                    }
+                }
+            }
+        };
+
+        // one step, first half: walk the top levels of this warp's ILP trees of stage q and ISSUE the
+        // loads of their bottom records into `dst` (not consumed here)
+        auto walk_top = [&](uint32_t q, BotRec<WIDE> (&dst)[ILP]) {
+            const uint32_t t0 = q * SP + sub * ILP;
+            uint32_t o[ILP];
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) o[c] = 0;
+            if (STAGED) {
+                mbar_wait(sbase + 8 * slot, par);
+                const uint32_t tb = sbase + kHdrBytes + slot * stage_bytes + sub * ILP * tree_bytes;
+                // Absolute shared-memory addresses as in dt_walk_tile, with 4-byte records:
+                // A' = tb_c + 2o + 4 + 4*right = (2A + 4 - tb_c) + 4*right.
+                uint32_t A[ILP], kb8[ILP];
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) { A[c] = tb + c * tree_bytes; kb8[c] = REC - A[c]; }
+                // The same skewed schedule as dt_walk_tile: S1 node record = LDS [A], S2 bin = LDS.U8, S3 compare
+                // + child address; tick k issues S3+S1 of chain k and S2 of chain k+-H.
+                constexpr int H = ILP / 2;
+                uint2 nd[ILP];
+                uint32_t xv[ILP];
+                auto S1 = [&](int c) { nd[c] = make_uint2(lds32(A[c]), 0u); };
+                auto S2 = [&](int c) { xv[c] = feat(node_fidx<true>(nd[c])); };
+                auto S3 = [&](int c) {
+                    const uint32_t a2 = A[c] + A[c] + kb8[c];
+                    A[c] = step_select(xv[c], node_thr<true>(nd[c]), node_meta<true>(nd[c]), kMissingBin, a2, a2 + REC);
+                };
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) S1(c);                         // level 0 nodes
+#pragma unroll
+                for (int c = 0; c < H; ++c) S2(c);                           // level 0 features, first half
+                const bool phased = p.Lw != 0xFFFFFFFFu;
+                for (uint32_t lvl = 0; lvl + 1 < p.Dtop; ++lvl) {
+                    if (phased && lvl == p.Lw) mbar_wait(sbase + 8 * (2 * p.nstages + slot), par);   // part B landed
+#pragma unroll
+                    for (int k = 0; k < H; ++k) { S3(k); S1(k); S2(k + H); }         // S2(k+H) still at level lvl
+#pragma unroll
+                    for (int k = H; k < ILP; ++k) { S3(k); S1(k); S2(k - H); }       // S2(k-H) already at level lvl+1
+                }
+                if (phased) {                                                // part A is no longer read: hand it back early
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(sbase + 8 * (p.nstages + slot));
+                }
+#pragma unroll
+                for (int k = 0; k < H; ++k) { S3(k); S2(k + H); }            // last staged level: no further node
+#pragma unroll
+                for (int k = H; k < ILP; ++k) S3(k);
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) o[c] = A[c] - (tb + c * tree_bytes);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(sbase + 8 * ((phased ? 3 * p.nstages : p.nstages) + slot));
+                if (++slot == p.nstages) { slot = 0; par ^= 1; }
+            } else {
+                const char* tp = reinterpret_cast<const char*>(p.top4 + (size_t)t0 * p.top_stride);
+                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+                    uint2 nd[ILP];
+                    uint32_t xv[ILP];
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c) nd[c] = make_uint2(ldg32_nc(tp + (size_t)c * tree_bytes + o[c]), 0u);
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c) xv[c] = feat(node_fidx<true>(nd[c]));
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c)
+                        o[c] = 2 * o[c] + step_select(xv[c], node_thr<true>(nd[c]), node_meta<true>(nd[c]), kMissingBin, 4u, 8u);
+                }
+            }
+            // bottom: last two comparison levels + leaves, ONE 32 B (64 B) record per walk
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) {
+                const uint32_t j = (o[c] >> 2) - (p.nb - 1);
+                if constexpr (WIDE) bot_load(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
+                else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
+            }
+        };
+
+        // Software pipeline with two register buffers (no copies): the records issued by step q are
+        // consumed after the top walk of step q+1, so their L2 latency hides behind shared-memory work.
+        BotRec<WIDE> recA[ILP], recB[ILP];
+        if (steps > 0) {
+            walk_top(0, recA);
+            uint32_t q = 1;
+            for (; q + 1 < steps; q += 2) {
+                walk_top(q, recB);
+                finish(recA, q - 1);
+                walk_top(q + 1, recA);
+                finish(recB, q);
+            }
+            if (q < steps) {
+                walk_top(q, recB);
+                finish(recA, q - 1);
+                finish(recB, q);
+            } else {
+                finish(recA, q - 1);
+            }
+        }
+
+        if constexpr (MC) {
+            const unsigned long long m = (unsigned long long)tile * M + col;
+            if (sub == 0 && m < p.n && p.labels && !p.accumulate) p.labels[m] = class_argmax(p.scores + m * p.classes, p.classes);
+        } else if (sub == 0) {
+            float tot = 0.0f;
+            for (uint32_t j = 0; j < p.K; ++j) tot = fadd_ref(acc_get(acc, j), tot);
+            const unsigned long long m = (unsigned long long)tile * M + col;
+            if (m < p.n) {
+                if (p.accumulate) {
+                    red_add_sys(p.scores + m, tot);
+                } else {
+                    p.scores[m] = tot;
+                    if (p.labels) p.labels[m] = tot > 0.0f ? 1 : 0;
+                }
+            }
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------
 // small helpers: labels, one ring-add hop, synthetic tuples
 // ---------------------------------------------------------------------------------------------
@@ -804,6 +1158,33 @@ __global__ void synth_tuples_kernel(uint32_t* out, unsigned long long first_elem
         uint32_t bits = __float_as_uint(v);
         if ((uint32_t)(z & 0xFFFFFFFFull) % 1000000u < missing_ppm) bits = missing_value;
         out[i] = bits;
+    }
+}
+
+// fp32 tuples [n][F] -> u8 bins [n][F] (DESIGN.md §9): bin = #{ j : (int32)x >= (int32)edges_f[j] } over the int32-sorted
+// edges edges[off[f] .. off[f+1]) of feature f, and 255 for the missing pattern.  One 128-bit load of 4 features and one
+// 32-bit store per thread (F is a multiple of 4, so the 4 features belong to one row); the edges are read through L1.
+__global__ void bin_tuples_kernel(const uint4* __restrict__ x, uint32_t* __restrict__ out, unsigned long long nq, uint32_t F,
+                                  const uint32_t* __restrict__ off, const uint32_t* __restrict__ edges, uint32_t missing) {
+    const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+    for (unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += stride) {
+        const uint4 v = ldg128_tuple(x + q);
+        const uint32_t f0 = (uint32_t)((q * 4ull) % F);
+        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+        uint32_t packed = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint32_t base = __ldg(off + f0 + k);
+            uint32_t lo = base, hi = __ldg(off + f0 + k + 1);
+            while (lo < hi) {                               // first edge > x
+                const uint32_t mid = (lo + hi) >> 1;
+                if ((int32_t)w[k] >= (int32_t)__ldg(edges + mid)) lo = mid + 1;
+                else hi = mid;
+            }
+            const uint32_t b = w[k] == missing ? 255u : lo - base;
+            packed |= b << (8 * k);
+        }
+        out[q] = packed;
     }
 }
 

@@ -56,6 +56,13 @@ ABI = [
     ("dte_synth_tuples_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint64,
                                            C.c_uint32, C.c_uint32, C.c_void_p]),
     ("dte_version", C.c_char_p, []),
+    ("dte_load_ensemble_binned", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
+                                           C.c_uint32]),
+    ("dte_bin_edges", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    ("dte_bin_tuples_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_device_binned", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_binned", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_kernel_name_binned", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
 ]
 
 
@@ -261,13 +268,18 @@ class Engine:
         return bool(d.value)
 
     # -- fast paths -----------------------------------------------------------------------------
-    def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1):
+    def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
-        call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes)."""
+        call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
+        binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
+        feature), which the *_binned calls walk with u8 tuples."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
-        if num_classes == 1:
+        if binned:
+            self._check(self._lib.dte_load_ensemble_binned(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
+                                                           int(first_tree), int(num_local_trees), int(num_classes)))
+        elif num_classes == 1:
             self._check(self._lib.dte_load_ensemble(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
                                                     int(first_tree), int(num_local_trees)))
         else:
@@ -305,6 +317,49 @@ class Engine:
         labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
         self._check(self._lib.dte_infer_host(self._h, _ptr(t), n, _ptr(scores), _ptr(labels)))
         return scores, labels
+
+    # -- binned inference (DESIGN.md §9) -----------------------------------------------------------
+    def bin_edges(self):
+        """-> (offsets uint32 [F + 1], edges uint32 [total]) of the resident binned layout: feature f's edges are
+        edges[offsets[f]:offsets[f + 1]], sorted as int32 (layout.bin_tuples takes them as they are)."""
+        F = int(self.info()["num_features"])
+        offsets = np.empty(F + 1, dtype=np.uint32)
+        total = C.c_size_t()
+        self._check(self._lib.dte_bin_edges(self._h, _ptr(offsets), None, 0, C.byref(total)))
+        edges = np.empty(max(1, total.value), dtype=np.uint32)
+        self._check(self._lib.dte_bin_edges(self._h, _ptr(offsets), _ptr(edges), edges.size, C.byref(total)))
+        return offsets, edges[: total.value]
+
+    def bin_tuples_device(self, d_tuples, n, d_bins, stream=None):
+        """fp32 tuples [n, F] -> u8 bins [n, F], both on the device (16-byte aligned)."""
+        self._check(self._lib.dte_bin_tuples_device(self._h, _ptr(d_tuples), int(n), _ptr(d_bins), _stream(stream)))
+
+    def infer_device_binned(self, d_bins, n, d_scores, d_labels=None, stream=None):
+        """infer_device on u8 bins [n, F] in device memory."""
+        self._check(self._lib.dte_infer_device_binned(self._h, _ptr(d_bins), int(n), _ptr(d_scores), _ptr(d_labels),
+                                                      _stream(stream)))
+
+    def infer_host_binned(self, bins, want_labels=True, out_scores=None, out_labels=None):
+        """infer_host on u8 bins [n, F] in host memory (numpy, or a pinned torch CPU tensor) -> (scores, labels)."""
+        if isinstance(bins, np.ndarray):
+            b = np.ascontiguousarray(bins, dtype=np.uint8)
+            n = b.shape[0]
+        else:
+            b = bins
+            n = int(bins.shape[0])
+        if out_scores is None:
+            nc = self.num_classes()
+            scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
+        else:
+            scores = out_scores
+        labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
+        self._check(self._lib.dte_infer_host_binned(self._h, _ptr(b), n, _ptr(scores), _ptr(labels)))
+        return scores, labels
+
+    def kernel_name_binned(self):
+        buf = C.create_string_buffer(256)
+        self._check(self._lib.dte_kernel_name_binned(self._h, buf, 256))
+        return buf.value.decode()
 
     def infer_device_accumulate(self, d_tuples, n, d_scores_accum, stream=None):
         """Walk and ADD the partial scores into d_scores_accum (local or peer-GPU buffer), fused in the kernel."""

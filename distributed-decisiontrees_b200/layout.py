@@ -79,12 +79,15 @@ def synth_tuples(first_tuple, n, num_features, seed=0x7091E5, missing_ppm=10000,
     return bits.reshape(int(n), F)
 
 
-def synth_ensemble(n_trees, depth_levels, num_features, seed=0xD7EE5, bias=0.02, negative=False):
+def synth_ensemble(n_trees, depth_levels, num_features, seed=0xD7EE5, bias=0.02, negative=False, cuts=None):
     """Random complete trees: thresholds U[0,1), feature index U{0..F-1}, bit 13 random, bit 14 = 0,
     leaves (U[-1,1) + bias) / T so a score is ~N(bias, 1/sqrt(3T)) and both labels occur.
 
     negative=True draws thresholds from U(-1,1) instead (the adversarial set: the int32 compare of
-    the RTL differs from IEEE when both operands are negative)."""
+    the RTL differs from IEEE when both operands are negative).
+
+    cuts=k (<= 254) makes a "histogram-trained" ensemble: every feature gets k cut values drawn like the thresholds,
+    and each node's threshold is one of its feature's cuts, so the ensemble fits the binned layout."""
     T, d, F = int(n_trees), int(depth_levels), int(num_features)
     n_int, n_all = (1 << d) - 1, (2 << d) - 1
     zt = splitmix64(seed, np.arange(T * n_all, dtype=np.uint64)).reshape(T, n_all)
@@ -99,7 +102,30 @@ def synth_ensemble(n_trees, depth_levels, num_features, seed=0xD7EE5, bias=0.02,
     fidx = (zf % np.uint64(F)).astype(np.uint16)
     mr = ((zf >> np.uint64(33)) & np.uint64(1)).astype(np.uint16)
     FI = fidx | (mr << np.uint16(13))
+    if cuts:
+        k = int(cuts)
+        zc = splitmix64(seed ^ 0xC075, np.arange(F * k, dtype=np.uint64)).reshape(F, k)
+        cv = (zc >> np.uint64(40)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+        if negative:
+            cv = cv * np.float32(2.0) - np.float32(1.0)
+        pick = ((zt[:, :n_int] >> np.uint64(8)) % np.uint64(k)).astype(np.int64)     # bits the thresholds did not use
+        W[:, :n_int] = cv[fidx.astype(np.int64), pick]
     return W.view(np.uint32).copy(), FI
+
+
+def bin_tuples(x_words, offsets, edges, missing=MISSING_DEFAULT):
+    """The binned tuple format, defined on the host: fp32 tuple words [n, F] -> u8 bins [n, F].
+
+    bin = number of edges e of the feature with (int32)x >= (int32)e (edges[offsets[f]:offsets[f+1]], sorted as
+    int32: what Engine.bin_edges returns), and 255 where x is the missing pattern."""
+    x = np.ascontiguousarray(x_words).view(np.uint32)
+    edges = np.asarray(edges, dtype=np.uint32).view(np.int32)
+    out = np.empty(x.shape, dtype=np.uint8)
+    for f in range(x.shape[1]):
+        col = x[:, f]
+        b = np.searchsorted(edges[offsets[f]:offsets[f + 1]], col.view(np.int32), side="right")
+        out[:, f] = np.where(col == np.uint32(missing), 255, b)
+    return out
 
 
 def result_lines(scores):

@@ -176,6 +176,37 @@ int dte_ipc_close(dte_t* engine, void* d_ptr, int owner);
  * h_scores (and h_labels if not NULL) are complete.  Pinned host buffers give full PCIe speed. */
 int dte_infer_host(dte_t* engine, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels);
 
+/* ---- binned inference: u8 tuples against rank-coded trees (DESIGN.md §9) --------------------- */
+/* dte_load_ensemble_classes (same arguments, same placement: class-major, Dealt replicates, Chunked keeps each ring
+ * position's tree range), and in addition the binned layout of a histogram-trained ensemble.  Edges of feature f = the
+ * distinct threshold words of the LIVE nodes testing f (not below an early leaf), sorted as int32, over EVERY tree of
+ * the streams passed in, so engines loaded with different first_tree chunks agree on the bins.  A tuple value x of
+ * feature f travels as one byte: bin = the number of edges e with (int32)x >= (int32)e, and 255 for the missing
+ * pattern (reg 205); every score word and label of a binned walk equals the fp32 walk's on x.  A bin above the
+ * feature's edge count acts like the edge count.  A feature with more than 254 edges returns DTE_ERR_UNSUPPORTED
+ * (the message names it) before anything is uploaded: the resident ensemble stays.  The fp32 calls keep working on a
+ * binned load; dte_load_ensemble, dte_load_ensemble_classes and a tree stream drop the binned layout, after which the
+ * binned calls return DTE_ERR_STATE. */
+int dte_load_ensemble_binned(dte_t* engine, const void* weight_cls, size_t n_weight_cls,
+                             const void* findex_cls, size_t n_findex_cls,
+                             uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes);
+/* The edge table of the resident binned layout, CSR: offsets[F + 1] (always written), feature f's edges (uint32 words,
+ * int32 order) are edges[offsets[f] .. offsets[f+1]).  *total = number of edges; edges = NULL only sizes, a cap below
+ * *total returns DTE_ERR_ARG.  Lets a caller bin on its side (searchsorted, side='right', over the int32 views). */
+int dte_bin_edges(dte_t* engine, uint32_t* offsets, uint32_t* edges, size_t cap, size_t* total);
+/* fp32 tuples [n][F] in device memory -> u8 bins [n][F] with the run's missing pattern.  Single-device handles;
+ * d_tuples and d_bins 16-byte aligned, else DTE_ERR_ARG.  Stream as dte_infer_device. */
+int dte_bin_tuples_device(dte_t* engine, const void* d_tuples, size_t n, uint8_t* d_bins, void* cuda_stream);
+/* dte_infer_device on u8 bins [n][F]: [n] or [n][C] scores and labels as there.  Single-device handles; d_bins
+ * 16-byte and d_scores 4-byte aligned, else DTE_ERR_ARG before any launch. */
+int dte_infer_device_binned(dte_t* engine, const void* d_bins, size_t n, float* d_scores, uint8_t* d_labels,
+                            void* cuda_stream);
+/* dte_infer_host on u8 bins [n][F] (F bytes per tuple over PCIe instead of 4F): every handle kind, single and
+ * multi-device (Dealt, Chunked); the same landing pipeline and the same refusal of a partial line-stream tuple. */
+int dte_infer_host_binned(dte_t* engine, const void* h_bins, size_t n, float* h_scores, uint8_t* h_labels);
+/* dte_kernel_name of the binned walk ("dt_walk_tile_u8<...> ..." / "dt_walk_generic_u8<...>"). */
+int dte_kernel_name_binned(dte_t* engine, char* buf, size_t len);
+
 /* Page-locked host memory every device of the handle can DMA from / to at full PCIe speed (cudaHostAlloc, portable):
  * what a Catapult host gets from the driver's DMA-buffer allocator (the slot buffers behind rtl/PCIeShim.sv:99-141).
  * Pageable memory works everywhere too, through the CUDA driver's staging copies (about 5 x slower). */

@@ -36,6 +36,13 @@ for id in "dt_walk_tile<8,1,1,1,288>-C1-typical-D10-F516" "dt_walk_tile<4,1,1,1,
   ktag=$(echo "$id" | cut -d- -f1 | tr -c 'A-Za-z0-9\n' '_')      # run() sets its own $tag
   for tool in memcheck synccheck; do run $tool "" ""; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_matrix_${ktag}.log"; done
 done
+# the binned walk (u8 tile, 4-byte tops): the headline plan (phased), the D = 5 staged plan that must not phase, and a
+# non-staged plan (D = 3 has one top level and is never staged)
+for T in tests/test_gpu_binned.py::test_headline_binned_multi_tile tests/test_gpu_binned.py::test_phased_at_depth_5_stays_unphased \
+         "tests/test_gpu_binned.py::test_depths[3]"; do
+  btag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  for tool in memcheck synccheck; do run $tool "" ""; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_binned_${btag}.log"; done
+done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1
 echo "racecheck [canonical textbook pipeline] rc=$? $(grep -E 'canonical|RACECHECK SUMMARY' $OUT/sanitizer_racecheck_canonical.log | tr '\n' ' ' | cut -c1-300)"
