@@ -123,10 +123,26 @@ __device__ __forceinline__ uint64_t l2_evict_first() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(q));
     return q;
 }
-__device__ __forceinline__ uint4 ldg128_stream(const void* p) {   // ensemble record read once per walk: keep out of L1
+__device__ __forceinline__ uint4 ldg128_stream(const void* p) {   // dt_walk_generic's bottom records: out of L1
     uint4 v;
     asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
                  : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_evict_last()));
+    return v;
+}
+// The tile walks' bottom-record gather.  The tuples of one CTA tile share records: their paths are skewed (a node
+// sends a tuple right with probability 1 - threshold), so at cfg3 the 160 tuples of a tile reach ~89 distinct records
+// of a tree, for which the paired gather issues ~144 sector requests (tools/gather_paths.py).  The records are
+// therefore allocated in L1 with evict_last priority, so a record another warp of the tile fetches next is served
+// from L1; the tuple-tile loads stay no_allocate, so the tuple stream cannot evict them (DESIGN.md §4).
+__device__ __forceinline__ uint4 ldg128_bot(const void* p) {      // and evict_last in L2 (see l2_evict_last)
+    uint4 v;
+    asm volatile("ld.global.nc.L1::evict_last.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(l2_evict_last()));
+    return v;
+}
+__device__ __forceinline__ uint4 ldg128_bot_l1(const void* p) {   // the L1 policy alone, without the L2 policy operand
+    uint4 v;
+    asm volatile("ld.global.nc.L1::evict_last.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
 __device__ __forceinline__ uint4 ldg128_tuple(const void* p) {    // tuple stream: out of L1, first out of L2
@@ -268,26 +284,27 @@ __device__ __forceinline__ uint8_t class_argmax(const float* row, uint32_t C) {
 template <bool WIDE> struct BotRec;
 template <> struct BotRec<false> { uint4 a, b; };
 template <> struct BotRec<true> { uint4 a, b, c; };
-#ifndef DTE_BOT_NA
-#define DTE_BOT_NA 1     // bottom records are touched once per (tuple, tree): do not allocate them in L1
-#endif
+// bot_load: the generic walk's record loads
 __device__ __forceinline__ void bot_load(BotRec<false>& r, const uint4* rec) {
-#if DTE_BOT_NA
     ldg_sector_nc_na(rec, r.a, r.b);
-#else
-    ldg_sector_nc(rec, r.a, r.b);
-#endif
 }
 __device__ __forceinline__ void bot_load(BotRec<true>& r, const uint4* rec) {
     ldg_sector_nc(rec, r.a, r.b);
     r.c = ldg128_nc(rec + 2);
 }
+// Wide records in the tile kernels: one 64-byte record per lane, with the tile gather's L1 policy (see ldg128_bot)
+__device__ __forceinline__ void bot_load_tile(BotRec<true>& r, const uint4* rec) {
+    r.a = ldg128_bot_l1(rec);
+    r.b = ldg128_bot_l1(rec + 1);
+    r.c = ldg128_bot_l1(rec + 2);
+}
 // Compact records in the tile kernels (all 32 lanes active): the two lanes of a pair fetch the two halves of ONE
 // record per 128-bit load, so each load touches 16 sectors instead of 32 — the gather costs what one 256-bit load
 // per lane would, which sm_90 does not have.  `recs` = this tree's records, j = this lane's record.  The halves
 // are swapped back by bot_pair_swap() when the record is consumed.
-// EVICT_LAST: load with the evict_last L2 policy (see l2_evict_last).  The ILP = 8 walks keep 8 records in flight
-// and sit at the 168-register cap, where the policy operand costs spills, so they load without it.
+// EVICT_LAST: the loads also carry the evict_last L2 policy (see l2_evict_last).  The ILP = 8 walks keep 8 records in
+// flight and sit at the 168-register cap, where the policy operand costs spills, so they load without it; the L1
+// policy is a qualifier of the load and costs no register, so every tile walk has it (see ldg128_bot).
 template <bool EVICT_LAST>
 __device__ __forceinline__ void bot_load_pair(BotRec<false>& r, const uint4* recs, uint32_t j) {
     const uint32_t half = threadIdx.x & 1u;
@@ -296,11 +313,11 @@ __device__ __forceinline__ void bot_load_pair(BotRec<false>& r, const uint4* rec
     const uint4* pa = recs + 2 * je + half;                    // even lane: its own a; odd lane: b of the even record
     const uint4* pb = recs + 2 * jo + half;                    // even lane: a of the odd record; odd lane: its own b
     if constexpr (EVICT_LAST) {
-        r.a = ldg128_stream(pa);
-        r.b = ldg128_stream(pb);
-    } else {
-        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.a.x), "=r"(r.a.y), "=r"(r.a.z), "=r"(r.a.w) : "l"(pa));
-        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.b.x), "=r"(r.b.y), "=r"(r.b.z), "=r"(r.b.w) : "l"(pb));
+        r.a = ldg128_bot(pa);
+        r.b = ldg128_bot(pb);
+    } else {      // ldg128_bot_l1 written out: through the helper, ptxas spills in dt_walk_tile_u8<8, 1, 0, 0, 288>
+        asm volatile("ld.global.nc.L1::evict_last.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.a.x), "=r"(r.a.y), "=r"(r.a.z), "=r"(r.a.w) : "l"(pa));
+        asm volatile("ld.global.nc.L1::evict_last.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.b.x), "=r"(r.b.y), "=r"(r.b.z), "=r"(r.b.w) : "l"(pb));
     }
 }
 __device__ __forceinline__ void bot_pair_swap(BotRec<false>& r) {
@@ -718,7 +735,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
 #pragma unroll
             for (int c = 0; c < ILP; ++c) {
                 const uint32_t j = (o[c] >> 3) - (p.nb - 1);
-                if constexpr (WIDE) bot_load(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
+                if constexpr (WIDE) bot_load_tile(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
                 else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
             }
         };
@@ -1031,7 +1048,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_u8(const WalkParams p) {
 #pragma unroll
             for (int c = 0; c < ILP; ++c) {
                 const uint32_t j = (o[c] >> 2) - (p.nb - 1);
-                if constexpr (WIDE) bot_load(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
+                if constexpr (WIDE) bot_load_tile(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
                 else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
             }
         };

@@ -8,8 +8,12 @@
 // ring) with CTA clusters of 1, 2 and 4 CTAs, the latter two with multicast copies (see run_fill).
 // Addresses come from a per-lane LCG so consecutive accesses are independent (no latency chain); the ALU work per
 // access (~4 instructions) is far below the issue limit at these rates.
+//   pipe_microbench --replay FILE   replays the tile walk's paired bottom-record gather instead (see run_replay) over
+//                                   the record indices FILE holds (tools/gather_paths.py --out FILE)
 #include <cstdio>
 #include <cstdint>
+#include <cstring>
+#include <random>
 #include <vector>
 #include <cuda_runtime.h>
 
@@ -200,11 +204,154 @@ double run(uint32_t records, int iters, const uint4* g, uint32_t gmask, unsigned
     return m / g_sms / ((double)iters * 11.0);      // cycles per warp instruction per SM (11 warps issue `iters` each)
 }
 
-int main() {
+// Replay of the tile walk's bottom-record gather (bot_load_pair in csrc/dte_kernels.cuh) in the order of the cfg3 plan,
+// dt_walk_tile<4, 2, 1, 0, 384>: G tuple groups of 32 tuples per CTA and two warps per group; of every tree8 step,
+// sub-warp 0 gathers trees 8q..8q+3 and sub-warp 1 trees 8q+4..8q+7, all groups of a CTA walk the same trees, and no
+// warp runs a step ahead of the others (the plan's one-stage ring; here a CTA barrier per step).  A warp issues the
+// records of step q before it consumes those of step q - 1, as the walk's two register buffers do.  CTA b walks tuples
+// [b*M, (b+1)*M) of the index file, staged into shared memory kReplayChunk trees at a time outside the timed region, and
+// the launch asks for the plan's dynamic shared memory, so the L1 keeps the share of the SM's 256 KiB the walk leaves it.
+// L1P: 0 = L1::no_allocate, 1 = L1::evict_normal, 2 = L1::evict_last, -1 = no load (the loop's own cost: index reads,
+// lane-pair swap, barrier).  L2H: the loads carry the L2::evict_last cache policy, made per load as the walk makes it.
+constexpr uint32_t kReplayChunk = 512;
+
+#define REPLAY_LDG(Q)                                                                                                   \
+    if constexpr (L2H) {                                                                                                \
+        uint64_t pol;                                                                                                   \
+        asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));                                \
+        asm volatile("ld.global.nc" Q ".L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"                                 \
+                     : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p), "l"(pol));                                   \
+    } else {                                                                                                            \
+        asm volatile("ld.global.nc" Q ".v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p)); \
+    }
+template <int L1P, bool L2H>
+__device__ __forceinline__ uint4 replay_ldg(const uint4* p) {
+    uint4 v = make_uint4((uint32_t)(uintptr_t)p, 0u, 0u, 0u);
+    if constexpr (L1P == 0) { REPLAY_LDG(".L1::no_allocate") }
+    else if constexpr (L1P == 1) { REPLAY_LDG(".L1::evict_normal") }
+    else if constexpr (L1P == 2) { REPLAY_LDG(".L1::evict_last") }
+    return v;
+}
+#undef REPLAY_LDG
+
+template <int L1P, bool L2H>
+__global__ void __launch_bounds__(384, 1) replay_kernel(const uint4* bottom, const uint16_t* idx, uint32_t T, uint32_t N,
+                                                        uint32_t nb, int passes, unsigned long long* sink,
+                                                        unsigned long long* cycles) {
+    extern __shared__ __align__(16) unsigned char replay_smem[];
+    uint16_t* sidx = reinterpret_cast<uint16_t*>(replay_smem);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31, half = lane & 1u;
+    const uint32_t M = blockDim.x / 2;                   // two warps of 32 lanes per 32-tuple group
+    const uint32_t sub = warp & 1u, col = (warp >> 1) * 32u + lane;
+    const size_t m0 = (size_t)blockIdx.x * M;
+    uint32_t acc = 0;
+    unsigned long long cyc = 0;
+    for (int it = 0; it < passes; ++it) {
+        for (uint32_t c0 = 0; c0 < T; c0 += kReplayChunk) {
+            __syncthreads();
+            for (uint32_t i = threadIdx.x; i < kReplayChunk * M; i += blockDim.x) sidx[i] = idx[(size_t)(c0 + i / M) * N + m0 + i % M];
+            __syncthreads();
+            const long long t0 = clock64();
+            uint4 ra[8], rb[8];
+            auto issue = [&](uint32_t q, uint4 (&r)[8]) {
+#pragma unroll
+                for (uint32_t k = 0; k < 4; ++k) {
+                    const uint32_t t = 8u * q + 4u * sub + k;
+                    const uint32_t j = sidx[t * M + col], jp = __shfl_xor_sync(0xFFFFFFFFu, j, 1);
+                    const uint4* recs = bottom + 2ull * (c0 + t) * nb;
+                    r[2 * k] = replay_ldg<L1P, L2H>(recs + 2 * (half ? jp : j) + half);
+                    r[2 * k + 1] = replay_ldg<L1P, L2H>(recs + 2 * (half ? j : jp) + half);
+                }
+            };
+            auto consume = [&](const uint4 (&r)[8]) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) acc += r[k].x ^ r[k].y ^ r[k].z ^ r[k].w;   // every word: 128-bit loads stay 128-bit
+            };
+            constexpr uint32_t steps = kReplayChunk / 8;
+            issue(0, ra);
+            for (uint32_t q = 1; q < steps; q += 2) {
+                __syncthreads();
+                issue(q, rb);
+                consume(ra);
+                __syncthreads();
+                if (q + 1 < steps) issue(q + 1, ra);
+                consume(rb);
+            }
+            cyc += (unsigned long long)(clock64() - t0);
+        }
+    }
+    if (acc == 0x12345678u) sink[0] = acc;
+    if (threadIdx.x == 0) cycles[blockIdx.x] = cyc;
+}
+
+// cycles per warp-gather (one warp's paired gather of one tree: two 128-bit loads) per SM, one CTA of `warps` warps per SM
+template <int L1P, bool L2H>
+double replay(const uint4* bottom, const uint16_t* idx, uint32_t T, uint32_t N, uint32_t nb, int warps, size_t smem,
+              unsigned long long* sink, unsigned long long* cyc) {
+    const int passes = 40;
+    cudaFuncSetAttribute(replay_kernel<L1P, L2H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    replay_kernel<L1P, L2H><<<g_sms, 32 * warps, smem>>>(bottom, idx, T, N, nb, 1, sink, cyc);          // warm-up
+    replay_kernel<L1P, L2H><<<g_sms, 32 * warps, smem>>>(bottom, idx, T, N, nb, passes, sink, cyc);
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1.0;
+    std::vector<unsigned long long> h(g_sms);
+    cudaMemcpy(h.data(), cyc, g_sms * 8, cudaMemcpyDeviceToHost);
+    double m = 0;
+    for (auto v : h) m += (double)v;
+    return m / g_sms / ((double)passes * T / 8 * warps * 4);
+}
+
+static void replay_row(const char* name, const uint4* bottom, const uint16_t* idx, uint32_t T, uint32_t N, uint32_t nb,
+                       int warps, size_t smem, unsigned long long* sink, unsigned long long* cyc, bool last) {
+    printf(" \"%s\": {\"warps\": %d, \"dynamic_smem\": %zu, \"no_load\": %.2f,\n", name, warps, smem,
+           replay<-1, false>(bottom, idx, T, N, nb, warps, smem, sink, cyc));
+    printf("   \"no_allocate\": %.2f, \"evict_normal\": %.2f, \"evict_last\": %.2f,\n",
+           replay<0, false>(bottom, idx, T, N, nb, warps, smem, sink, cyc), replay<1, false>(bottom, idx, T, N, nb, warps, smem, sink, cyc),
+           replay<2, false>(bottom, idx, T, N, nb, warps, smem, sink, cyc));
+    printf("   \"no_allocate+L2_evict_last\": %.2f, \"evict_normal+L2_evict_last\": %.2f, \"evict_last+L2_evict_last\": %.2f}%s\n",
+           replay<0, true>(bottom, idx, T, N, nb, warps, smem, sink, cyc), replay<1, true>(bottom, idx, T, N, nb, warps, smem, sink, cyc),
+           replay<2, true>(bottom, idx, T, N, nb, warps, smem, sink, cyc), last ? "" : ",");
+}
+
+// --replay FILE: the cfg3 record stream of tools/gather_paths.py against uniformly random records of the same shape,
+// with the cfg3 plan's 5 tuple groups (231,552 B of shared memory) and with 4 (DTE_TUNE=warps=8: 198,784 B)
+static int run_replay(const char* path) {
+    FILE* f = fopen(path, "rb");
+    uint32_t hdr[4] = {0, 0, 0, 0};
+    if (!f || fread(hdr, 4, 4, f) != 4 || hdr[0] != 0x47455444u) { fprintf(stderr, "%s: not a gather_paths.py file\n", path); return 2; }
+    const uint32_t T = hdr[1], N = hdr[2], nb = hdr[3];
+    if (T % kReplayChunk || N < (uint32_t)g_sms * 160u || nb > 65536u) { fprintf(stderr, "%s: unsupported shape\n", path); return 2; }
+    std::vector<uint16_t> stream((size_t)T * N), uniform((size_t)T * N);
+    if (fread(stream.data(), 2, stream.size(), f) != stream.size()) { fprintf(stderr, "%s: truncated\n", path); return 2; }
+    fclose(f);
+    std::mt19937 rng(0x6A7E);
+    for (auto& j : uniform) j = (uint16_t)(rng() % nb);
+    unsigned long long *sink, *cyc;
+    uint4* bottom;
+    uint16_t *d_stream, *d_uniform;
+    const size_t bbytes = (size_t)T * nb * 32;
+    cudaMalloc(&sink, 8); cudaMalloc(&cyc, g_sms * 8); cudaMalloc(&bottom, bbytes);
+    cudaMalloc(&d_stream, stream.size() * 2); cudaMalloc(&d_uniform, uniform.size() * 2);
+    cudaMemset(bottom, 1, bbytes);
+    cudaMemcpy(d_stream, stream.data(), stream.size() * 2, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_uniform, uniform.data(), uniform.size() * 2, cudaMemcpyHostToDevice);
+    cudaDeviceProp prop;
+    cudaGetDeviceProperties(&prop, 0);
+    printf("{\"what\": \"cycles per warp-gather per SM: one warp's paired gather of one tree's 32-byte bottom records "
+           "(two 128-bit loads), in the cfg3 plan's order, one CTA per SM\", \"device\": \"%s\", \"sms\": %d, "
+           "\"trees\": %u, \"records_per_tree\": %u,\n", prop.name, g_sms, T, nb);
+    replay_row("uniform_5_groups", bottom, d_uniform, T, N, nb, 10, 231552, sink, cyc, false);
+    replay_row("cfg3_stream_5_groups", bottom, d_stream, T, N, nb, 10, 231552, sink, cyc, false);
+    replay_row("cfg3_stream_4_groups", bottom, d_stream, T, N, nb, 8, 198784, sink, cyc, true);
+    printf("}\n");
+    return cudaGetLastError() == cudaSuccess ? 0 : 1;
+}
+
+int main(int argc, char** argv) {
     unsigned long long *sink, *cyc;
     uint4* g;
     const size_t gbytes = 32ull << 20;               // 32 MiB: L2-resident like the bottom records of cfg3
     if (cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0) != cudaSuccess) return 1;
+    if (argc == 3 && !strcmp(argv[1], "--replay")) return run_replay(argv[2]);
     cudaMalloc(&sink, 8); cudaMalloc(&cyc, g_sms * 8); cudaMalloc(&g, gbytes);
     cudaMemset(g, 1, gbytes);
     const uint32_t gmask = (uint32_t)(gbytes / 32 - 1);
