@@ -84,6 +84,7 @@ struct EnsembleShape {
     uint32_t C = 1;                   // classes: tree t of the stream belongs to class t % C
     uint32_t gpc = 0;                 // tree8 groups per class (C >= 2: Tpad = C * gpc * 8)
     uint32_t cls_max = 0;             // trees of the largest class (C = 1: T)
+    uint32_t first = 0;               // global stream index of local tree 0 (its class is first % C)
 };
 
 // The ensemble in the device layout, still in host memory (built once, uploaded to one or many devices).
@@ -95,12 +96,17 @@ struct EnsembleShape {
 //   binned layout (DESIGN.md §9), built only when pack_ensemble is given the edge table:
 //   top_b[t][2^(D-2)]     4-byte heap records rank | fidx << 8 | missing_right << 20
 //   bottom_b              the bottom records with the rank of each node in its threshold word
+//   leaf-id layout (DESIGN.md §10), built only when pack_ensemble is asked for it:
+//   bottom_id             the bottom records with, in each leaf word, the stream cell index (in the tree's own heap
+//                         W[0 .. 2^(D+1)-2]) whose word the score walk adds: an expanded early leaf's cell in every slot
+//                         below it, cells 1, 1, 2, 2 for D = 1
 struct PackedEnsemble {
     EnsembleShape shape;
     std::vector<uint2> top;
     std::vector<uint4> bottom;
     std::vector<uint32_t> top_b;
     std::vector<uint4> bottom_b;
+    std::vector<uint4> bottom_id;
 };
 
 // Per-feature edge table of the binned layout: feature f's distinct live threshold words, sorted as int32, are
@@ -172,11 +178,11 @@ inline int bin_edges(const Geom& g, const unsigned char* wl, size_t n_wl, const 
 // Packs trees [first, first + count) of the streams; `first` is the global stream index of the first packed tree, so
 // with `classes` = C >= 2 tree first + t belongs to class (first + t) % C.  The trees are then stored class-major:
 // class c occupies tree slots [c * gpc * 8, (c + 1) * gpc * 8) in stream order, gpc = ceil(largest class / 8).
-// With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well.
-// Returns 0 or a negative dte_status; *msg receives the reason.
+// With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well, and with `leaf` the
+// leaf-id layout.  Returns 0 or a negative dte_status; *msg receives the reason.
 inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl,
                          uint32_t first, uint32_t count, uint32_t classes, PackedEnsemble& out, std::string& msg,
-                         const BinEdges* bins = nullptr) {
+                         const BinEdges* bins = nullptr, bool leaf = false) {
     char buf[256];
     if (classes < 1) { msg = "class count 0"; return -1; }
     if (n_wl % g.w_cls) {
@@ -242,14 +248,17 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     const bool wide = max_f >= 512;
     const uint32_t BV = wide ? 4 : 2;
 
-    out.shape = {g, count, Tpad, Dtop, top_stride, nb, wide, classes, gpc, cls_max};
+    out.shape = {g, count, Tpad, Dtop, top_stride, nb, wide, classes, gpc, cls_max, first};
     out.top.assign((size_t)Tpad * top_stride, make_uint2(0u, 8u << 16));
     out.bottom.assign((size_t)Tpad * nb * BV, make_uint4(0, 0, 0, 0));
     out.top_b.assign(bins ? (size_t)Tpad * top_stride : 0, 0u);
     out.bottom_b.assign(bins ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
+    out.bottom_id.assign(leaf ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
     std::vector<uint32_t> Wk((2u << Dk) - 1);
     std::vector<uint16_t> Fk((1u << Dk) - 1);
+    std::vector<uint32_t> cell((2u << Dk) - 1);        // stream cell each cell of the packed heap stands for
     for (uint32_t t = 0; t < count; ++t) {
+        for (uint32_t i = 0; i < cell.size(); ++i) cell[i] = i;
         const uint32_t* W = Wall + (size_t)(first + t) * wstride;
         const uint16_t* FI = Fall + (size_t)(first + t) * fstride;
         if (D == 1) {
@@ -258,6 +267,7 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
             Wk[0] = W[0]; Wk[1] = 0; Wk[2] = 0;
             Wk[3] = W[1]; Wk[4] = W[1]; Wk[5] = W[2]; Wk[6] = W[2];
             Fk[0] = FI[0]; Fk[1] = 0; Fk[2] = 0;
+            cell[3] = cell[4] = 1; cell[5] = cell[6] = 2;
         } else {
             std::copy(W, W + ((2u << D) - 1), Wk.begin());
             std::copy(FI, FI + ((1u << D) - 1), Fk.begin());
@@ -271,6 +281,7 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                     if (konst[i]) {                       // inside a constant subtree: value travels in Wk[i]
                         const uint32_t v = Wk[i];
                         Wk[l] = v; Wk[r] = v;
+                        cell[l] = cell[r] = cell[i];
                         if (r < n_int) konst[l] = konst[r] = 1;
                         Wk[i] = 0; Fk[i] = 0;             // any threshold / feature 0: both ways lead to v
                     } else if ((Fk[i] & 0x4000u) && r < n_int) {
@@ -302,6 +313,14 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                 bp[j * 2 + 1] = leaves;
             }
         }
+        if (leaf) {
+            uint4* bi = out.bottom_id.data() + (size_t)slot_of[t] * nb * BV;
+            std::copy(bp, bp + (size_t)nb * BV, bi);
+            for (uint32_t j = 0; j < nb; ++j) {
+                const uint32_t n = nb - 1 + j, l = 2 * n + 1, r = 2 * n + 2;
+                bi[j * BV + (wide ? 2 : 1)] = make_uint4(cell[2 * l + 1], cell[2 * l + 2], cell[2 * r + 1], cell[2 * r + 2]);
+            }
+        }
         if (bins) {
             // Don't-care nodes (the dummy level of D = 1, the constant nodes of an expanded early leaf) store rank 0:
             // both children hold the same value, so the direction does not matter.  Every other node is a live node of
@@ -330,6 +349,7 @@ struct Slot {
     float* d_sc = nullptr;        // final scores of this slot (single / data-sharded / host node of a group)
     float* d_part = nullptr;      // group (ensemble-sharded) mode: this device's partial scores
     uint8_t* d_lb = nullptr;
+    uint16_t* d_leaf = nullptr;   // leaf calls: [cap][T] cells of this slot (allocated by the first leaf call)
     size_t fill = 0;              // bytes of tuple stream landed (or enqueued to land) in d_tup
     size_t walked = 0;            // whole tuples already submitted to the walk kernel
     cudaEvent_t ev_walk = nullptr;   // last walk reading d_tup / writing d_sc, d_part
@@ -359,6 +379,8 @@ struct Dev {
     uint4* d_bottom_b = nullptr;
     uint32_t* d_bin_off = nullptr;
     uint32_t* d_bin_edges = nullptr;
+    // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
+    uint4* d_bottom_id = nullptr;
     bool run_bin = false;             // the landing slots carry u8 bins (F bytes per tuple) during dte_infer_host_binned
     size_t run_tuple_bytes() const { return run_bin ? shape.g.F() : shape.g.tuple_bytes(); }
 
@@ -372,6 +394,12 @@ struct Dev {
     // result sink of the next submitted tuples: direct host pointers (fast path) or the pinned ring (line stream)
     float* sink_sc = nullptr;
     uint8_t* sink_lb = nullptr;
+    // leaf calls (dte_infer_host_leaves): the walk writes cells into Slot::d_leaf and its rows land in sink_leaf, whose
+    // rows are leaf_pitch cells apart (this device's columns of the caller's rows)
+    bool run_leaf = false;
+    uint16_t* sink_leaf = nullptr;
+    size_t leaf_pitch = 0;
+    size_t leaf_slot_cells = 0;       // cells allocated per Slot::d_leaf
     float* h_ring = nullptr;          // pinned, device-local tuple order
     size_t ring_cap = 0;              // tuples
     uint64_t res_enq = 0;             // result tuples whose D2H has been enqueued (device-local count)
@@ -559,10 +587,81 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     return rc;
 }
 
-// bin: the binned walk's plan, named dt_walk_generic_u8 / dt_walk_tile_u8
-inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len, bool bin = false) {
+using LeafKernel = void (*)(LeafParams);
+// The leaf walk of family R with the given WIDE flag and thread bound nt
+template <int R, bool WIDE>
+LeafKernel tile_leaf_kernel(int nt) {
+    constexpr TileFamily f = kTileFamilies[R];
+    return nt == f.nt ? dt_walk_tile_leaf<f.ilp, f.pair, f.staged, WIDE, f.nt>
+                      : dt_walk_tile_leaf<f.ilp, f.pair, f.staged, WIDE, std::min(f.nt, 384)>;
+}
+// [row][WIDE]: every leaf tile kernel, one entry per row of kTileFamilies
+template <size_t... R>
+constexpr auto tile_leaf_kernel_table(std::index_sequence<R...>) {
+    using Pick = LeafKernel (*)(int);
+    return std::array<std::array<Pick, 2>, sizeof...(R)>{{{tile_leaf_kernel<R, false>, tile_leaf_kernel<R, true>}...}};
+}
+inline constexpr auto kTileLeafKernels = tile_leaf_kernel_table(std::make_index_sequence<kNumTileFamilies>());
+inline constexpr LeafKernel kGenericLeafKernels[2] = {dt_walk_generic_leaf<false>, dt_walk_generic_leaf<true>};
+
+// Launch the leaf walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident leaf-id layout:
+// d_leaves[i][t] for the shape.T local trees.  The plan is the fp32 walk's plan of the same ensemble; every tree slot is
+// walked whatever K and S say.  Returns a cudaError_t.
+inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, int want_variant, const void* d_tuples, size_t n,
+                                    uint16_t* d_leaves, cudaStream_t st, const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const Plan pl = make_plan(d, tune, want_variant);
+    LeafParams lp = {};
+    WalkParams& wp = lp.w;
+    wp.top = d.d_top;
+    wp.bottom = d.d_bottom_id;
+    wp.tuples = static_cast<const float*>(d_tuples);
+    wp.n = n;
+    wp.F = d.shape.g.F();
+    wp.Dtop = d.shape.Dtop;
+    wp.top_stride = d.shape.top_stride;
+    wp.nb = d.shape.nb;
+    wp.groups = d.shape.Tpad / 8;
+    wp.K = 1;
+    wp.missing = run.missing;
+    wp.nwarps = (uint32_t)pl.nwarps;
+    wp.nstages = (uint32_t)pl.nstages;
+    wp.fill_split = tune.fill ? 1u : 0u;
+    wp.Lw = phased_level(d, tune, pl);
+    wp.classes = d.shape.C;
+    wp.groups_per_class = d.shape.gpc;
+    lp.leaves = d_leaves;
+    lp.T = d.shape.T;
+    lp.first = d.shape.first % d.shape.C;
+    cudaError_t rc;
+    if (pl.row < 0) {
+        const int threads = 128;
+        const unsigned long long blocks = (n + threads - 1) / threads;
+        if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+        kGenericLeafKernels[pl.wide]<<<(unsigned)blocks, threads, 0, st>>>(lp);
+        rc = cudaGetLastError();
+    } else {
+        const size_t M = pl.tuples_per_cta();
+        const unsigned long long tiles = (n + M - 1) / M;
+        if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+        wp.tiles = (uint32_t)tiles;
+        const int grid = (int)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count);
+        const LeafKernel k = kTileLeafKernels[pl.row][pl.wide](pl.thread_bound());
+        rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+        if (rc != cudaSuccess) return rc;
+        k<<<grid, pl.threads(), pl.smem, st>>>(lp);
+        rc = cudaGetLastError();
+    }
+    if (rc == cudaSuccess) d.kernel_launches++;
+    return rc;
+}
+
+// bin: the binned walk's plan, named dt_walk_generic_u8 / dt_walk_tile_u8.  leaf: the leaf walk's plan (the fp32 plan),
+// named dt_walk_generic_leaf / dt_walk_tile_leaf
+inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len, bool bin = false, bool leaf = false) {
     const Plan pl = make_plan(d, tune, want, bin);
-    const char* sfx = bin ? "_u8" : "";
+    const char* sfx = bin ? "_u8" : leaf ? "_leaf" : "";
     if (pl.row < 0) {
         snprintf(buf, len, "dt_walk_generic%s<%d>", sfx, pl.wide ? 1 : 0);
     } else {

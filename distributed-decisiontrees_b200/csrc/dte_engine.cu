@@ -85,6 +85,7 @@ struct dte_engine {
     uint32_t cycle_mhz = 0;
     int combine_nccl = 0;
     size_t opt_queue_lines = 0, opt_chunk_tuples = 0;
+    bool opt_leaf = false;            // DTE_OPT_LEAF_LAYOUT: placements also build the leaf-id layout
 
     // ---- stream state (PCIeReceiver.sv FSM) ----
     enum { ST_IDLE = 0, ST_TREES = 1, ST_WAIT = 2, ST_DATA = 3 } state = ST_IDLE;
@@ -270,8 +271,9 @@ int decide_partition(dte_engine* e, const Geom& g) {
 
 // A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
 // layout and the validated feature-index range; K, S and the missing pattern are free to change).  bin: the run walks
-// u8 bins and needs the binned layout as well.
-int check_resident(dte_engine* e, const Geom& g, bool bin = false) {
+// u8 bins and needs the binned layout as well.  leaf: the run is a leaf walk, which needs the leaf-id layout and walks
+// every tree whatever K and S say.
+int check_resident(dte_engine* e, const Geom& g, bool bin = false, bool leaf = false) {
     if (e->multi() && e->placed) {
         if (e->part != *e->placed)
             return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
@@ -282,11 +284,13 @@ int check_resident(dte_engine* e, const Geom& g, bool bin = false) {
     for (Dev& d : e->devs) {
         if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
         if (bin && !d.d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
+        if (leaf && !d.d_bottom_id)
+            return fail(e, DTE_ERR_STATE, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1");
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
                         g.F(), g.D, d.shape.g.F(), d.shape.g.D);
         // a multi-class walk covers every tree: the slots must hold the largest class (no silent truncation per class)
-        if (d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
+        if (!leaf && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
             return fail(e, DTE_ERR_CONFIG, "reg 205: S=%u x K=%u x 8 slots hold fewer trees than the largest of the %u classes (%u trees): "
                         "a multi-class run needs S >= %u", g.S, g.K, d.shape.C, d.shape.cls_max, (d.shape.cls_max + 8 * g.K - 1) / (8 * g.K));
     }
@@ -299,8 +303,10 @@ uint32_t classes_of(const dte_engine* e) { return host_dev(e).shape.C; }
 // ---- placement of the ensemble on the devices ---------------------------------------------------------
 void free_ensemble(Dev& d) {
     cudaSetDevice(d.ordinal);
-    for (void* p : {(void*)d.d_top, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges})
+    for (void* p : {(void*)d.d_top, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges,
+                    (void*)d.d_bottom_id})
         if (p) cudaFree(p);
+    d.d_bottom_id = nullptr;
     d.d_top = nullptr;
     d.d_bottom = nullptr;
     d.d_top_b = nullptr;
@@ -333,6 +339,10 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
         TRY(upload(e, d.d_bin_edges, bins->edges));
         d.ensemble_bytes += pk.top_b.size() * sizeof(uint32_t) + pk.bottom_b.size() * sizeof(uint4);
     }
+    if (!pk.bottom_id.empty()) {
+        TRY(upload(e, d.d_bottom_id, pk.bottom_id));
+        d.ensemble_bytes += pk.bottom_id.size() * sizeof(uint4);
+    }
     return DTE_OK;
 }
 
@@ -347,7 +357,8 @@ struct TreeShare {
 // partition packs share[0] once and replicates it.  Records the placement for check_resident.  `classes` >= 2: every
 // share is packed class-major, the class of a tree taken from its global stream index (share.first counts from the
 // start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
-// binned layout is dropped.
+// binned layout is dropped.  With DTE_OPT_LEAF_LAYOUT the leaf-id layout is built and uploaded too; without it any
+// resident leaf-id layout is dropped.
 int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr) {
     const bool chunked = e->part == Part::Chunked;
     PackedEnsemble pk;
@@ -355,7 +366,7 @@ int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_
         if (chunked || r == 0) {
             const TreeShare& s = share[r];
             std::string msg;
-            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg, bins);
+            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg, bins, e->opt_leaf);
             if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
         }
         TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins));
@@ -390,11 +401,29 @@ void free_slots(Dev& d) {
         if (s.d_sc) cudaFree(s.d_sc);
         if (s.d_part) cudaFree(s.d_part);
         if (s.d_lb) cudaFree(s.d_lb);
-        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr;
+        if (s.d_leaf) cudaFree(s.d_leaf);
+        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_leaf = nullptr;
         s.fill = s.walked = 0;
     }
     d.cap_tuples = 0;
     d.slot_parts = false;
+    d.leaf_slot_cells = 0;
+}
+
+// leaf calls: Slot::d_leaf of [cap][T] cells on every slot (score runs never allocate them)
+int ensure_leaf_slots(dte_engine* e, Dev& d) {
+    const size_t cells = d.cap_tuples * d.shape.T;
+    if (d.leaf_slot_cells >= cells) return DTE_OK;
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    CUDA_TRY(e, cudaDeviceSynchronize());
+    for (Slot& s : d.slot) {
+        if (s.d_leaf) cudaFree(s.d_leaf);
+        s.d_leaf = nullptr;
+    }
+    d.leaf_slot_cells = 0;
+    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_leaf, cells * sizeof(uint16_t)));
+    d.leaf_slot_cells = cells;
+    return DTE_OK;
 }
 
 // `C` score words per tuple: d_sc / d_part hold [cap][C] fp32 (C >= 2 for a multi-class ensemble)
@@ -488,6 +517,28 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
     return DTE_OK;
 }
 
+// D2H of the cells of `cnt` tuples of slot s starting at slot-local tuple `from` into the device's leaf sink: rows of
+// shape.T cells, leaf_pitch cells apart on the host.
+int enqueue_leaves(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt) {
+    const size_t T = d.shape.T;
+    CUDA_TRY(e, cudaStreamWaitEvent(d.s_d2h, s.ev_walk, 0));
+    CUDA_TRY(e, cudaMemcpy2DAsync(d.sink_leaf, d.leaf_pitch * 2, s.d_leaf + from * T, T * 2, T * 2, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
+    d.sink_leaf += cnt * d.leaf_pitch;
+    CUDA_TRY(e, cudaEventRecord(s.ev_d2h, d.s_d2h));
+    cudaEvent_t ev = get_event(d);
+    CUDA_TRY(e, cudaEventRecord(ev, d.s_d2h));
+    d.res_enq += cnt;
+    d.pend.push_back({ev, d.res_enq});
+    return DTE_OK;
+}
+
+int leaf_walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, uint16_t* leaves, cudaStream_t st) {
+    const char* why = nullptr;
+    const cudaError_t rc = launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, leaves, st, &why);
+    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "leaf walk launch failed: %s", why ? why : cudaGetErrorString(rc));
+    return DTE_OK;
+}
+
 // Launch the walk of n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.
 // bin: `tuples` are u8 bins walked against the binned layout.
 int walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, float* scores, uint8_t* labels, cudaStream_t st,
@@ -511,6 +562,14 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaEventRecord(s.ev_land, d.s_h2d));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // score buffer of this slot drained
+    if (d.run_leaf) {
+        TRY(leaf_walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_leaf + s.walked * d.shape.T, d.s_main));
+        CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
+        TRY(enqueue_leaves(e, d, s, s.walked, cnt));
+        s.walked = whole;
+        e->tuples_out += cnt;
+        return DTE_OK;
+    }
     const bool labels = d.sink_sc && d.sink_lb;
     TRY(walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked * d.slot_C, labels ? s.d_lb + s.walked : nullptr, d.s_main, false, d.run_bin));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
@@ -670,6 +729,21 @@ int submit_group(dte_engine* e, int b) {
     for (Dev& d : e->devs) {
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         CUDA_TRY(e, cudaEventRecord(d.slot[b].ev_land, d.s_h2d));
+    }
+    if (h.run_leaf) {
+        // every ring position walks every tuple for its own trees and lands its block in its columns: no combine
+        for (Dev& d : e->devs) {
+            Slot& s = d.slot[b];
+            CUDA_TRY(e, cudaSetDevice(d.ordinal));
+            for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));
+            CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));
+            TRY(leaf_walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_leaf + walked * d.shape.T, d.s_main));
+            CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
+            TRY(enqueue_leaves(e, d, s, walked, cnt));
+            s.walked = whole;
+        }
+        e->tuples_out += cnt;
+        return DTE_OK;
     }
     for (Dev& d : e->devs) {
         Slot& s = d.slot[b];
@@ -839,7 +913,8 @@ int prepare_data_phase(dte_engine* e, bool need_ring) {
     return DTE_OK;
 }
 
-int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels);
+int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
+                   uint16_t* h_leaves = nullptr);
 
 // Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
 // score buffer as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every
@@ -869,7 +944,9 @@ int infer_host(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_
 }
 
 // The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.
-int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
+// h_leaves (leaf calls, Dev::run_leaf set): [n][columns] cells, every device's rows landing in its own columns.
+int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
+                   uint16_t* h_leaves) {
     const size_t tb = e->devs[0].run_tuple_bytes();
     std::vector<uint64_t> enq0(e->devs.size());
     for (size_t i = 0; i < e->devs.size(); ++i) {
@@ -883,6 +960,16 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
         Dev& h = host_dev(e);
         h.sink_sc = h_scores;
         h.sink_lb = h_labels;
+        if (h_leaves) {                                  // ring position r owns columns [sum of T before r, + T_r)
+            size_t cols = 0, off = 0;
+            for (const Dev& d : e->devs) cols += d.shape.T;
+            for (size_t r = 0; r < e->devs.size(); ++r) {
+                Dev& d = e->devs[(size_t)e->pos2dev[r]];
+                d.sink_leaf = h_leaves + off;
+                d.leaf_pitch = cols;
+                off += d.shape.T;
+            }
+        }
         rc = land_group(e, h_tuples, n * tb);
         if (!rc) rc = submit_group(e, h.cur);
         for (Dev& d : e->devs)
@@ -897,8 +984,12 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
             size_t i = g;
             for (size_t off = g * chunk; off < n && !r; off += G * chunk, i += G) {
                 const size_t cnt = std::min(chunk, n - off);
-                d.sink_sc = h_scores + off * C;                // scores are [n][C]
+                d.sink_sc = h_scores ? h_scores + off * C : nullptr;      // scores are [n][C]
                 d.sink_lb = h_labels ? h_labels + off : nullptr;
+                if (h_leaves) {
+                    d.sink_leaf = h_leaves + off * d.shape.T;
+                    d.leaf_pitch = d.shape.T;
+                }
                 r = land_dev(e, d, h_tuples + off * tb, cnt * tb);
                 if (!r && d.slot[d.cur].fill) {          // a short last chunk
                     r = submit_dev(e, d, d.cur);
@@ -930,13 +1021,44 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
         cudaSetDevice(d.ordinal);
         if (cudaEventElapsedTime(&ms, d.ev_t0, d.ev_t1) == cudaSuccess) d.last_walk_ms = ms;
         ms_max = std::max(ms_max, ms);
-        d.sink_sc = nullptr; d.sink_lb = nullptr;
+        d.sink_sc = nullptr; d.sink_lb = nullptr; d.sink_leaf = nullptr;
         d.res_enq = d.res_done = enq0[i];            // direct-sink results are not part of the line-stream queue
     }
     e->last_walk_ms = ms_max;
     if (rc || rc2) return rc ? rc : rc2;
     e->tuples_in += n;
     return DTE_OK;
+}
+
+// dte_infer_host_leaves: infer_host's landing pipeline with the leaf walk; no scores, no labels.
+int infer_host_leaves(dte_engine* e, const unsigned char* h_tuples, size_t n, uint16_t* h_leaves) {
+    Geom g;
+    TRY(decode_geom(e, g));
+    if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "infer_host_leaves while the tree stream is being received");
+    if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
+    TRY(drain_all(e));
+    if (e->multi()) TRY(decide_partition(e, g));
+    TRY(check_resident(e, g, false, true));
+    if (n == 0) return DTE_OK;
+    e->g = g;
+    for (Dev& d : e->devs)
+        if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
+    // The landing slots hold default_chunk tuples; their cells (2T bytes per tuple) may take at most twice the tuple
+    // budget, so a many-tree, few-feature ensemble lands fewer tuples per slot instead of allocating GiBs of cells.
+    const uint32_t F = g.F();
+    uint32_t tmax = 1;
+    for (const Dev& d : e->devs) tmax = std::max(tmax, d.shape.T);
+    const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
+    const size_t cap = std::min(default_chunk(e, F), std::max<size_t>(4, budget / (2 * (size_t)tmax)) & ~(size_t)3);
+    for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
+    for (Dev& d : e->devs) TRY(ensure_leaf_slots(e, d));
+    for (Dev& d : e->devs) d.run_leaf = true;
+    const int rc = infer_host_run(e, h_tuples, n, nullptr, nullptr, h_leaves);
+    for (Dev& d : e->devs) {
+        if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
+        d.run_leaf = false;
+    }
+    return rc;
 }
 
 cudaStream_t pick_stream(Dev& d, void* cuda_stream) { return cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : d.s_main; }
@@ -1215,6 +1337,10 @@ int dte_set_option(dte_t* e, int option, uint64_t value) {
             break;
         case DTE_OPT_RESULT_QUEUE_LINES: e->opt_queue_lines = (size_t)value; break;
         case DTE_OPT_CHUNK_TUPLES: e->opt_chunk_tuples = (size_t)value; break;
+        case DTE_OPT_LEAF_LAYOUT:
+            if (value > 1) return fail(e, DTE_ERR_ARG, "DTE_OPT_LEAF_LAYOUT: 0 (scores only) or 1 (also the leaf-id layout)");
+            e->opt_leaf = value != 0;
+            break;
         default: return fail(e, DTE_ERR_ARG, "unknown option %d", option);
     }
     return DTE_OK;
@@ -1577,6 +1703,43 @@ int dte_kernel_name_binned(dte_t* e, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
     if (!e->devs[0].d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
     kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, true);
+    return DTE_OK;
+}
+
+// ---- leaf-index inference (DESIGN.md §10) ----
+int dte_infer_device_leaves(dte_t* e, const void* d_tuples, size_t n, uint16_t* d_leaves, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_leaves))) return DTE_ERR_ARG;
+    // tuple rows are read as 16-byte vectors and the cells of a row go out in stores of up to 16 bytes
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "dte_infer_device_leaves: d_tuples not 16-byte aligned");
+    if (reinterpret_cast<uintptr_t>(d_leaves) & 15u) return fail(e, DTE_ERR_ARG, "dte_infer_device_leaves: d_leaves not 16-byte aligned");
+    TRY(single_only(e, "dte_infer_device_leaves"));
+    Geom g;
+    TRY(decode_geom(e, g));
+    TRY(check_resident(e, g, false, true));
+    Dev& d = e->devs[0];
+    e->g = g;
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    cudaStream_t st = pick_stream(d, cuda_stream);
+    CUDA_TRY(e, cudaEventRecord(d.ev_t0, st));
+    TRY(leaf_walk_or_fail(e, d, d_tuples, n, d_leaves, st));
+    CUDA_TRY(e, cudaEventRecord(d.ev_t1, st));
+    d.timing_pending = true;
+    e->tuples_in += n;
+    e->tuples_out += n;
+    if (!cuda_stream) CUDA_TRY(e, cudaStreamSynchronize(st));
+    return DTE_OK;
+}
+
+int dte_infer_host_leaves(dte_t* e, const void* h_tuples, size_t n, uint16_t* h_leaves) {
+    if (!e || (n && (!h_tuples || !h_leaves))) return DTE_ERR_ARG;
+    return infer_host_leaves(e, static_cast<const unsigned char*>(h_tuples), n, h_leaves);
+}
+
+int dte_kernel_name_leaves(dte_t* e, char* buf, size_t len) {
+    if (!e || !buf || !len) return DTE_ERR_ARG;
+    if (!e->devs[0].d_bottom_id)
+        return fail(e, DTE_ERR_STATE, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1");
+    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, false, true);
     return DTE_OK;
 }
 

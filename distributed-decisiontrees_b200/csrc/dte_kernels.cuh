@@ -65,6 +65,16 @@ struct WalkParams {
     const uint8_t* bins;        // [n][F] row-major
 };
 
+// Parameters of the leaf walks (dt_walk_tile_leaf, dt_walk_generic_leaf; DESIGN.md §10).  A struct of its own: growing
+// WalkParams past its 128 bytes changes the code ptxas emits for the score kernels.
+struct LeafParams {
+    WalkParams w;               // the walk; w.bottom = the leaf-id records (stream cell index in each leaf word),
+                                // w.groups = every tree8 group of every class
+    uint16_t* leaves;           // [n][T] row-major, 16-byte aligned: leaves[i][leaf_column(slot)]
+    uint32_t T;                 // local trees = output columns
+    uint32_t first;             // first_tree % classes of the resident chunk
+};
+
 // ---------------------------------------------------------------------------------------------
 // small PTX helpers
 // ---------------------------------------------------------------------------------------------
@@ -430,6 +440,69 @@ __global__ void __launch_bounds__(128) dt_walk_generic(const WalkParams p) {
             p.scores[i] = tot;
             if (p.labels) p.labels[i] = tot > 0.0f ? 1 : 0;
         }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Leaf walks (DESIGN.md §10): the same walk against the leaf-id records, whose leaf words are the stream cell index of
+// each leaf slot, so bot_finish() returns the cell; no reduction.  Tree slot s is written to column leaf_column(s) of
+// the tuple's row: one class keeps stream order, several classes undo the class-major slot order, and a column >= T is
+// a padding slot, which is not written.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t leaf_column(const LeafParams& lp, uint32_t s) {
+    const WalkParams& p = lp.w;
+    if (p.classes == 1) return s;
+    const uint32_t per = p.groups_per_class * 8u, c = s / per;     // class c, k = s - c * per-th tree of that class
+    return (c + p.classes - lp.first) % p.classes + (s - c * per) * p.classes;
+}
+// leaf-id stores: written once, read by the host or the next kernel, so out of L1 and first out of L2 (the ensemble
+// keeps its evict_last lines, see l2_evict_last)
+__device__ __forceinline__ void stg16_leaf(uint16_t* a, uint32_t v) {
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.u16 [%0], %1, %2;" ::"l"(a), "h"((unsigned short)v), "l"(l2_evict_first())
+                 : "memory");
+}
+// ILP consecutive cells of one row as one 4-, 8- or 16-byte store (a must be aligned to 2 * ILP bytes)
+template <int ILP>
+__device__ __forceinline__ void stg_cells(uint16_t* a, const uint32_t (&c)[ILP]) {
+    if constexpr (ILP == 2) {
+        asm volatile("st.global.L1::no_allocate.L2::cache_hint.u32 [%0], %1, %2;" ::"l"(a), "r"(c[0] | c[1] << 16), "l"(l2_evict_first())
+                     : "memory");
+    } else if constexpr (ILP == 4) {
+        asm volatile("st.global.L1::no_allocate.L2::cache_hint.v2.u32 [%0], {%1, %2}, %3;" ::"l"(a), "r"(c[0] | c[1] << 16),
+                     "r"(c[2] | c[3] << 16), "l"(l2_evict_first()) : "memory");
+    } else {
+        static_assert(ILP == 8, "ILP 2, 4 or 8");
+        asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(a), "r"(c[0] | c[1] << 16),
+                     "r"(c[2] | c[3] << 16), "r"(c[4] | c[5] << 16), "r"(c[6] | c[7] << 16), "l"(l2_evict_first()) : "memory");
+    }
+}
+
+// The generic leaf walk: dt_walk_generic's walk over every resident tree slot, one thread per tuple.
+template <bool WIDE>
+__global__ void __launch_bounds__(128) dt_walk_generic_leaf(const LeafParams lp) {
+    constexpr int BV = WIDE ? 4 : 2;
+    const WalkParams& p = lp.w;
+    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n) return;
+    const uint32_t* x = reinterpret_cast<const uint32_t*>(p.tuples) + i * p.F;
+    auto feat = [&](uint32_t f) -> uint32_t { return __ldg(x + f); };
+    uint16_t* row = lp.leaves + i * lp.T;
+    const uint32_t slots = p.groups * 8u;
+#pragma unroll 1
+    for (uint32_t t = 0; t < slots; ++t) {
+        const uint32_t c = leaf_column(lp, t);
+        if (c >= lp.T) continue;
+        const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
+        uint32_t o = 0;
+        for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+            uint2 nd = ldg64_nc(tp + o);
+            uint32_t xv = feat(nd.y & 0xFFFFu);
+            o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
+        }
+        const uint32_t j = (o >> 3) - (p.nb - 1);
+        BotRec<WIDE> br;
+        bot_load(br, p.bottom + ((size_t)t * p.nb + j) * BV);
+        row[c] = (uint16_t)__float_as_uint(bot_finish<WIDE>(br, p.missing, feat));
     }
 }
 
@@ -1090,6 +1163,245 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_u8(const WalkParams p) {
                 }
             }
         }
+    }
+}
+
+// The leaf tile walk (DESIGN.md §10): dt_walk_tile's producer warp, ring, phased refill, tuple tile and bottom-record
+// pipeline against the leaf-id records (WalkParams::bottom), with the tree8 reduction replaced by the stores of the
+// cells.  Every resident tree slot is walked (p.groups = all groups).  One class with T a multiple of ILP writes each
+// warp's ILP cells of a row as one aligned 2*ILP-byte store; otherwise each cell is a 2-byte store to leaf_column().
+// A separate kernel rather than a flag on dt_walk_tile, for the reason dt_walk_tile_u8 gives.  Shared memory is laid
+// out as dt_walk_tile's (the exchange area is unused), so a leaf plan is the fp32 plan of the same ensemble.
+template <int ILP, int P, bool STAGED, bool WIDE, int NT>
+__global__ void __launch_bounds__(NT, 1) dt_walk_tile_leaf(const LeafParams lp) {
+    static_assert(ILP * P == 8 || ILP * P == 4, "a step covers a tree8 group or half of one");
+    const WalkParams& p = lp.w;
+    constexpr int BV = WIDE ? 4 : 2;
+    constexpr int SP = ILP * P;                         // trees per ring stage / per step
+    extern __shared__ __align__(128) unsigned char smem_raw[];
+    const uint32_t sbase = smem_u32(smem_raw);
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t G = p.nwarps / P;                    // tuple groups per CTA
+    const uint32_t M = 32u * G;
+    const uint32_t tree_bytes = p.top_stride * 8u;
+    const uint32_t stage_bytes = (uint32_t)SP * tree_bytes;
+    const uint32_t ring_bytes = STAGED ? p.nstages * stage_bytes : 0u;
+    const uint32_t xs_base = sbase + kHdrBytes + ring_bytes;
+    const uint32_t row_bytes = M * 4u;
+    const uint32_t steps = p.groups * (8 / SP);         // SP trees per step
+    const uint32_t my_tiles = (p.tiles > blockIdx.x) ? (p.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
+
+    if (STAGED) {
+        if (threadIdx.x == 0) {
+            for (uint32_t s = 0; s < p.nstages; ++s) {
+                mbar_init(sbase + 8 * s, 1);
+                mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);
+                mbar_init(sbase + 8 * (2 * p.nstages + s), 1);
+                mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);
+            }
+            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        }
+        __syncthreads();
+        if (warp == p.nwarps) {
+            // producer: dt_walk_tile's, unchanged
+            if (lane == 0) {
+                const uint64_t total = (uint64_t)my_tiles * steps;
+                const char* src0 = reinterpret_cast<const char*>(p.top);
+                uint32_t slot = 0, par = 1;
+                uint32_t q = 0;
+                const bool phased = p.Lw != 0xFFFFFFFFu;
+                const uint32_t bytesA = phased ? (16u << p.Lw) : tree_bytes;
+                const uint32_t bytesB = tree_bytes - bytesA;
+                for (uint64_t it = 0; it < total; ++it) {
+                    const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
+                    const char* src = src0 + (size_t)q * stage_bytes;
+                    mbar_wait(sbase + 8 * (p.nstages + slot), par);
+                    const uint32_t full = sbase + 8 * slot;
+                    if (!phased) {
+                        mbar_arrive_expect_tx(full, stage_bytes);
+                        if (p.fill_split == 0) {
+                            bulk_g2s(dst, src, stage_bytes, full);
+                        } else {
+#pragma unroll
+                            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
+                        }
+                    } else {
+                        mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
+#pragma unroll
+                        for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
+                        mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
+                        const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
+                        mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
+#pragma unroll
+                        for (int c = 0; c < SP; ++c)
+                            bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
+                    }
+                    if (++q == steps) q = 0;
+                    if (++slot == p.nstages) { slot = 0; par ^= 1; }
+                }
+            }
+            return;
+        }
+    }
+
+    // ---------------- consumers ----------------
+    const uint32_t grp = warp / P, sub = warp % P;
+    const uint32_t col = grp * 32u + lane;
+    const uint32_t xcol = xs_base + col * 4u;
+    auto feat = [&](uint32_t f) { return lds32(xcol + f * row_bytes); };
+    uint32_t slot = 0, par = 0;
+    const bool vec = p.classes == 1 && lp.T % ILP == 0;   // then slot = column and t0 < T covers all ILP cells
+
+    for (uint32_t tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
+        __syncwarp();
+        {
+            const unsigned long long m = (unsigned long long)tile * M + col;
+            const bool live = m < p.n;
+            const uint4* row = reinterpret_cast<const uint4*>(p.tuples + (live ? m : 0ull) * p.F);
+            const uint32_t nvec = p.F >> 2;
+            uint32_t v = 4 * sub;
+            auto put4 = [&](uint32_t a, const uint4& d) {
+                sts32(a, d.x); sts32(a + row_bytes, d.y); sts32(a + 2 * row_bytes, d.z); sts32(a + 3 * row_bytes, d.w);
+            };
+            for (; v + 4 <= nvec; v += 4 * P) {
+                uint4 d0 = ldg128_tuple(row + v), d1 = ldg128_tuple(row + v + 1);
+                uint4 d2 = ldg128_tuple(row + v + 2), d3 = ldg128_tuple(row + v + 3);
+                if (!live) { d0 = d1 = d2 = d3 = make_uint4(0, 0, 0, 0); }
+                const uint32_t a = xcol + (4 * v) * row_bytes;
+                put4(a, d0); put4(a + 4 * row_bytes, d1); put4(a + 8 * row_bytes, d2); put4(a + 12 * row_bytes, d3);
+            }
+            if (sub == 0) {
+                for (v = nvec & ~3u; v < nvec; ++v) {
+                    uint4 d0 = ldg128_tuple(row + v);
+                    if (!live) d0 = make_uint4(0, 0, 0, 0);
+                    put4(xcol + (4 * v) * row_bytes, d0);
+                }
+            }
+        }
+        if (P > 1) group_barrier(1 + grp, 32 * P); else __syncwarp();
+
+        const unsigned long long m = (unsigned long long)tile * M + col;
+        const bool live = m < p.n;
+        uint16_t* const out = lp.leaves + (live ? m : 0ull) * lp.T;
+
+        // resolve the ILP bottom records of step qf into cells and store them (every lane takes part in the swap)
+        auto finish = [&](const BotRec<WIDE> (&rec)[ILP], uint32_t qf) {
+            uint32_t cell[ILP];
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) {
+                BotRec<WIDE> r = rec[c];
+                if constexpr (!WIDE) bot_pair_swap(r);
+                cell[c] = __float_as_uint(bot_finish<WIDE>(r, p.missing, feat));
+            }
+            const uint32_t t0 = qf * SP + sub * ILP;
+            if (!live) return;
+#ifdef DTE_LEAF_STORE_ABLATION
+            // experiment build only (DESIGN.md §10): every cell is computed, but a store is issued only for the cell
+            // 0xFFFF, which no heap of D <= 15 has, so the walk is timed without its output
+            bool keep = false;
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) keep |= cell[c] == 0xFFFFu;
+            if (!keep) return;
+#endif
+            if (vec) {
+                if (t0 < lp.T) stg_cells<ILP>(out + t0, cell);
+            } else {
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) {
+                    const uint32_t oc = leaf_column(lp, t0 + c);
+                    if (oc < lp.T) stg16_leaf(out + oc, cell[c]);
+                }
+            }
+        };
+
+        // dt_walk_tile's walk_top, unchanged
+        auto walk_top = [&](uint32_t q, BotRec<WIDE> (&dst)[ILP]) {
+            const uint32_t t0 = q * SP + sub * ILP;
+            uint32_t o[ILP];
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) o[c] = 0;
+            if (STAGED) {
+                mbar_wait(sbase + 8 * slot, par);
+                const uint32_t tb = sbase + kHdrBytes + slot * stage_bytes + sub * ILP * tree_bytes;
+                uint32_t A[ILP], kb8[ILP];
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) { A[c] = tb + c * tree_bytes; kb8[c] = 8u - A[c]; }
+                constexpr int H = ILP / 2;
+                uint2 nd[ILP];
+                uint32_t xv[ILP];
+                auto S1 = [&](int c) { nd[c] = lds64(A[c]); };
+                auto S2 = [&](int c) { xv[c] = feat(nd[c].y & 0xFFFFu); };
+                auto S3 = [&](int c) {
+                    const uint32_t a2 = A[c] + A[c] + kb8[c];
+                    A[c] = step_select(xv[c], nd[c].x, nd[c].y, p.missing, a2, a2 + 8u);
+                };
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) S1(c);
+#pragma unroll
+                for (int c = 0; c < H; ++c) S2(c);
+                const bool phased = p.Lw != 0xFFFFFFFFu;
+                for (uint32_t lvl = 0; lvl + 1 < p.Dtop; ++lvl) {
+                    if (phased && lvl == p.Lw) mbar_wait(sbase + 8 * (2 * p.nstages + slot), par);
+#pragma unroll
+                    for (int k = 0; k < H; ++k) { S3(k); S1(k); S2(k + H); }
+#pragma unroll
+                    for (int k = H; k < ILP; ++k) { S3(k); S1(k); S2(k - H); }
+                }
+                if (phased) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(sbase + 8 * (p.nstages + slot));
+                }
+#pragma unroll
+                for (int k = 0; k < H; ++k) { S3(k); S2(k + H); }
+#pragma unroll
+                for (int k = H; k < ILP; ++k) S3(k);
+#pragma unroll
+                for (int c = 0; c < ILP; ++c) o[c] = A[c] - (tb + c * tree_bytes);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(sbase + 8 * ((phased ? 3 * p.nstages : p.nstages) + slot));
+                if (++slot == p.nstages) { slot = 0; par ^= 1; }
+            } else {
+                const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t0 * p.top_stride);
+                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+                    uint2 nd[ILP];
+                    uint32_t xv[ILP];
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c) nd[c] = ldg64_nc(tp + (size_t)c * tree_bytes + o[c]);
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c) xv[c] = feat(nd[c].y & 0xFFFFu);
+#pragma unroll
+                    for (int c = 0; c < ILP; ++c) o[c] = 2 * o[c] + step_inc(xv[c], nd[c].x, nd[c].y, p.missing);
+                }
+            }
+#pragma unroll
+            for (int c = 0; c < ILP; ++c) {
+                const uint32_t j = (o[c] >> 3) - (p.nb - 1);
+                if constexpr (WIDE) bot_load_tile(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
+                else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
+            }
+        };
+
+        BotRec<WIDE> recA[ILP], recB[ILP];
+        if (steps > 0) {
+            walk_top(0, recA);
+            uint32_t q = 1;
+            for (; q + 1 < steps; q += 2) {
+                walk_top(q, recB);
+                finish(recA, q - 1);
+                walk_top(q + 1, recA);
+                finish(recB, q);
+            }
+            if (q < steps) {
+                walk_top(q, recB);
+                finish(recA, q - 1);
+                finish(recB, q);
+            } else {
+                finish(recA, q - 1);
+            }
+        }
+        // dt_walk_tile's half-sum exchange keeps the P warps of a group in step; here the group waits explicitly
+        // before the next tile overwrites the columns its partner warps may still read
+        if (P > 1) group_barrier(1 + grp, 32 * P);
     }
 }
 

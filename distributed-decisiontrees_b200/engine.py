@@ -63,6 +63,9 @@ ABI = [
     ("dte_infer_device_binned", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_binned", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_kernel_name_binned", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_infer_device_leaves", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_leaves", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_kernel_name_leaves", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
 ]
 
 
@@ -78,6 +81,7 @@ class DteInfo(C.Structure):
 
 
 DTE_OPT_CYCLE_MHZ, DTE_OPT_COMBINE, DTE_OPT_RESULT_QUEUE_LINES, DTE_OPT_CHUNK_TUPLES = 1, 2, 3, 4
+DTE_OPT_LEAF_LAYOUT = 5
 DTE_ERR_BACKPRESSURE = -7
 CUDA_STREAM_LEGACY = 0x1        # cudaStreamLegacy: the handle value that NAMES the legacy default stream
 
@@ -245,6 +249,8 @@ class Engine:
 
     def set_option(self, option, value):
         self._check(self._lib.dte_set_option(self._h, int(option), int(value)))
+        if int(option) == DTE_OPT_LEAF_LAYOUT:
+            self._leaf_opt = int(value)
 
     def ring_combine_device(self, d_parts, n, d_out, d_labels=None, stream=None):
         """out = (((p0 + p1) + p2) + ...) in ring order, one kernel; d_parts may be peer-GPU buffers."""
@@ -268,14 +274,23 @@ class Engine:
         return bool(d.value)
 
     # -- fast paths -----------------------------------------------------------------------------
-    def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False):
+    def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False,
+                      leaves=False):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
         call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
         binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
-        feature), which the *_binned calls walk with u8 tuples."""
+        feature), which the *_binned calls walk with u8 tuples.
+        leaves=True: DTE_OPT_LEAF_LAYOUT = 1 for this load, so the *_leaves calls can walk it."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
+        if leaves:
+            saved = getattr(self, "_leaf_opt", 0)
+            self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
+            try:
+                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned)
+            finally:
+                self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
         if binned:
             self._check(self._lib.dte_load_ensemble_binned(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
                                                            int(first_tree), int(num_local_trees), int(num_classes)))
@@ -359,6 +374,29 @@ class Engine:
     def kernel_name_binned(self):
         buf = C.create_string_buffer(256)
         self._check(self._lib.dte_kernel_name_binned(self._h, buf, 256))
+        return buf.value.decode()
+
+    # -- leaf-index inference (DESIGN.md §10) ----------------------------------------------------------
+    def infer_device_leaves(self, d_tuples, n, d_leaves, stream=None):
+        """[n, T] uint16 leaf cells of fp32 tuples [n, F] into d_leaves (both on the device, 16-byte aligned)."""
+        self._check(self._lib.dte_infer_device_leaves(self._h, _ptr(d_tuples), int(n), _ptr(d_leaves), _stream(stream)))
+
+    def infer_host_leaves(self, tuples, out=None):
+        """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> [n, T] uint16: the cell, in tree t's
+        own weight heap, of the leaf that local tree t sends each tuple to (T = info()["num_trees"])."""
+        if isinstance(tuples, np.ndarray):
+            t = np.ascontiguousarray(tuples)
+            n = t.shape[0]
+        else:
+            t = tuples
+            n = int(tuples.shape[0])
+        leaves = out if out is not None else np.empty((n, int(self.info()["num_trees"])), dtype=np.uint16)
+        self._check(self._lib.dte_infer_host_leaves(self._h, _ptr(t), n, _ptr(leaves)))
+        return leaves
+
+    def kernel_name_leaves(self):
+        buf = C.create_string_buffer(256)
+        self._check(self._lib.dte_kernel_name_leaves(self._h, buf, 256))
         return buf.value.decode()
 
     def infer_device_accumulate(self, d_tuples, n, d_scores_accum, stream=None):

@@ -128,6 +128,16 @@ def bin_tuples(x_words, offsets, edges, missing=MISSING_DEFAULT):
     return out
 
 
+def leaf_values(W, cells, first=0):
+    """Per-tree leaf words from leaf cells: W uint32 [T_all, 2^(D+1)-1] (the stream's weight heaps), cells [n, T] as
+    Engine.infer_*_leaves returns them for the chunk starting at stream tree `first` -> uint32 [n, T] with
+    out[i, t] = W[first + t, cells[i, t]], bit for bit the leaf word the score adds."""
+    W = np.asarray(W, dtype=np.uint32)
+    cells = np.asarray(cells).astype(np.int64)
+    T = cells.shape[1]
+    return W[int(first) + np.arange(T)[None, :], cells]
+
+
 def result_lines(scores):
     """Scores in tuple order -> result CLs, 4 per line; a trailing group of < 4 is not emitted
     (rtl/DTEngine/ResultsCombiner.sv:132-162)."""

@@ -207,6 +207,30 @@ int dte_infer_host_binned(dte_t* engine, const void* h_bins, size_t n, float* h_
 /* dte_kernel_name of the binned walk ("dt_walk_tile_u8<...> ..." / "dt_walk_generic_u8<...>"). */
 int dte_kernel_name_binned(dte_t* engine, char* buf, size_t len);
 
+/* ---- leaf-index inference (DESIGN.md §10) ----------------------------------------------------- */
+/* Which leaf every tree sends each tuple to (XGBoost / LightGBM pred_leaf, scikit-learn apply).  leaves[i][t] is a uint16:
+ * the index, in tree t's own weight heap W[t][0 .. 2^(D+1)-2] of the tree streams, of the cell whose word the score walk
+ * adds for tuple i, i.e. where the walk n = 0; D times { n = 2n+1+right }, stopping after the step taken from a node
+ * with bit 14 set, ends.  W[t][leaves[i][t]] is always bit for bit the leaf word of the score.  A complete tree gives
+ * cells 2^D-1 .. 2^(D+1)-2; an early leaf gives its own cell; D = 1 gives 1 or 2 (D <= 15, so cells fit 16 bits).
+ * Column t is local tree t in stream order (stream tree first_tree + t of the loaded chunk) whatever the class count.
+ * Every resident tree is walked: registers 204/205 supply F, D and the missing pattern, and K and S do not matter (a
+ * multi-class ensemble whose largest class exceeds S*K*8 is not refused here).  Needs the leaf-id layout of a
+ * placement made with DTE_OPT_LEAF_LAYOUT = 1, else DTE_ERR_STATE.  A binned load builds it too; these calls take fp32
+ * tuples. */
+/* [n][T] cells into d_leaves for n fp32 tuples in device memory; T = the resident trees.  Single-device handles; stream
+ * as dte_infer_device.  d_tuples and d_leaves must be 16-byte aligned (cells go out in stores of up to 16 bytes), else
+ * DTE_ERR_ARG before any launch. */
+int dte_infer_device_leaves(dte_t* engine, const void* d_tuples, size_t n, uint16_t* d_leaves, void* cuda_stream);
+/* The same from host memory through the landing pipeline, every handle kind: [n][T] cells with T = dte_info.num_trees.
+ * Data-sharded handles return the rows in global tuple order; ensemble-sharded handles walk every tuple on every ring
+ * position, which lands its cells in its own columns (position r: columns from the trees of positions 0..r-1 on).
+ * The leaf buffers of the landing slots are allocated by the first call. */
+int dte_infer_host_leaves(dte_t* engine, const void* h_tuples, size_t n, uint16_t* h_leaves);
+/* dte_kernel_name of the leaf walk ("dt_walk_tile_leaf<...> ..." / "dt_walk_generic_leaf<...>"); DTE_ERR_STATE without a
+ * leaf-id layout. */
+int dte_kernel_name_leaves(dte_t* engine, char* buf, size_t len);
+
 /* Page-locked host memory every device of the handle can DMA from / to at full PCIe speed (cudaHostAlloc, portable):
  * what a Catapult host gets from the driver's DMA-buffer allocator (the slot buffers behind rtl/PCIeShim.sv:99-141).
  * Pageable memory works everywhere too, through the CUDA driver's staging copies (about 5 x slower). */
@@ -242,7 +266,10 @@ typedef enum {
     DTE_OPT_COMBINE = 2,          /* multi-device aggregate mode: 0 (default) = ring-order peer-read kernel (bit-exact),
                                      1 = one ncclReduce(SUM) to the host device (order free: 1e-5 relative) */
     DTE_OPT_RESULT_QUEUE_LINES = 3, /* capacity of the result queue in 128-bit lines (0 = derive from reg 207) */
-    DTE_OPT_CHUNK_TUPLES = 4      /* tuples per landing buffer of the H2D | walk | D2H pipeline (0 = 64 MiB worth) */
+    DTE_OPT_CHUNK_TUPLES = 4,     /* tuples per landing buffer of the H2D | walk | D2H pipeline (0 = 64 MiB worth) */
+    DTE_OPT_LEAF_LAYOUT = 5       /* 1: every placement of an ensemble (dte_load_ensemble*, a tree line stream) also builds
+                                     and uploads the leaf-id layout the dte_*_leaves calls walk, and ensemble_bytes counts
+                                     it; 0 (default): a placement builds none and drops a resident one */
 } dte_option;
 int dte_set_option(dte_t* engine, int option, uint64_t value);
 

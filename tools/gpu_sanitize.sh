@@ -3,7 +3,8 @@
 # dt_walk_tile<4,2,1,0,384>, phased ring refill, CTAs with two tiles) and over the planner's alternatives.
 # Logs (with the kernel name printed by the test) go to <logdir>/sanitizer_<tool>_<plan>.log.
 #   bash tools/gpu_sanitize.sh [logdir=sanitizer_logs]   memcheck + synccheck over four launch plans, a 3-class
-#                                                        ensemble and seven kernel-matrix instantiations, racecheck
+#                                                        ensemble, seven kernel-matrix instantiations, the binned and
+#                                                        the leaf walks, racecheck
 #                                                        once (AUTO)
 # racecheck does not model the mbarrier / cp.async.bulk (async-proxy) hand-off: tools/racecheck_canonical.cu is the
 # textbook producer/consumer ring with exactly that synchronisation, run under the same tool for comparison.
@@ -42,6 +43,11 @@ for T in tests/test_gpu_binned.py::test_headline_binned_multi_tile tests/test_gp
          "tests/test_gpu_binned.py::test_depths[3]"; do
   btag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   for tool in memcheck synccheck; do run $tool "" ""; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_binned_${btag}.log"; done
+done
+# the leaf walk (cell stores instead of the reduction): the headline plan with three tiles per CTA, and the generic kernel
+for T in tests/test_gpu_leaves.py::test_headline_leaf_plan_multi_tile "tests/test_gpu_leaves.py::test_small_batches[33]"; do
+  ltag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  for tool in memcheck synccheck; do run $tool "" ""; mv "$OUT/sanitizer_${tool}_auto.log" "$OUT/sanitizer_${tool}_leaf_${ltag}.log"; done
 done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1

@@ -7,8 +7,12 @@
 // With <classes> the T trees starting at stream tree <first> are packed as a multi-class ensemble (class-major, every
 // class padded to whole tree8 groups).  The class-major permutation is undone here from the stream index alone, so the
 // leaves come out in stream order; every padding slot must decode to the leaf +0 for every tuple (exit 5 otherwise).
+//   pack_check leaf <same arguments>
+//     ->  n*T uint16 leaf cells (binary, stdout): the leaf-id layout (bottom_id) packed as well and decoded as the leaf
+//         walks decode it, the cell in the stream tree's own heap that each (tuple, tree) ends in
 #include "../distributed-decisiontrees_b200/csrc/dte_device.cuh"
 #include <cstdio>
+#include <cstring>
 using namespace dte;
 
 static std::vector<unsigned char> slurp(const char* p) {
@@ -23,7 +27,8 @@ static std::vector<unsigned char> slurp(const char* p) {
 }
 
 // leaf word of tree slot `slot` of the packed layout for tuple x, decoded as the kernels decode it
-static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x, uint32_t missing) {
+// `bottom`: pk.bottom (leaf words) or pk.bottom_id (leaf cells)
+static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x, uint32_t missing, const std::vector<uint4>& bottom) {
     const EnsembleShape& sh = pk.shape;
     const int BV = sh.wide ? 4 : 2;
     // top: byte offset o into the tree's 8-byte heap records, child = 2o + 8 + 8*right  (step_inc in dte_kernels.cuh)
@@ -37,7 +42,7 @@ static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x,
         o = 2 * o + inc;
     }
     const uint32_t j = (o >> 3) - (sh.nb - 1);
-    const uint4* rec = pk.bottom.data() + ((size_t)slot * sh.nb + j) * BV;
+    const uint4* rec = bottom.data() + ((size_t)slot * sh.nb + j) * BV;
     uint32_t fp, fl_, fr, mp, ml, mr; uint4 leaves;
     if (sh.wide) {
         fp = rec[0].w & 0xFFFFu; mp = rec[0].w >> 16; fl_ = rec[1].x & 0xFFFFu; ml = rec[1].x >> 16;
@@ -55,6 +60,8 @@ static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x,
 }
 
 int main(int argc, char** argv) {
+    const bool leaf = argc > 1 && !strcmp(argv[1], "leaf");
+    if (leaf) { --argc; ++argv; }
     if (argc < 9) return 2;
     Geom g;
     g.D = (uint32_t)atoi(argv[1]); const uint32_t F = (uint32_t)atoi(argv[2]), T = (uint32_t)atoi(argv[3]);
@@ -67,8 +74,8 @@ int main(int argc, char** argv) {
     const uint32_t C = classed ? (uint32_t)atoi(argv[9]) : 1u, first = argc > 10 ? (uint32_t)atoi(argv[10]) : 0u;
     PackedEnsemble pk;
     std::string msg;
-    int rc = classed ? pack_ensemble(g, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16, first, T, C, pk, msg)
-                     : pack_ensemble(g, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16, 0, 0, 1, pk, msg);
+    int rc = classed ? pack_ensemble(g, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16, first, T, C, pk, msg, nullptr, leaf)
+                     : pack_ensemble(g, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16, 0, 0, 1, pk, msg, nullptr, leaf);
     if (rc) { fprintf(stderr, "pack_ensemble: %d %s\n", rc, msg.c_str()); return 3; }
     const EnsembleShape& sh = pk.shape;
     if (sh.T != T || sh.C != C) return 4;
@@ -86,12 +93,24 @@ int main(int argc, char** argv) {
     std::vector<uint8_t> used(sh.Tpad, 0);
     for (uint32_t t = 0; t < T; ++t) { slot[t] += ((first + t) % C) * gpc * 8; used[slot[t]] = 1; }
     const uint32_t* X = reinterpret_cast<const uint32_t*>(xs.data());
+    if (leaf) {
+        if (pk.bottom_id.size() != pk.bottom.size()) return 4;
+        std::vector<uint16_t> cells(n * T);
+        for (size_t i = 0; i < n; ++i)
+            for (uint32_t t = 0; t < T; ++t) {
+                const uint32_t c = walk(pk, slot[t], X + i * F, g.missing, pk.bottom_id);
+                if (c > 0xFFFFu) return 6;
+                cells[i * T + t] = (uint16_t)c;
+            }
+        fwrite(cells.data(), 2, cells.size(), stdout);
+        return 0;
+    }
     std::vector<uint32_t> out(n * T);
     for (size_t i = 0; i < n; ++i) {
         const uint32_t* x = X + i * F;
-        for (uint32_t t = 0; t < T; ++t) out[i * T + t] = walk(pk, slot[t], x, g.missing);
+        for (uint32_t t = 0; t < T; ++t) out[i * T + t] = walk(pk, slot[t], x, g.missing, pk.bottom);
         for (uint32_t s = 0; s < sh.Tpad; ++s)
-            if (!used[s] && walk(pk, s, x, g.missing) != 0u) {
+            if (!used[s] && walk(pk, s, x, g.missing, pk.bottom) != 0u) {
                 fprintf(stderr, "padding slot %u gives a non-zero leaf for tuple %zu\n", s, i);
                 return 5;
             }

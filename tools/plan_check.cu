@@ -5,6 +5,7 @@
 //     <D> <F> <C> <variant> <phased level, -1 = off> <kernel name>
 // tests/test_plan_table.py compares the output with tests/golden/plan_table.txt.xz.  Test infrastructure.
 //   plan_check bin   the same grid for the binned walk (u8 tile, 4-byte tree tops): tests/golden/plan_table_binned.txt.xz
+//   plan_check leaf  the same grid for the leaf walk (dt_walk_*_leaf): tests/golden/plan_table_leaf.txt.xz
 #include "../distributed-decisiontrees_b200/csrc/dte_device.cuh"
 #include <cstdio>
 #include <cstdlib>
@@ -28,6 +29,7 @@ static const char* const kTunes[] = {
 
 int main(int argc, char** argv) {
     const bool bin = argc > 1 && !strcmp(argv[1], "bin");
+    const bool leaf = argc > 1 && !strcmp(argv[1], "leaf");
     const uint32_t Fs[] = {4, 8, 32, 64, 96, 128, 192, 256, 384, 512, 516, 768, 1024, 1536, 1796, 1800, 2048};
     for (const char* s : kTunes) {
         setenv("DTE_TUNE", s, 1);
@@ -52,7 +54,7 @@ int main(int argc, char** argv) {
                     sh.Tpad = C * sh.gpc * 8;
                     for (int want = KERNEL_AUTO; want <= KERNEL_TILE_STAGED; ++want) {
                         char name[256];
-                        kernel_name(d, tune, want, name, sizeof name, bin);
+                        kernel_name(d, tune, want, name, sizeof name, bin, leaf);
                         const auto pl = make_plan(d, tune, want, bin);
                         printf("%u %u %u %d %d %s\n", D, F, C, want, (int)phased_level(d, tune, pl), name);
                     }
