@@ -44,23 +44,23 @@ def numpy_edges(W, FI, D, F):
     return np.array(offsets, dtype=np.uint32), (np.concatenate(edges) if edges else np.zeros(0, np.int32)).view(np.uint32)
 
 
-def run_bin_check(tmp_path, W, FI, x, D, T, first=0, classes=1):
+def run_bin_check(tmp_path, W, FI, x, D, T, first=0, classes=1, missing=L.MISSING_DEFAULT):
     from ddt_b200 import build as B
     exe = B.build_bin_check()
     F = x.shape[1]
     wl, fl = L.pack_streams(W, FI, D)
     for name, arr in (("w", wl), ("f", fl), ("x", x)):
         np.ascontiguousarray(arr).tofile(tmp_path / (name + ".bin"))
-    out = subprocess.run([exe, str(D), str(F), str(T), str(x.shape[0]), str(L.MISSING_DEFAULT), str(tmp_path / "w.bin"),
+    out = subprocess.run([exe, str(D), str(F), str(T), str(x.shape[0]), str(missing), str(tmp_path / "w.bin"),
                           str(tmp_path / "f.bin"), str(tmp_path / "x.bin"), str(classes), str(first), str(tmp_path / "e.bin")],
                          capture_output=True, timeout=300)
     return out
 
 
-def check_against_oracle(tmp_path, W, FI, x, D, first=0, T=None, classes=1, stride=1):
+def check_against_oracle(tmp_path, W, FI, x, D, first=0, T=None, classes=1, stride=1, missing=L.MISSING_DEFAULT):
     T_all, F = W.shape[0], x.shape[1]
     T = T_all - first if T is None else T
-    out = run_bin_check(tmp_path, W, FI, x, D, T, first, classes)
+    out = run_bin_check(tmp_path, W, FI, x, D, T, first, classes, missing)
     assert out.returncode == 0, (D, out.returncode, out.stderr)
     got = np.frombuffer(out.stdout, dtype=np.uint32).reshape(x.shape[0], T)
     e = np.fromfile(tmp_path / "e.bin", dtype=np.uint32)
@@ -68,7 +68,7 @@ def check_against_oracle(tmp_path, W, FI, x, D, first=0, T=None, classes=1, stri
     want_off, want_edges = numpy_edges(W, FI, D, F)
     assert (off == want_off).all() and (edges == want_edges).all(), "edge table differs from np.unique over the live nodes"
     lib = O.lib()
-    cfg = oracle_cfg(D, 1, 1, L.MISSING_DEFAULT, F, T_all)
+    cfg = oracle_cfg(D, 1, 1, missing, F, T_all)
     wl, fl = L.pack_streams(W, FI, D)
     wt_all, ft_all = wl.reshape(T_all, -1), fl.reshape(T_all, -1)
     for t in range(T):
@@ -79,7 +79,7 @@ def check_against_oracle(tmp_path, W, FI, x, D, first=0, T=None, classes=1, stri
             want = lib.dteo_leaf(C.byref(cfg), wt.ctypes.data, ft.ctypes.data, xi.ctypes.data)
             assert got[i, t] == want, (D, first + t, i, hex(got[i, t]), hex(want))
     # and the host definition of the bin format agrees with the checker's edges
-    b = L.bin_tuples(x, off, edges)
+    b = L.bin_tuples(x, off, edges, missing)
     assert b.dtype == np.uint8 and b.max() <= 255
     return off, edges
 

@@ -11,6 +11,7 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
+from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_leaves
 from helpers import geometry_regs, multi_node_regs, oracle_scores, L
 from oracle import oracle as O
 
@@ -46,15 +47,29 @@ def plan_rows():
 
 
 def matrix_cases():
-    """One typical (|D - 10|, F smallest) and one extreme (largest D, F) row per (binned kernel template, C)."""
+    """One typical (|D - 10|, F smallest) and one extreme (largest D, F) row per (binned kernel template, C), as
+    (row, None); then the typical row of every group on edge operands (tests/edge_operands.py), as (row, missing
+    pattern) with the pattern taken from MISSING_ROTATION by group index."""
     groups = collections.OrderedDict()
     for r in plan_rows():
         groups.setdefault((r.name.split(">")[0] + ">", r.C), []).append(r)
-    out = []
-    for (t, C), rs in groups.items():
-        for kind, r in (("typical", min(rs, key=lambda r: (abs(r.D - 10), r.F))), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
-            out.append(pytest.param(r, id="%s-C%d-%s-D%d-F%d" % (t.replace(" ", ""), C, kind, r.D, r.F)))
-    return out
+    out, edge = [], []
+    for i, ((t, C), rs) in enumerate(groups.items()):
+        typical = min(rs, key=lambda r: (abs(r.D - 10), r.F))
+        for kind, r in (("typical", typical), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
+            out.append(pytest.param(r, None, id="%s-C%d-%s-D%d-F%d" % (t.replace(" ", ""), C, kind, r.D, r.F)))
+        m = MISSING_ROTATION[i % len(MISSING_ROTATION)]
+        edge.append(pytest.param(typical, m, id="%s-C%d-edge-D%d-F%d-m%08x" % (t.replace(" ", ""), C, typical.D, typical.F, m)))
+    return out + edge
+
+
+def wave_tuples(name, sm_count=132):
+    """Tuples of one wave of CTAs of a binned plan (32 x consumer warps / warps per group per CTA); 128 per block for
+    the generic kernel."""
+    if "tile" not in name:
+        return 128 * sm_count
+    pair = int(name.split("<")[1].split(",")[1])
+    return sm_count * 32 * int(name.split("warps=")[1].split()[0]) // pair
 
 
 def hist_ensemble(T, D, F, seed, cuts=254, wide=None):
@@ -68,14 +83,14 @@ def hist_ensemble(T, D, F, seed, cuts=254, wide=None):
     return W, FI
 
 
-def oracle_words(W, FI, x, D, K, S, C):
+def oracle_words(W, FI, x, D, K, S, C, missing=L.MISSING_DEFAULT):
     kw = dict(threads=O.max_threads())
     if C == 1:
-        return oracle_scores(W, FI, x, D, K, S, L.MISSING_DEFAULT, **kw)
+        return oracle_scores(W, FI, x, D, K, S, missing, **kw)
     out = np.zeros((x.shape[0], C), dtype=np.uint32)
     for c in range(C):
         if W[c::C].shape[0]:
-            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, L.MISSING_DEFAULT, **kw)
+            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, missing, **kw)
     return out
 
 
@@ -91,58 +106,70 @@ def assert_words(sc, lb, want, C, what):
         assert (np.asarray(lb) == labels_of(want, C)).all(), what + ": labels differ"
 
 
-def make_engine(T, D, F, K, S):
+def make_engine(T, D, F, K, S, missing=L.MISSING_DEFAULT):
     e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, L.MISSING_DEFAULT).items()):
+    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
         e.softreg_write(a, v)
     return e
 
 
-def run_case(torch, T, D, F, K, S, C, n, seed, variants=VARIANTS):
+def run_case(torch, T, D, F, K, S, C, n, seed, variants=VARIANTS, missing=None):
     """Load binned; for every variant: host binned (bins from bin_edges + layout.bin_tuples) and device binned (bins from
-    dte_bin_tuples_device on a non-default stream) against the oracle; the device bins equal the host bins byte for byte."""
-    W, FI = hist_ensemble(T, D, F, seed)
-    x = L.synth_tuples(0, n, F, seed=seed + 1, missing_ppm=20000)
-    wl, fl = L.pack_streams(W, FI, D)
-    want = oracle_words(W, FI, x, D, K, S, C)
+    dte_bin_tuples_device on a non-default stream) against the oracle; the device bins equal the host bins byte for byte.
+    missing given: edge operands (tests/edge_operands.py) with that missing pattern, the same trees loaded with wide and
+    then with small leaves on one handle."""
+    if missing is None:
+        W, FI = hist_ensemble(T, D, F, seed)
+        x = L.synth_tuples(0, n, F, seed=seed + 1, missing_ppm=20000)
+        loads, missing = [W], L.MISSING_DEFAULT
+    else:
+        W, FI, pools = edge_ensemble(T, D, F, seed, leaves="wide", missing=missing)
+        x = edge_tuples(n, F, pools, seed + 1, missing)
+        loads = [W, with_leaves(W, D, "small", seed)]
     names = {}
-    with make_engine(T, D, F, K, S) as e:
-        e.load_ensemble(wl, fl, num_classes=C, binned=True)
-        off, edges = e.bin_edges()
-        b = L.bin_tuples(x, off, edges)
-        dx = torch.from_numpy(x.view(np.int32)).cuda()
-        db = torch.empty((n, F), dtype=torch.uint8, device="cuda")
-        s = torch.cuda.Stream()
-        e.bin_tuples_device(dx, n, db, stream=s.cuda_stream)
-        s.synchronize()
-        assert (db.cpu().numpy() == b).all(), "dte_bin_tuples_device differs from layout.bin_tuples"
-        for v in variants:
-            e.set_kernel_variant(v)
-            names[v] = e.kernel_name_binned()
-            sc, lb = e.infer_host_binned(b)
-            assert_words(sc, lb, want, C, "host %s" % names[v])
-            ds = torch.empty((n, C) if C > 1 else (n,), dtype=torch.float32, device="cuda")
-            dl = torch.empty(n, dtype=torch.uint8, device="cuda")
-            e.infer_device_binned(db, n, ds, dl, stream=s.cuda_stream)
+    with make_engine(T, D, F, K, S, missing) as e:
+        for Wl in loads:
+            want = oracle_words(Wl, FI, x, D, K, S, C, missing)
+            e.load_ensemble(*L.pack_streams(Wl, FI, D), num_classes=C, binned=True)
+            off, edges = e.bin_edges()
+            b = L.bin_tuples(x, off, edges, missing)
+            dx = torch.from_numpy(x.view(np.int32)).cuda()
+            db = torch.empty((n, F), dtype=torch.uint8, device="cuda")
+            s = torch.cuda.Stream()
+            e.bin_tuples_device(dx, n, db, stream=s.cuda_stream)
             s.synchronize()
-            assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "device %s" % names[v])
-        # the fp32 calls still score a binned load correctly
-        e.set_kernel_variant(E.DTE_KERNEL_AUTO)
-        sc, lb = e.infer_host(x)
-        assert_words(sc, lb, want, C, "fp32 after a binned load")
+            assert (db.cpu().numpy() == b).all(), "dte_bin_tuples_device differs from layout.bin_tuples"
+            for v in variants:
+                e.set_kernel_variant(v)
+                names[v] = e.kernel_name_binned()
+                sc, lb = e.infer_host_binned(b)
+                assert_words(sc, lb, want, C, "host %s" % names[v])
+                ds = torch.empty((n, C) if C > 1 else (n,), dtype=torch.float32, device="cuda")
+                dl = torch.empty(n, dtype=torch.uint8, device="cuda")
+                e.infer_device_binned(db, n, ds, dl, stream=s.cuda_stream)
+                s.synchronize()
+                assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "device %s" % names[v])
+            # the fp32 calls still score a binned load correctly
+            e.set_kernel_variant(E.DTE_KERNEL_AUTO)
+            sc, lb = e.infer_host(x)
+            assert_words(sc, lb, want, C, "fp32 after a binned load")
     return names
 
 
-@pytest.mark.parametrize("row", matrix_cases())
-def test_reachable_binned_instantiation_bit_exact(torch_cuda, row, monkeypatch):
+@pytest.mark.parametrize("row,missing", matrix_cases())
+def test_reachable_binned_instantiation_bit_exact(torch_cuda, row, missing, monkeypatch):
     """Every binned kernel the planner reaches, with its pin, geometry and variant from the binned plan table; enough
-    tuples for every CTA to walk two tiles."""
+    tuples for every CTA to walk two tiles.  Edge cases (missing given): edge operands on one wave of CTAs plus a ragged
+    tail."""
     monkeypatch.setenv("DTE_TUNE", row.tune)
     T = 8 * 3 * max(1, row.C) if row.C > 1 else 40
     K, S = 1, 5
-    n = 132 * 2 * 32 * 12 + 33 if row.variant != E.DTE_KERNEL_GENERIC else 5000
-    names = run_case(torch_cuda, T, row.D, row.F, K, S, row.C, min(n, 100_000 if row.F <= 512 else 20_000), 1000 + row.D,
-                     variants=[row.variant])
+    if missing is None:
+        n = 132 * 2 * 32 * 12 + 33 if row.variant != E.DTE_KERNEL_GENERIC else 5000
+        n = min(n, 100_000 if row.F <= 512 else 20_000)
+    else:
+        n = wave_tuples(row.name) + 33
+    names = run_case(torch_cuda, T, row.D, row.F, K, S, row.C, n, 1000 + row.D, variants=[row.variant], missing=missing)
     assert names[row.variant] == row.name
 
 

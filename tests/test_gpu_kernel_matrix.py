@@ -19,6 +19,7 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
+from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_leaves
 from helpers import geometry_regs, oracle_scores, L
 from oracle import oracle as O
 
@@ -85,10 +86,22 @@ def compiled_templates():
 
 
 def matrix_cases():
+    """(row, None): the typical and the extreme row of every group on the standard data."""
     out = []
     for (template, C), (typical, extreme) in kernel_groups().items():
         for kind, row in (("typical", typical), ("extreme", extreme)):
-            out.append(pytest.param(row, id="%s-C%d-%s-D%d-F%d" % (template.replace(" ", ""), C, kind, row.D, row.F)))
+            out.append(pytest.param(row, None, id="%s-C%d-%s-D%d-F%d" % (template.replace(" ", ""), C, kind, row.D, row.F)))
+    return out
+
+
+def edge_cases():
+    """(row, missing pattern): the typical row of every group on edge operands (tests/edge_operands.py), the missing
+    pattern taken from MISSING_ROTATION by group index."""
+    out = []
+    for i, ((template, C), (typical, _)) in enumerate(kernel_groups().items()):
+        missing = MISSING_ROTATION[i % len(MISSING_ROTATION)]
+        out.append(pytest.param(typical, missing, id="%s-C%d-edge-D%d-F%d-m%08x" % (
+            template.replace(" ", ""), C, typical.D, typical.F, missing)))
     return out
 
 
@@ -100,9 +113,9 @@ def torch_cuda():
     return torch
 
 
-def make_engine(T, D, F, K, S):
+def make_engine(T, D, F, K, S, missing=L.MISSING_DEFAULT):
     e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, L.MISSING_DEFAULT).items()):
+    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
         e.softreg_write(a, v)
     return e
 
@@ -128,16 +141,16 @@ def ensemble(T, D, F, seed, max_index=None):
     return W, FI
 
 
-def oracle_words(W, FI, x, D, K, S, C):
+def oracle_words(W, FI, x, D, K, S, C, missing=L.MISSING_DEFAULT):
     """uint32 words [n] (C = 1) or [n, C]: column c is the oracle's score of the class-c trees alone (tree t of the
     stream belongs to class t % C); a class without trees scores +0."""
     kw = dict(threads=O.max_threads())
     if C == 1:
-        return oracle_scores(W, FI, x, D, K, S, L.MISSING_DEFAULT, **kw)
+        return oracle_scores(W, FI, x, D, K, S, missing, **kw)
     out = np.zeros((x.shape[0], C), dtype=np.uint32)
     for c in range(C):
         if W[c::C].shape[0]:
-            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, L.MISSING_DEFAULT, **kw)
+            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, missing, **kw)
     return out
 
 
@@ -209,44 +222,58 @@ def test_plan_table_reaches_42_kernel_groups():
             assert r.template == t and r.C == C and r.name.endswith(" classes=3") == (C == 3)
         assert (extreme.D, extreme.F) >= (typical.D, typical.F)
     assert len(matrix_cases()) == 84
+    edge = edge_cases()
+    assert len(edge) == 42 and {p.values[1] for p in edge} == set(MISSING_ROTATION)
 
 
 # ---- 2a: the instantiation matrix -----------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("row", matrix_cases())
-def test_reachable_instantiation_bit_exact(row, monkeypatch, torch_cuda):
+@pytest.mark.parametrize("row,missing", matrix_cases() + edge_cases())
+def test_reachable_instantiation_bit_exact(row, missing, monkeypatch, torch_cuda):
     """The table row's pin, geometry and variant: the live kernel name is the table's, and on enough tuples that every
     CTA walks at least two tiles (ring wrap, tile reload, dead lanes in the last tile) every score word and label equals
     the oracle's, through dte_infer_host and through dte_infer_device on a non-default torch stream.  T is not a
-    multiple of 8; C = 3 has classes of 10, 10 and 9 trees (two groups per class)."""
+    multiple of 8; C = 3 has classes of 10, 10 and 9 trees (two groups per class).
+    Edge cases (missing given): edge operands with that missing pattern on one wave of CTAs plus a ragged tail, the
+    same trees loaded with wide and then with small leaves on one handle."""
     torch = torch_cuda
     monkeypatch.setenv("DTE_TUNE", row.tune)
     D, F, C = row.D, row.F, row.C
     T, K, S = (21, 2, 2) if C == 1 else (29, 2, 1)
-    seed = 5000 + 97 * D + F + C
-    W, FI = ensemble(T, D, F, seed)
-    wl, fl = L.pack_streams(W, FI, D)
-    with make_engine(T, D, F, K, S) as e:
-        e.load_ensemble(wl, fl, num_classes=C)
-        e.set_kernel_variant(row.variant)
-        assert e.kernel_name() == row.name
-        info = e.info()
-        cap = info["tuples_per_cta"] * info["sm_count"]
-        n = cap + 33 if SANITIZER else 2 * cap + 33
-        assert cap < n
-        x = tuples(0, n, F, seed + 1)
-        want = oracle_words(W, FI, x, D, K, S, C)
-        sc, lb = e.infer_host(x)
-        assert_words(sc, lb, want, C, "infer_host %s" % row.name)
-        st = torch.cuda.Stream()
-        with torch.cuda.stream(st):
-            dx = torch.from_numpy(x.view(np.int32)).cuda()
-            ds = torch.full(want.shape, float("nan"), dtype=torch.float32, device="cuda")
-            dl = torch.full((n,), 77, dtype=torch.uint8, device="cuda")
-            e.infer_device(dx, n, ds, dl, stream=st.cuda_stream)
-        st.synchronize()
-        assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "infer_device %s" % row.name)
-        del dx, ds, dl
+    if missing is None:
+        seed = 5000 + 97 * D + F + C
+        W, FI = ensemble(T, D, F, seed)
+        loads, missing = [W], L.MISSING_DEFAULT
+    else:
+        seed = 9000 + 97 * D + F + C
+        W, FI, pools = edge_ensemble(T, D, F, seed, leaves="wide", missing=missing)
+        loads = [W, with_leaves(W, D, "small", seed)]
+    with make_engine(T, D, F, K, S, missing) as e:
+        for Wl in loads:
+            e.load_ensemble(*L.pack_streams(Wl, FI, D), num_classes=C)
+            e.set_kernel_variant(row.variant)
+            assert e.kernel_name() == row.name
+            info = e.info()
+            cap = info["tuples_per_cta"] * info["sm_count"]
+            if len(loads) == 1:
+                n = cap + 33 if SANITIZER else 2 * cap + 33
+                x = tuples(0, n, F, seed + 1)
+            else:
+                n = cap + 33
+                x = edge_tuples(n, F, pools, seed + 1, missing)
+            assert cap < n
+            want = oracle_words(Wl, FI, x, D, K, S, C, missing)
+            sc, lb = e.infer_host(x)
+            assert_words(sc, lb, want, C, "infer_host %s" % row.name)
+            st = torch.cuda.Stream()
+            with torch.cuda.stream(st):
+                dx = torch.from_numpy(x.view(np.int32)).cuda()
+                ds = torch.full(want.shape, float("nan"), dtype=torch.float32, device="cuda")
+                dl = torch.full((n,), 77, dtype=torch.uint8, device="cuda")
+                e.infer_device(dx, n, ds, dl, stream=st.cuda_stream)
+            st.synchronize()
+            assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "infer_device %s" % row.name)
+            del dx, ds, dl
 
 
 # ---- 2b: edges ------------------------------------------------------------------------------------------------------

@@ -12,6 +12,7 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
+from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples
 from helpers import geometry_regs, multi_node_regs, L
 from leaf_oracle import leaf_cells
 from oracle import oracle as O
@@ -31,10 +32,10 @@ def torch_cuda():
     return torch
 
 
-def make_engine(T, D, F, K=8, S=None):
+def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
     e = ddt.Engine(0)
     S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, L.MISSING_DEFAULT).items()):
+    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
         e.softreg_write(a, v)
     return e
 
@@ -101,41 +102,57 @@ def plan_rows():
 
 
 def matrix_cases():
-    """One typical and one extreme row per (leaf kernel template, C) of the leaf plan table."""
+    """(row, whole, missing): one typical and one extreme row per (leaf kernel template, C) of the leaf plan table, each
+    at a ragged and at a whole T on the standard data (missing None); then the typical row of every group at the ragged
+    T on edge operands (tests/edge_operands.py), the missing pattern taken from MISSING_ROTATION by group index."""
     groups = collections.OrderedDict()
     for r in plan_rows():
         groups.setdefault((r.name.split(">")[0] + ">", r.C), []).append(r)
-    out = []
-    for (t, C), rs in groups.items():
-        for kind, r in (("typical", min(rs, key=lambda r: (abs(r.D - 10), r.F))), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
-            out.append(pytest.param(r, id="%s-C%d-%s-D%d-F%d" % (t.replace(" ", ""), C, kind, r.D, r.F)))
-    return out
+    out, edge = [], []
+    for i, ((t, C), rs) in enumerate(groups.items()):
+        typical = min(rs, key=lambda r: (abs(r.D - 10), r.F))
+        for kind, r in (("typical", typical), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
+            for whole, wid in ((False, "T-ragged"), (True, "T-whole")):
+                out.append(pytest.param(r, whole, None, id="%s-C%d-%s-D%d-F%d-%s" % (t.replace(" ", ""), C, kind, r.D, r.F, wid)))
+        m = MISSING_ROTATION[i % len(MISSING_ROTATION)]
+        edge.append(pytest.param(typical, False, m, id="%s-C%d-edge-D%d-F%d-m%08x-T-ragged" % (
+            t.replace(" ", ""), C, typical.D, typical.F, m)))
+    return out + edge
 
 
-@pytest.mark.parametrize("whole", [False, True], ids=["T-ragged", "T-whole"])
-@pytest.mark.parametrize("row", matrix_cases())
-def test_every_reachable_leaf_kernel(torch_cuda, row, whole, monkeypatch):
+@pytest.mark.parametrize("row,whole,missing", matrix_cases())
+def test_every_reachable_leaf_kernel(torch_cuda, row, whole, missing, monkeypatch):
     """Pin the row's DTE_TUNE and variant, check the kernel name, and walk two tiles per CTA.  T-ragged: T not a
     multiple of 8 (one class: the 2-byte cell stores; several: padding slots).  T-whole: T = 32 per class, so a
-    one-class walk takes the 2*ILP-byte vector stores."""
+    one-class walk takes the 2*ILP-byte vector stores.  Edge cases (missing given): edge operands with early leaves
+    and that missing pattern on one wave of CTAs plus a ragged tail."""
     monkeypatch.setenv("DTE_TUNE", row.tune)
     D, F, C = row.D, row.F, row.C
     T = 32 * C if whole else 32 * C - (3 if C > 1 else 5)
-    W, FI = L.synth_ensemble(T, D, F, seed=800 + D)
-    if F > 512:
-        FI[0, (1 << D) - 2] = (FI[0, (1 << D) - 2] & 0x2000) | (F - 1)
+    edge = missing is not None
+    if not edge:
+        W, FI = L.synth_ensemble(T, D, F, seed=800 + D)
+        if F > 512:
+            FI[0, (1 << D) - 2] = (FI[0, (1 << D) - 2] & 0x2000) | (F - 1)
+        missing = L.MISSING_DEFAULT
+    else:
+        W, FI, pools = edge_ensemble(T, D, F, seed=850 + D, missing=missing)
     if D >= 2:
         FI = early(FI, D, D)
     wl, fl = L.pack_streams(W, FI, D)
-    with make_engine(T, D, F) as e:
+    with make_engine(T, D, F, missing=missing) as e:
         e.load_ensemble(wl, fl, num_classes=C, leaves=True)
         e.set_kernel_variant(row.variant)
         name = e.kernel_name_leaves()
         assert name == row.name, (name, row.name)
         tpc = int(e.info()["tuples_per_cta"]) if "tile" in name else 128
-        n = min(2 * 132 * tpc + 7, max(4096, 300000 // max(1, F)))
-        x = L.synth_tuples(0, n, F, seed=801, missing_ppm=20000)
-        want = leaf_cells(W, FI, x, D, L.MISSING_DEFAULT)
+        if edge:
+            n = 132 * tpc + 7
+            x = edge_tuples(n, F, pools, seed=851 + D, missing=missing)
+        else:
+            n = min(2 * 132 * tpc + 7, max(4096, 300000 // max(1, F)))
+            x = L.synth_tuples(0, n, F, seed=801, missing_ppm=20000)
+        want = leaf_cells(W, FI, x, D, missing)
         s = torch_cuda.cuda.Stream()
         assert_cells(device_leaves(torch_cuda, e, x, T, stream=s.cuda_stream), want, name)
 

@@ -30,14 +30,14 @@ def with_early_leaves(FI, D, rng, per_tree=3, root_tree=None):
     return FI
 
 
-def pack_check_leaf(tmp_path, W, FI, x, D, classes=None, first=0, T=None):
+def pack_check_leaf(tmp_path, W, FI, x, D, classes=None, first=0, T=None, missing=L.MISSING_DEFAULT):
     from ddt_b200 import build as B
     wl, fl = L.pack_streams(W, FI, D)
     for name, arr in (("w", wl), ("f", fl), ("x", x)):
         np.ascontiguousarray(arr).tofile(tmp_path / (name + ".bin"))
     T = W.shape[0] if T is None else T
     n, F = x.shape
-    args = [B.build_pack_check(), "leaf", str(D), str(F), str(T), str(n), str(L.MISSING_DEFAULT),
+    args = [B.build_pack_check(), "leaf", str(D), str(F), str(T), str(n), str(missing),
             str(tmp_path / "w.bin"), str(tmp_path / "f.bin"), str(tmp_path / "x.bin")]
     if classes is not None:
         args += [str(classes), str(first)]
