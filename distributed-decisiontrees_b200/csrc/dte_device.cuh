@@ -528,6 +528,50 @@ inline constexpr WalkKernel kGenericKernels[8] = {
     dt_walk_generic<true, true, false>, dt_walk_generic<false, false, true>, dt_walk_generic<false, true, true>,
     dt_walk_generic<true, false, true>, dt_walk_generic<true, true, true>};
 
+// The WalkParams of an fp32 walk of n tuples with plan pl on device d: the resident layout, the plan, the tuples and
+// the missing pattern of `run`.  The launchers add what their walk reads and writes.
+inline WalkParams walk_params(const Dev& d, const Geom& run, const Tune& tune, const Plan& pl, const void* d_tuples, size_t n) {
+    WalkParams wp = {};
+    wp.top = d.d_top;
+    wp.tuples = static_cast<const float*>(d_tuples);
+    wp.n = n;
+    wp.F = d.shape.g.F();
+    wp.Dtop = d.shape.Dtop;
+    wp.top_stride = d.shape.top_stride;
+    wp.nb = d.shape.nb;
+    wp.classes = d.shape.C;
+    wp.groups_per_class = d.shape.gpc;
+    wp.missing = run.missing;
+    wp.nwarps = (uint32_t)pl.nwarps;
+    wp.nstages = (uint32_t)pl.nstages;
+    wp.fill_split = tune.fill ? 1u : 0u;      // DTE_TUNE fill=1: one bulk copy per tree instead of one per stage
+    wp.Lw = phased_level(d, tune, pl);
+    return wp;
+}
+inline WalkParams& walk_of(WalkParams& p) { return p; }
+inline WalkParams& walk_of(LeafParams& p) { return p.w; }
+
+// Launch `kernel`, the instantiation plan pl selects, over n tuples: one 128-thread block per 128 tuples for the generic
+// walk, else one persistent CTA per SM (at most one per tile) with the plan's dynamic shared memory.  Sets the tile
+// count of the parameter block and counts the launch.  Returns a cudaError_t.
+template <class Params>
+inline cudaError_t launch_plan(Dev& d, const Plan& pl, void (*kernel)(Params), Params& params, size_t n, cudaStream_t st,
+                               const char** why) {
+    const unsigned long long units = (n + pl.tuples_per_cta() - 1) / pl.tuples_per_cta();   // blocks or tiles
+    if (units > (pl.row < 0 ? 0x7FFFFFFFull : 0xFFFFFFFFull)) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+    unsigned grid = (unsigned)units;
+    if (pl.row >= 0) {
+        walk_of(params).tiles = (uint32_t)units;
+        grid = (unsigned)std::min<unsigned long long>(units, (unsigned long long)d.sm_count);
+        const cudaError_t rc = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+        if (rc != cudaSuccess) return rc;
+    }
+    kernel<<<grid, pl.threads(), pl.row < 0 ? 0 : pl.smem, st>>>(params);
+    const cudaError_t rc = cudaGetLastError();
+    if (rc == cudaSuccess) d.kernel_launches++;
+    return rc;
+}
+
 // Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
 // `run`; the layout comes from the resident ensemble.  bin: d_tuples are u8 bins [n][F], walked against the resident
 // binned layout.  Returns a cudaError_t.
@@ -537,54 +581,21 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     *why = nullptr;
     if (n == 0) return cudaSuccess;
     const Plan pl = make_plan(d, tune, want_variant, bin);
-    WalkParams wp;
-    wp.top = d.d_top;
+    WalkParams wp = walk_params(d, run, tune, pl, bin ? nullptr : d_tuples, n);
     wp.bottom = bin ? d.d_bottom_b : d.d_bottom;
-    wp.tuples = bin ? nullptr : static_cast<const float*>(d_tuples);
     wp.top4 = bin ? d.d_top_b : nullptr;
     wp.bins = bin ? static_cast<const uint8_t*>(d_tuples) : nullptr;
     wp.scores = d_scores;
     wp.labels = d_labels;
-    wp.n = n;
-    wp.F = d.shape.g.F();
-    wp.Dtop = d.shape.Dtop;
-    wp.top_stride = d.shape.top_stride;
-    wp.nb = d.shape.nb;
     // slots beyond S are never issued (DTPU.sv:519-531); groups past the last tree add exact zeros.  A multi-class walk
     // covers every group of every class (the engine refuses a run whose S*K*8 is below the largest class).
     const bool mc = d.shape.C >= 2;
     wp.groups = mc ? d.shape.C * d.shape.gpc : (uint32_t)std::min<uint64_t>((uint64_t)run.S * run.K, d.shape.Tpad / 8);
-    wp.classes = d.shape.C;
-    wp.groups_per_class = d.shape.gpc;
     wp.K = run.K;
-    wp.missing = bin ? 255u : run.missing;           // the bin of the missing pattern
-    wp.nwarps = (uint32_t)pl.nwarps;
-    wp.nstages = (uint32_t)pl.nstages;
+    if (bin) wp.missing = 255u;                      // the bin of the missing pattern
     wp.accumulate = accumulate ? 1u : 0u;
-    wp.fill_split = tune.fill ? 1u : 0u;      // DTE_TUNE fill=1: one bulk copy per tree instead of one per stage
-    wp.Lw = phased_level(d, tune, pl);
-    wp.tiles = 0;
-    cudaError_t rc;
-    if (pl.row < 0) {
-        const int threads = 128;
-        const unsigned long long blocks = (n + threads - 1) / threads;
-        if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
-        kGenericKernels[4 * bin + 2 * pl.wide + mc]<<<(unsigned)blocks, threads, 0, st>>>(wp);
-        rc = cudaGetLastError();
-    } else {
-        const size_t M = pl.tuples_per_cta();
-        const unsigned long long tiles = (n + M - 1) / M;
-        if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
-        wp.tiles = (uint32_t)tiles;
-        const int grid = (int)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count);
-        const WalkKernel k = kTileKernels[pl.row][4 * bin + 2 * pl.wide + mc](pl.thread_bound());
-        rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
-        if (rc != cudaSuccess) return rc;
-        k<<<grid, pl.threads(), pl.smem, st>>>(wp);
-        rc = cudaGetLastError();
-    }
-    if (rc == cudaSuccess) d.kernel_launches++;
-    return rc;
+    const int v = 4 * bin + 2 * pl.wide + mc;
+    return launch_plan(d, pl, pl.row < 0 ? kGenericKernels[v] : kTileKernels[pl.row][v](pl.thread_bound()), wp, n, st, why);
 }
 
 using LeafKernel = void (*)(LeafParams);
@@ -613,48 +624,15 @@ inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, i
     if (n == 0) return cudaSuccess;
     const Plan pl = make_plan(d, tune, want_variant);
     LeafParams lp = {};
-    WalkParams& wp = lp.w;
-    wp.top = d.d_top;
-    wp.bottom = d.d_bottom_id;
-    wp.tuples = static_cast<const float*>(d_tuples);
-    wp.n = n;
-    wp.F = d.shape.g.F();
-    wp.Dtop = d.shape.Dtop;
-    wp.top_stride = d.shape.top_stride;
-    wp.nb = d.shape.nb;
-    wp.groups = d.shape.Tpad / 8;
-    wp.K = 1;
-    wp.missing = run.missing;
-    wp.nwarps = (uint32_t)pl.nwarps;
-    wp.nstages = (uint32_t)pl.nstages;
-    wp.fill_split = tune.fill ? 1u : 0u;
-    wp.Lw = phased_level(d, tune, pl);
-    wp.classes = d.shape.C;
-    wp.groups_per_class = d.shape.gpc;
+    lp.w = walk_params(d, run, tune, pl, d_tuples, n);
+    lp.w.bottom = d.d_bottom_id;
+    lp.w.groups = d.shape.Tpad / 8;
+    lp.w.K = 1;
     lp.leaves = d_leaves;
     lp.T = d.shape.T;
     lp.first = d.shape.first % d.shape.C;
-    cudaError_t rc;
-    if (pl.row < 0) {
-        const int threads = 128;
-        const unsigned long long blocks = (n + threads - 1) / threads;
-        if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
-        kGenericLeafKernels[pl.wide]<<<(unsigned)blocks, threads, 0, st>>>(lp);
-        rc = cudaGetLastError();
-    } else {
-        const size_t M = pl.tuples_per_cta();
-        const unsigned long long tiles = (n + M - 1) / M;
-        if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
-        wp.tiles = (uint32_t)tiles;
-        const int grid = (int)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count);
-        const LeafKernel k = kTileLeafKernels[pl.row][pl.wide](pl.thread_bound());
-        rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
-        if (rc != cudaSuccess) return rc;
-        k<<<grid, pl.threads(), pl.smem, st>>>(lp);
-        rc = cudaGetLastError();
-    }
-    if (rc == cudaSuccess) d.kernel_launches++;
-    return rc;
+    return launch_plan(d, pl, pl.row < 0 ? kGenericLeafKernels[pl.wide] : kTileLeafKernels[pl.row][pl.wide](pl.thread_bound()), lp,
+                       n, st, why);
 }
 
 // bin: the binned walk's plan, named dt_walk_generic_u8 / dt_walk_tile_u8.  leaf: the leaf walk's plan (the fp32 plan),

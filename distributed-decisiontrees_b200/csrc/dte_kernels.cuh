@@ -374,9 +374,35 @@ __device__ __forceinline__ float bot_finish(const BotRec<WIDE>& r, uint32_t miss
 // MC = multi-class walk (WalkParams::classes >= 2); the MC = false instantiations are the single-class kernels.
 // BIN = binned walk: u8 bins and 4-byte tree tops (WalkParams::bins / top4).
 // ---------------------------------------------------------------------------------------------
+// The generic walks' top levels of tree t from global memory, returning the bottom record the walk reaches
+template <bool WIDE, bool BIN, class Feat>
+__device__ __forceinline__ BotRec<WIDE> generic_walk_top(const WalkParams& p, uint32_t t, Feat feat) {
+    constexpr int BV = WIDE ? 4 : 2;
+    uint32_t o = 0;
+    if constexpr (BIN) {
+        const char* tp = reinterpret_cast<const char*>(p.top4 + (size_t)t * p.top_stride);
+        for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+            const uint2 nd = make_uint2(ldg32_nc(tp + o), 0u);
+            const uint32_t xv = feat(node_fidx<true>(nd));
+            o = 2 * o + step_select(xv, node_thr<true>(nd), node_meta<true>(nd), p.missing, 4u, 8u);
+        }
+        o *= 2;                                          // as a byte offset into 8-byte records
+    } else {
+        const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
+        for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
+            uint2 nd = ldg64_nc(tp + o);
+            uint32_t xv = feat(nd.y & 0xFFFFu);
+            o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
+        }
+    }
+    const uint32_t j = (o >> 3) - (p.nb - 1);
+    BotRec<WIDE> br;
+    bot_load(br, p.bottom + ((size_t)t * p.nb + j) * BV);
+    return br;
+}
+
 template <bool WIDE, bool MC, bool BIN = false>
 __global__ void __launch_bounds__(128) dt_walk_generic(const WalkParams p) {
-    constexpr int BV = WIDE ? 4 : 2;
     unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
     const uint32_t* x = reinterpret_cast<const uint32_t*>(p.tuples) + i * p.F;
@@ -394,28 +420,7 @@ __global__ void __launch_bounds__(128) dt_walk_generic(const WalkParams p) {
         for (int k = 0; k < 8; ++k) l[k] = 0.0f;
 #pragma unroll 1
         for (int q = 0; q < 8; ++q) {
-            const uint32_t t = g * 8 + q;
-            uint32_t o = 0;
-            if constexpr (BIN) {
-                const char* tp = reinterpret_cast<const char*>(p.top4 + (size_t)t * p.top_stride);
-                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
-                    const uint2 nd = make_uint2(ldg32_nc(tp + o), 0u);
-                    const uint32_t xv = feat(node_fidx<true>(nd));
-                    o = 2 * o + step_select(xv, node_thr<true>(nd), node_meta<true>(nd), p.missing, 4u, 8u);
-                }
-                o *= 2;                                          // as a byte offset into 8-byte records
-            } else {
-                const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
-                for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
-                    uint2 nd = ldg64_nc(tp + o);
-                    uint32_t xv = feat(nd.y & 0xFFFFu);
-                    o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
-                }
-            }
-            const uint32_t j = (o >> 3) - (p.nb - 1);
-            BotRec<WIDE> br;
-            bot_load(br, p.bottom + ((size_t)t * p.nb + j) * BV);
-            float leaf = bot_finish<WIDE>(br, p.missing, feat);
+            float leaf = bot_finish<WIDE>(generic_walk_top<WIDE, BIN>(p, g * 8 + q, feat), p.missing, feat);
             // static register index for l[q]
 #pragma unroll
             for (int k = 0; k < 8; ++k) l[k] = (k == q) ? leaf : l[k];
@@ -480,7 +485,6 @@ __device__ __forceinline__ void stg_cells(uint16_t* a, const uint32_t (&c)[ILP])
 // The generic leaf walk: dt_walk_generic's walk over every resident tree slot, one thread per tuple.
 template <bool WIDE>
 __global__ void __launch_bounds__(128) dt_walk_generic_leaf(const LeafParams lp) {
-    constexpr int BV = WIDE ? 4 : 2;
     const WalkParams& p = lp.w;
     unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
@@ -492,17 +496,7 @@ __global__ void __launch_bounds__(128) dt_walk_generic_leaf(const LeafParams lp)
     for (uint32_t t = 0; t < slots; ++t) {
         const uint32_t c = leaf_column(lp, t);
         if (c >= lp.T) continue;
-        const char* tp = reinterpret_cast<const char*>(p.top + (size_t)t * p.top_stride);
-        uint32_t o = 0;
-        for (uint32_t lvl = 0; lvl < p.Dtop; ++lvl) {
-            uint2 nd = ldg64_nc(tp + o);
-            uint32_t xv = feat(nd.y & 0xFFFFu);
-            o = 2 * o + step_inc(xv, nd.x, nd.y, p.missing);
-        }
-        const uint32_t j = (o >> 3) - (p.nb - 1);
-        BotRec<WIDE> br;
-        bot_load(br, p.bottom + ((size_t)t * p.nb + j) * BV);
-        row[c] = (uint16_t)__float_as_uint(bot_finish<WIDE>(br, p.missing, feat));
+        row[c] = (uint16_t)__float_as_uint(bot_finish<WIDE>(generic_walk_top<WIDE, false>(p, t, feat), p.missing, feat));
     }
 }
 
@@ -546,6 +540,68 @@ __host__ __device__ constexpr int tile_warp_cap(int nt) { return nt / 32 - 1; }
 // NT of the instantiation that runs a plan of `threads` threads of a family with thread bound nt
 __host__ __device__ constexpr int tile_nt(int nt, int threads) { return (nt > 384 && threads <= 384) ? 384 : nt; }
 
+// Ring barriers of a staged walk, per stage: full and empty of part A, full and empty of part B (phased refill only)
+__device__ __forceinline__ void ring_init(const WalkParams& p, uint32_t sbase) {
+    if (threadIdx.x == 0) {
+        for (uint32_t s = 0; s < p.nstages; ++s) {
+            mbar_init(sbase + 8 * s, 1);                        // full (part A): producer's arrive + tx bytes
+            mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);   // empty (part A): one arrive per consumer warp
+            mbar_init(sbase + 8 * (2 * p.nstages + s), 1);      // full, part B  (phased refill only)
+            mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);   // empty, part B
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+}
+
+// The producer (lane 0 of the warp after the consumers): stream the SP tree tops of every step of every tile of this
+// CTA from `tops` through the ring.  A tree top is tree_bytes long, made of records of unitA / 2 bytes.
+// Phased refill (p.Lw set): a stage is refilled in two parts with their own barriers.
+//   part A = the first unitA*2^Lw bytes of every tree top (levels 0..Lw and the first record of level Lw+1), part B =
+//   the rest (75 % of the bytes).  The consumers hand part A back before their last level and part B after it, and
+//   need part B only from level iteration Lw on, so ONE stage overlaps copy and walk: B of step q+1 streams in under
+//   levels 0..Lw of step q+1, A of step q+1 under the last level + bottom records + leaf sums of step q.  Bulk copies
+//   move multiples of 16 bytes, and a binned part A of 8 << Lw bytes is none at Lw = 0, so the planner never phases a
+//   binned walk at Lw = 0.
+template <int SP>
+__device__ __forceinline__ void ring_produce(const WalkParams& p, uint32_t sbase, const void* tops, uint32_t tree_bytes,
+                                             uint32_t stage_bytes, uint32_t steps, uint32_t my_tiles, uint32_t unitA) {
+    const uint64_t total = (uint64_t)my_tiles * steps;
+    const char* src0 = reinterpret_cast<const char*>(tops);
+    uint32_t slot = 0, par = 1;                          // fresh barrier: parity-1 wait passes
+    uint32_t q = 0;
+    const bool phased = p.Lw != 0xFFFFFFFFu;
+    const uint32_t bytesA = phased ? (unitA << p.Lw) : tree_bytes;
+    const uint32_t bytesB = tree_bytes - bytesA;
+    for (uint64_t it = 0; it < total; ++it) {
+        const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
+        const char* src = src0 + (size_t)q * stage_bytes;
+        mbar_wait(sbase + 8 * (p.nstages + slot), par);
+        const uint32_t full = sbase + 8 * slot;
+        if (!phased) {
+            mbar_arrive_expect_tx(full, stage_bytes);
+            if (p.fill_split == 0) {
+                bulk_g2s(dst, src, stage_bytes, full);                 // the SP tree tops are contiguous: one copy
+            } else {
+#pragma unroll
+                for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
+            }
+        } else {
+            mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
+#pragma unroll
+            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
+            mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
+            const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
+            mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
+#pragma unroll
+            for (int c = 0; c < SP; ++c)
+                bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
+        }
+        if (++q == steps) q = 0;
+        if (++slot == p.nstages) { slot = 0; par ^= 1; }
+    }
+}
+
 // NT = thread bound of the instantiation.  Registers are allocated per SM sub-partition (16 K each), so the
 // per-thread limit is set by ceil(warps / 4): 9..12 warps -> 168 registers, 13..16 warps -> 128.  The planner
 // picks the 384-thread instantiation whenever the plan fits in 12 warps (cfg3: 5 tuple groups x 2 + producer).
@@ -569,60 +625,9 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
     const uint32_t my_tiles = (p.tiles > blockIdx.x) ? (p.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
     if (STAGED) {
-        if (threadIdx.x == 0) {
-            for (uint32_t s = 0; s < p.nstages; ++s) {
-                mbar_init(sbase + 8 * s, 1);                        // full (part A): producer's arrive + tx bytes
-                mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);   // empty (part A): one arrive per consumer warp
-                mbar_init(sbase + 8 * (2 * p.nstages + s), 1);      // full, part B  (phased refill only)
-                mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);   // empty, part B
-            }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (warp == p.nwarps) {
-            // ---------------- producer: stream tree tops through the ring ----------------
-            if (lane == 0) {
-                const uint64_t total = (uint64_t)my_tiles * steps;
-                const char* src0 = reinterpret_cast<const char*>(p.top);
-                uint32_t slot = 0, par = 1;                          // fresh barrier: parity-1 wait passes
-                uint32_t q = 0;
-                // Phased refill (p.Lw set): a stage is refilled in two parts with their own barriers.
-                //   part A = the first 8*2^(Lw+1) bytes of every tree top (levels 0..Lw and the first record of
-                //   level Lw+1), part B = the rest (75 % of the bytes).  The consumers hand part A back before
-                //   their last level and part B after it, and need part B only from level iteration Lw on, so
-                //   ONE stage overlaps copy and walk: B of step q+1 streams in under levels 0..Lw of step q+1,
-                //   A of step q+1 under the last level + bottom records + leaf sums of step q.
-                const bool phased = p.Lw != 0xFFFFFFFFu;
-                const uint32_t bytesA = phased ? (16u << p.Lw) : tree_bytes;
-                const uint32_t bytesB = tree_bytes - bytesA;
-                for (uint64_t it = 0; it < total; ++it) {
-                    const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
-                    const char* src = src0 + (size_t)q * stage_bytes;
-                    mbar_wait(sbase + 8 * (p.nstages + slot), par);
-                    const uint32_t full = sbase + 8 * slot;
-                    if (!phased) {
-                        mbar_arrive_expect_tx(full, stage_bytes);
-                        if (p.fill_split == 0) {
-                            bulk_g2s(dst, src, stage_bytes, full);                 // the SP tree tops are contiguous: one copy
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
-                        }
-                    } else {
-                        mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
-                        mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
-                        const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
-                        mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c)
-                            bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
-                    }
-                    if (++q == steps) q = 0;
-                    if (++slot == p.nstages) { slot = 0; par ^= 1; }
-                }
-            }
+        ring_init(p, sbase);
+        if (warp == p.nwarps) {                         // producer: stream tree tops through the ring
+            if (lane == 0) ring_produce<SP>(p, sbase, p.top, tree_bytes, stage_bytes, steps, my_tiles, 16u);
             return;
         }
     }
@@ -879,61 +884,9 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_u8(const WalkParams p) {
     const uint32_t my_tiles = (p.tiles > blockIdx.x) ? (p.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
     if (STAGED) {
-        if (threadIdx.x == 0) {
-            for (uint32_t s = 0; s < p.nstages; ++s) {
-                mbar_init(sbase + 8 * s, 1);                        // full (part A): producer's arrive + tx bytes
-                mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);   // empty (part A): one arrive per consumer warp
-                mbar_init(sbase + 8 * (2 * p.nstages + s), 1);      // full, part B  (phased refill only)
-                mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);   // empty, part B
-            }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (warp == p.nwarps) {
-            // ---------------- producer: stream tree tops through the ring ----------------
-            if (lane == 0) {
-                const uint64_t total = (uint64_t)my_tiles * steps;
-                const char* src0 = reinterpret_cast<const char*>(p.top4);
-                uint32_t slot = 0, par = 1;                          // fresh barrier: parity-1 wait passes
-                uint32_t q = 0;
-                // Phased refill (p.Lw set): a stage is refilled in two parts with their own barriers.
-                //   part A = the first 4*2^(Lw+1) bytes of every tree top (levels 0..Lw and the first record of
-                //   level Lw+1), part B = the rest (75 % of the bytes).  The consumers hand part A back before
-                //   their last level and part B after it, and need part B only from level iteration Lw on, so
-                //   ONE stage overlaps copy and walk: B of step q+1 streams in under levels 0..Lw of step q+1,
-                //   A of step q+1 under the last level + bottom records + leaf sums of step q.  Bulk copies move
-                //   multiples of 16 bytes, so the planner does not phase a binned walk at Lw = 0.
-                const bool phased = p.Lw != 0xFFFFFFFFu;
-                const uint32_t bytesA = phased ? (8u << p.Lw) : tree_bytes;
-                const uint32_t bytesB = tree_bytes - bytesA;
-                for (uint64_t it = 0; it < total; ++it) {
-                    const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
-                    const char* src = src0 + (size_t)q * stage_bytes;
-                    mbar_wait(sbase + 8 * (p.nstages + slot), par);
-                    const uint32_t full = sbase + 8 * slot;
-                    if (!phased) {
-                        mbar_arrive_expect_tx(full, stage_bytes);
-                        if (p.fill_split == 0) {
-                            bulk_g2s(dst, src, stage_bytes, full);                 // the SP tree tops are contiguous: one copy
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
-                        }
-                    } else {
-                        mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
-                        mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
-                        const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
-                        mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c)
-                            bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
-                    }
-                    if (++q == steps) q = 0;
-                    if (++slot == p.nstages) { slot = 0; par ^= 1; }
-                }
-            }
+        ring_init(p, sbase);
+        if (warp == p.nwarps) {                         // producer: stream tree tops through the ring
+            if (lane == 0) ring_produce<SP>(p, sbase, p.top4, tree_bytes, stage_bytes, steps, my_tiles, 8u);
             return;
         }
     }
@@ -1166,9 +1119,10 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_u8(const WalkParams p) {
     }
 }
 
-// The leaf tile walk (DESIGN.md §10): dt_walk_tile's producer warp, ring, phased refill, tuple tile and bottom-record
-// pipeline against the leaf-id records (WalkParams::bottom), with the tree8 reduction replaced by the stores of the
-// cells.  Every resident tree slot is walked (p.groups = all groups).  One class with T a multiple of ILP writes each
+// The leaf tile walk (DESIGN.md §10): the shared ring (ring_init, ring_produce) and dt_walk_tile's tuple tile, top walk
+// and bottom-record pipeline against the leaf-id records (WalkParams::bottom), with the tree8 reduction replaced by the
+// stores of the cells.  The tile walks' remaining pieces are written out per kernel: shared, they change the kernels'
+// SASS (DESIGN.md §9, shared pieces).  Every resident tree slot is walked (p.groups = all groups).  One class with T a multiple of ILP writes each
 // warp's ILP cells of a row as one aligned 2*ILP-byte store; otherwise each cell is a 2-byte store to leaf_column().
 // A separate kernel rather than a flag on dt_walk_tile, for the reason dt_walk_tile_u8 gives.  Shared memory is laid
 // out as dt_walk_tile's (the exchange area is unused), so a leaf plan is the fp32 plan of the same ensemble.
@@ -1192,54 +1146,9 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_leaf(const LeafParams lp) 
     const uint32_t my_tiles = (p.tiles > blockIdx.x) ? (p.tiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
     if (STAGED) {
-        if (threadIdx.x == 0) {
-            for (uint32_t s = 0; s < p.nstages; ++s) {
-                mbar_init(sbase + 8 * s, 1);
-                mbar_init(sbase + 8 * (p.nstages + s), p.nwarps);
-                mbar_init(sbase + 8 * (2 * p.nstages + s), 1);
-                mbar_init(sbase + 8 * (3 * p.nstages + s), p.nwarps);
-            }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (warp == p.nwarps) {
-            // producer: dt_walk_tile's, unchanged
-            if (lane == 0) {
-                const uint64_t total = (uint64_t)my_tiles * steps;
-                const char* src0 = reinterpret_cast<const char*>(p.top);
-                uint32_t slot = 0, par = 1;
-                uint32_t q = 0;
-                const bool phased = p.Lw != 0xFFFFFFFFu;
-                const uint32_t bytesA = phased ? (16u << p.Lw) : tree_bytes;
-                const uint32_t bytesB = tree_bytes - bytesA;
-                for (uint64_t it = 0; it < total; ++it) {
-                    const uint32_t dst = sbase + kHdrBytes + slot * stage_bytes;
-                    const char* src = src0 + (size_t)q * stage_bytes;
-                    mbar_wait(sbase + 8 * (p.nstages + slot), par);
-                    const uint32_t full = sbase + 8 * slot;
-                    if (!phased) {
-                        mbar_arrive_expect_tx(full, stage_bytes);
-                        if (p.fill_split == 0) {
-                            bulk_g2s(dst, src, stage_bytes, full);
-                        } else {
-#pragma unroll
-                            for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
-                        }
-                    } else {
-                        mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, bytesA, full);
-                        mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
-                        const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
-                        mbar_arrive_expect_tx(fullB, (uint32_t)SP * bytesB);
-#pragma unroll
-                        for (int c = 0; c < SP; ++c)
-                            bulk_g2s(dst + c * tree_bytes + bytesA, src + (size_t)c * tree_bytes + bytesA, bytesB, fullB);
-                    }
-                    if (++q == steps) q = 0;
-                    if (++slot == p.nstages) { slot = 0; par ^= 1; }
-                }
-            }
+        ring_init(p, sbase);
+        if (warp == p.nwarps) {                         // producer: stream tree tops through the ring
+            if (lane == 0) ring_produce<SP>(p, sbase, p.top, tree_bytes, stage_bytes, steps, my_tiles, 16u);
             return;
         }
     }
@@ -1314,7 +1223,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile_leaf(const LeafParams lp) 
             }
         };
 
-        // dt_walk_tile's walk_top, unchanged
+        // dt_walk_tile's walk_top
         auto walk_top = [&](uint32_t q, BotRec<WIDE> (&dst)[ILP]) {
             const uint32_t t0 = q * SP + sub * ILP;
             uint32_t o[ILP];
