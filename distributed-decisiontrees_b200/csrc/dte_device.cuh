@@ -22,6 +22,10 @@ constexpr int kNumSlots = 3;          // landing slots per device: H2D of i+1, w
 
 enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED = 3 };
 
+// What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), or the leaf cell every
+// tree reaches (DESIGN.md §10)
+enum class Walk { Fp32, Binned, Leaf };
+
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
 //  phased: 0 off / k>=1 on with part A ending k levels earlier, fill=1: one bulk copy per tree,
@@ -67,7 +71,7 @@ struct Plan {               // how the next walk will be launched
     int row = -1;           // kTileFamilies row of a tile plan; -1: dt_walk_generic
     int nstages = 0, nwarps = 0;                       // nwarps = consumer warps = groups * pair
     bool wide = false;
-    bool bin = false;       // binned walk (u8 tile, 4-byte tree tops)
+    Walk walk = Walk::Fp32;
     size_t smem = 0;
     const TileFamily& fam() const { return kTileFamilies[row]; }
     int variant() const { return row < 0 ? KERNEL_GENERIC : fam().staged ? KERNEL_TILE_STAGED : KERNEL_TILE; }
@@ -178,11 +182,11 @@ inline int bin_edges(const Geom& g, const unsigned char* wl, size_t n_wl, const 
 // Packs trees [first, first + count) of the streams; `first` is the global stream index of the first packed tree, so
 // with `classes` = C >= 2 tree first + t belongs to class (first + t) % C.  The trees are then stored class-major:
 // class c occupies tree slots [c * gpc * 8, (c + 1) * gpc * 8) in stream order, gpc = ceil(largest class / 8).
-// With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well, and with `leaf` the
+// With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well, and with `id_layout` the
 // leaf-id layout.  Returns 0 or a negative dte_status; *msg receives the reason.
 inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl,
                          uint32_t first, uint32_t count, uint32_t classes, PackedEnsemble& out, std::string& msg,
-                         const BinEdges* bins = nullptr, bool leaf = false) {
+                         const BinEdges* bins = nullptr, bool id_layout = false) {
     char buf[256];
     if (classes < 1) { msg = "class count 0"; return -1; }
     if (n_wl % g.w_cls) {
@@ -253,7 +257,7 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     out.bottom.assign((size_t)Tpad * nb * BV, make_uint4(0, 0, 0, 0));
     out.top_b.assign(bins ? (size_t)Tpad * top_stride : 0, 0u);
     out.bottom_b.assign(bins ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
-    out.bottom_id.assign(leaf ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
+    out.bottom_id.assign(id_layout ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
     std::vector<uint32_t> Wk((2u << Dk) - 1);
     std::vector<uint16_t> Fk((1u << Dk) - 1);
     std::vector<uint32_t> cell((2u << Dk) - 1);        // stream cell each cell of the packed heap stands for
@@ -313,7 +317,7 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                 bp[j * 2 + 1] = leaves;
             }
         }
-        if (leaf) {
+        if (id_layout) {
             uint4* bi = out.bottom_id.data() + (size_t)slot_of[t] * nb * BV;
             std::copy(bp, bp + (size_t)nb * BV, bi);
             for (uint32_t j = 0; j < nb; ++j) {
@@ -381,8 +385,8 @@ struct Dev {
     uint32_t* d_bin_edges = nullptr;
     // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
     uint4* d_bottom_id = nullptr;
-    bool run_bin = false;             // the landing slots carry u8 bins (F bytes per tuple) during dte_infer_host_binned
-    size_t run_tuple_bytes() const { return run_bin ? shape.g.F() : shape.g.tuple_bytes(); }
+    Walk walk = Walk::Fp32;           // the walk the landing slots feed: binned calls land u8 bins (F bytes per tuple)
+    size_t run_tuple_bytes() const { return walk == Walk::Binned ? shape.g.F() : shape.g.tuple_bytes(); }
 
     // ---- landing slots ----
     Slot slot[kNumSlots];
@@ -396,7 +400,6 @@ struct Dev {
     uint8_t* sink_lb = nullptr;
     // leaf calls (dte_infer_host_leaves): the walk writes cells into Slot::d_leaf and its rows land in sink_leaf, whose
     // rows are leaf_pitch cells apart (this device's columns of the caller's rows)
-    bool run_leaf = false;
     uint16_t* sink_leaf = nullptr;
     size_t leaf_pitch = 0;
     size_t leaf_slot_cells = 0;       // cells allocated per Slot::d_leaf
@@ -419,9 +422,10 @@ struct Dev {
 };
 
 // ---- launch planning ---------------------------------------------------------------------------
-// bin: the binned walk's 4-byte tree tops and one byte per feature in the tile
-inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride, bool bin = false) {
-    return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * (bin ? 4 : 8) + (size_t)F * 32 * groups * (bin ? 1 : 4);
+// the binned walk stages 4-byte tree tops and holds one byte per feature in the tile
+inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride, Walk w = Walk::Fp32) {
+    const size_t top = w == Walk::Binned ? 4 : 8, feature = w == Walk::Binned ? 1 : 4;
+    return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * top + (size_t)F * 32 * groups * feature;
 }
 
 // The family a DTE_TUNE pin selects: the row with this ilp and pair, else the first row with this pair, else the same
@@ -439,29 +443,30 @@ inline int tile_row(int ilp, int pair, bool staged) {
 
 // Tuple groups (32 tuples, F*128 B of shared memory each, F*32 B binned) of family f that fit next to a ring of nstages
 // stages, and at most `warps` consumer warps when warps > 0.
-inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps, bool bin = false) {
+inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps, Walk w = Walk::Fp32) {
     if (f.staged && d.shape.Dtop < 3) return 0;        // below that there is nothing worth staging
     const uint32_t F = d.shape.g.F();
     const size_t budget = (size_t)d.smem_optin;
-    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride, bin);
+    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride, w);
     if (fixed >= budget) return 0;
-    int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * (bin ? 32 : 128)));
+    int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * (w == Walk::Binned ? 32 : 128)));
     if (warps) g = std::min(g, std::max(1, warps / f.pair));
     return g;
 }
 
-// bin: plan the binned walk of the resident binned layout (same candidates and rules, binned tile and top sizes)
-inline Plan make_plan(const Dev& d, const Tune& tune, int want, bool bin = false) {
+// The plan of a walk of kind w on the resident ensemble.  Every kind has the same candidates and rules; a binned plan
+// sizes the binned tile and tops, a leaf plan is the fp32 plan.
+inline Plan make_plan(const Dev& d, const Tune& tune, int want, Walk w = Walk::Fp32) {
     auto tile_plan = [&](int row, int nstages, int groups) {
         const TileFamily& f = kTileFamilies[row];
         Plan p;
-        p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide; p.bin = bin;
-        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride, bin);
+        p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide; p.walk = w;
+        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride, w);
         return p;
     };
     Plan generic, staged;
     generic.wide = d.shape.wide;
-    generic.bin = bin;
+    generic.walk = w;
     // staged candidates {trees per warp, warps per tuple group, ring stages}; the candidate that fits with the most
     // walks in flight wins (dte_autotune times the alternatives on the resident ensemble).
     const int cand[6][3] = {{4, 2, 1}, {2, 4, 1}, {8, 1, 1}, {8, 1, 2}, {4, 1, 2}, {4, 1, 1}};
@@ -470,13 +475,13 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want, bool bin = false
         const int row = tile_row(tune.ilp ? tune.ilp : c[0], tune.pair ? tune.pair : c[1], true);
         const int ilp = kTileFamilies[row].ilp, pair = kTileFamilies[row].pair;
         const int st = std::max(1, std::min(tune.stages ? tune.stages : c[2], 4));
-        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps, bin);
+        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps, w);
         const int score = g * pair * ilp * 8 + (pair == 2 ? 4 : 0) - (pair == 4 ? 4 : 0) + st;
         if (g >= 1 && score > best) { best = score; staged = tile_plan(row, st, g); }
         if (tune.ilp && tune.stages && tune.pair) break;
     }
     const int tile_r = tile_row(tune.ilp, 1, false);
-    const int tile_g = tile_groups(d, kTileFamilies[tile_r], 0, tune.warps, bin);
+    const int tile_g = tile_groups(d, kTileFamilies[tile_r], 0, tune.warps, w);
     const Plan tile = tile_g >= 1 ? tile_plan(tile_r, 0, tile_g) : generic;
     if (want == KERNEL_TILE_STAGED && staged.nwarps >= 1) return staged;
     if (want == KERNEL_TILE && tile.nwarps >= 1) return tile;
@@ -496,7 +501,7 @@ inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
     // part A = levels 0..Lw; DTE_TUNE phased=k moves the split k-1 levels further up (smaller part A)
     const uint32_t up = tune.phased > 1 ? (uint32_t)tune.phased - 1 : 0;
     // a binned part A of 8 << Lw bytes is no whole number of 16-byte bulk-copy units at Lw = 0
-    const bool fits = d.shape.Dtop >= 3 + up + (pl.bin ? 1 : 0);
+    const bool fits = d.shape.Dtop >= 3 + up + (pl.walk == Walk::Binned ? 1 : 0);
     return (phased && fits && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
@@ -573,18 +578,19 @@ inline cudaError_t launch_plan(Dev& d, const Plan& pl, void (*kernel)(Params), P
 }
 
 // Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
-// `run`; the layout comes from the resident ensemble.  bin: d_tuples are u8 bins [n][F], walked against the resident
-// binned layout.  Returns a cudaError_t.
+// `run`; the layout comes from the resident ensemble.  A Walk::Binned walk reads u8 bins [n][F] from d_tuples against
+// the resident binned layout.  Returns a cudaError_t.
 inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int want_variant, const void* d_tuples, size_t n,
                                float* d_scores, uint8_t* d_labels, cudaStream_t st, bool accumulate, const char** why,
-                               bool bin = false) {
+                               Walk w = Walk::Fp32) {
     *why = nullptr;
     if (n == 0) return cudaSuccess;
-    const Plan pl = make_plan(d, tune, want_variant, bin);
-    WalkParams wp = walk_params(d, run, tune, pl, bin ? nullptr : d_tuples, n);
-    wp.bottom = bin ? d.d_bottom_b : d.d_bottom;
-    wp.top4 = bin ? d.d_top_b : nullptr;
-    wp.bins = bin ? static_cast<const uint8_t*>(d_tuples) : nullptr;
+    const bool u8 = w == Walk::Binned;
+    const Plan pl = make_plan(d, tune, want_variant, w);
+    WalkParams wp = walk_params(d, run, tune, pl, u8 ? nullptr : d_tuples, n);
+    wp.bottom = u8 ? d.d_bottom_b : d.d_bottom;
+    wp.top4 = u8 ? d.d_top_b : nullptr;
+    wp.bins = u8 ? static_cast<const uint8_t*>(d_tuples) : nullptr;
     wp.scores = d_scores;
     wp.labels = d_labels;
     // slots beyond S are never issued (DTPU.sv:519-531); groups past the last tree add exact zeros.  A multi-class walk
@@ -592,9 +598,9 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     const bool mc = d.shape.C >= 2;
     wp.groups = mc ? d.shape.C * d.shape.gpc : (uint32_t)std::min<uint64_t>((uint64_t)run.S * run.K, d.shape.Tpad / 8);
     wp.K = run.K;
-    if (bin) wp.missing = 255u;                      // the bin of the missing pattern
+    if (u8) wp.missing = 255u;                       // the bin of the missing pattern
     wp.accumulate = accumulate ? 1u : 0u;
-    const int v = 4 * bin + 2 * pl.wide + mc;
+    const int v = 4 * u8 + 2 * pl.wide + mc;
     return launch_plan(d, pl, pl.row < 0 ? kGenericKernels[v] : kTileKernels[pl.row][v](pl.thread_bound()), wp, n, st, why);
 }
 
@@ -622,7 +628,7 @@ inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, i
                                     uint16_t* d_leaves, cudaStream_t st, const char** why) {
     *why = nullptr;
     if (n == 0) return cudaSuccess;
-    const Plan pl = make_plan(d, tune, want_variant);
+    const Plan pl = make_plan(d, tune, want_variant, Walk::Leaf);
     LeafParams lp = {};
     lp.w = walk_params(d, run, tune, pl, d_tuples, n);
     lp.w.bottom = d.d_bottom_id;
@@ -635,11 +641,10 @@ inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, i
                        n, st, why);
 }
 
-// bin: the binned walk's plan, named dt_walk_generic_u8 / dt_walk_tile_u8.  leaf: the leaf walk's plan (the fp32 plan),
-// named dt_walk_generic_leaf / dt_walk_tile_leaf
-inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len, bool bin = false, bool leaf = false) {
-    const Plan pl = make_plan(d, tune, want, bin);
-    const char* sfx = bin ? "_u8" : leaf ? "_leaf" : "";
+// The plan of a walk of kind w, named dt_walk_generic / dt_walk_tile with the kind's suffix: _u8 binned, _leaf leaf
+inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len, Walk w = Walk::Fp32) {
+    const Plan pl = make_plan(d, tune, want, w);
+    const char* sfx = w == Walk::Binned ? "_u8" : w == Walk::Leaf ? "_leaf" : "";
     if (pl.row < 0) {
         snprintf(buf, len, "dt_walk_generic%s<%d>", sfx, pl.wide ? 1 : 0);
     } else {

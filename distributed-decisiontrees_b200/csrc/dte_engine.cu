@@ -269,11 +269,19 @@ int decide_partition(dte_engine* e, const Geom& g) {
     return DTE_OK;
 }
 
+// Why device d cannot run a walk of kind w: the layout that walk reads is not resident (nullptr: it is).
+const char* missing_layout(const Dev& d, Walk w) {
+    switch (w) {
+        case Walk::Binned: return d.d_top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
+        case Walk::Leaf: return d.d_bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
+        default: return d.d_top ? nullptr : "no ensemble loaded";
+    }
+}
+
 // A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
-// layout and the validated feature-index range; K, S and the missing pattern are free to change).  bin: the run walks
-// u8 bins and needs the binned layout as well.  leaf: the run is a leaf walk, which needs the leaf-id layout and walks
-// every tree whatever K and S say.
-int check_resident(dte_engine* e, const Geom& g, bool bin = false, bool leaf = false) {
+// layout and the validated feature-index range; K, S and the missing pattern are free to change), and needs the layout
+// of its walk.  A leaf walk walks every tree whatever K and S say.
+int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
     if (e->multi() && e->placed) {
         if (e->part != *e->placed)
             return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
@@ -282,15 +290,13 @@ int check_resident(dte_engine* e, const Geom& g, bool bin = false, bool leaf = f
             return fail(e, DTE_ERR_CONFIG, "devices_list (registers 208-210) changed since the tree chunks were programmed: the ring order of the partial sums would change");
     }
     for (Dev& d : e->devs) {
-        if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
-        if (bin && !d.d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
-        if (leaf && !d.d_bottom_id)
-            return fail(e, DTE_ERR_STATE, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1");
+        for (Walk need : {Walk::Fp32, w})            // the ensemble, then the layout of the walk
+            if (const char* why = missing_layout(d, need)) return fail(e, DTE_ERR_STATE, "%s", why);
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
                         g.F(), g.D, d.shape.g.F(), d.shape.g.D);
         // a multi-class walk covers every tree: the slots must hold the largest class (no silent truncation per class)
-        if (!leaf && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
+        if (w != Walk::Leaf && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
             return fail(e, DTE_ERR_CONFIG, "reg 205: S=%u x K=%u x 8 slots hold fewer trees than the largest of the %u classes (%u trees): "
                         "a multi-class run needs S >= %u", g.S, g.K, d.shape.C, d.shape.cls_max, (d.shape.cls_max + 8 * g.K - 1) / (8 * g.K));
     }
@@ -489,11 +495,16 @@ int poll_dev(dte_engine* e, Dev& d, uint64_t need) {
     return DTE_OK;
 }
 
-// D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink.  A result is
-// slot_C score words (the direct sink only: the line stream's pinned ring always carries one word per tuple).
+// D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink.  A leaf walk's
+// result is shape.T cells, its rows leaf_pitch cells apart on the host; a score is slot_C words (the direct sink only:
+// the line stream's pinned ring always carries one word per tuple).
 int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, bool labels) {
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_d2h, s.ev_walk, 0));
-    if (d.sink_sc) {
+    if (d.walk == Walk::Leaf) {
+        const size_t T = d.shape.T;
+        CUDA_TRY(e, cudaMemcpy2DAsync(d.sink_leaf, d.leaf_pitch * 2, s.d_leaf + from * T, T * 2, T * 2, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
+        d.sink_leaf += cnt * d.leaf_pitch;
+    } else if (d.sink_sc) {
         const size_t C = d.slot_C;
         CUDA_TRY(e, cudaMemcpyAsync(d.sink_sc, s.d_sc + from * C, cnt * C * 4, cudaMemcpyDeviceToHost, d.s_d2h));
         d.sink_sc += cnt * C;
@@ -517,35 +528,17 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
     return DTE_OK;
 }
 
-// D2H of the cells of `cnt` tuples of slot s starting at slot-local tuple `from` into the device's leaf sink: rows of
-// shape.T cells, leaf_pitch cells apart on the host.
-int enqueue_leaves(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt) {
-    const size_t T = d.shape.T;
-    CUDA_TRY(e, cudaStreamWaitEvent(d.s_d2h, s.ev_walk, 0));
-    CUDA_TRY(e, cudaMemcpy2DAsync(d.sink_leaf, d.leaf_pitch * 2, s.d_leaf + from * T, T * 2, T * 2, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
-    d.sink_leaf += cnt * d.leaf_pitch;
-    CUDA_TRY(e, cudaEventRecord(s.ev_d2h, d.s_d2h));
-    cudaEvent_t ev = get_event(d);
-    CUDA_TRY(e, cudaEventRecord(ev, d.s_d2h));
-    d.res_enq += cnt;
-    d.pend.push_back({ev, d.res_enq});
-    return DTE_OK;
-}
-
-int leaf_walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, uint16_t* leaves, cudaStream_t st) {
+// Launch the walk of kind w over n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.  `out`
+// receives the scores [n][C] (labels too when given), or for a leaf walk the cells [n][T].
+int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, void* out, uint8_t* labels, cudaStream_t st,
+                 bool accumulate = false) {
     const char* why = nullptr;
-    const cudaError_t rc = launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, leaves, st, &why);
-    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "leaf walk launch failed: %s", why ? why : cudaGetErrorString(rc));
-    return DTE_OK;
-}
-
-// Launch the walk of n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.
-// bin: `tuples` are u8 bins walked against the binned layout.
-int walk_or_fail(dte_engine* e, Dev& d, const void* tuples, size_t n, float* scores, uint8_t* labels, cudaStream_t st,
-                 bool accumulate, bool bin) {
-    const char* why = nullptr;
-    const cudaError_t rc = launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, scores, labels, st, accumulate, &why, bin);
-    if (rc != cudaSuccess) return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "walk kernel launch failed: %s", why ? why : cudaGetErrorString(rc));
+    const cudaError_t rc =
+        w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
+                        : launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
+    if (rc != cudaSuccess)
+        return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s", w == Walk::Leaf ? "leaf walk" : "walk kernel",
+                    why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
 
@@ -561,17 +554,10 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaEventRecord(s.ev_land, d.s_h2d));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
-    CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // score buffer of this slot drained
-    if (d.run_leaf) {
-        TRY(leaf_walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_leaf + s.walked * d.shape.T, d.s_main));
-        CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
-        TRY(enqueue_leaves(e, d, s, s.walked, cnt));
-        s.walked = whole;
-        e->tuples_out += cnt;
-        return DTE_OK;
-    }
+    CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // result buffer of this slot drained
     const bool labels = d.sink_sc && d.sink_lb;
-    TRY(walk_or_fail(e, d, s.d_tup + s.walked * tb, cnt, s.d_sc + s.walked * d.slot_C, labels ? s.d_lb + s.walked : nullptr, d.s_main, false, d.run_bin));
+    void* out = d.walk == Walk::Leaf ? (void*)(s.d_leaf + s.walked * d.shape.T) : (void*)(s.d_sc + s.walked * d.slot_C);
+    TRY(walk_or_fail(e, d, d.walk, s.d_tup + s.walked * tb, cnt, out, labels ? s.d_lb + s.walked : nullptr, d.s_main));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
     TRY(enqueue_results(e, d, s, s.walked, cnt, labels));
     s.walked = whole;
@@ -730,49 +716,47 @@ int submit_group(dte_engine* e, int b) {
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         CUDA_TRY(e, cudaEventRecord(d.slot[b].ev_land, d.s_h2d));
     }
-    if (h.run_leaf) {
-        // every ring position walks every tuple for its own trees and lands its block in its columns: no combine
-        for (Dev& d : e->devs) {
-            Slot& s = d.slot[b];
-            CUDA_TRY(e, cudaSetDevice(d.ordinal));
-            for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));
-            CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));
-            TRY(leaf_walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_leaf + walked * d.shape.T, d.s_main));
-            CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
-            TRY(enqueue_leaves(e, d, s, walked, cnt));
-            s.walked = whole;
-        }
-        e->tuples_out += cnt;
-        return DTE_OK;
-    }
+    // every ring position walks every tuple for its own trees: a leaf walk lands its cells in its own columns, a score
+    // walk leaves partials that are ring-combined on the host device
+    const bool cells = h.walk == Walk::Leaf;
     for (Dev& d : e->devs) {
         Slot& s = d.slot[b];
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));   // every piece has landed here
-        CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, h.slot[b].ev_comb, 0));    // the previous combine is done with our partials
-        TRY(walk_or_fail(e, d, s.d_tup + walked * tb, cnt, s.d_part + walked * C, nullptr, d.s_main, false, d.run_bin));
+        // the cells of this slot have been copied out / the previous combine is done with our partials
+        CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, cells ? s.ev_d2h : h.slot[b].ev_comb, 0));
+        void* out = cells ? (void*)(s.d_leaf + walked * d.shape.T) : (void*)(s.d_part + walked * C);
+        TRY(walk_or_fail(e, d, h.walk, s.d_tup + walked * tb, cnt, out, nullptr, d.s_main));
         CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
         s.walked = whole;
     }
-    Slot& hs = h.slot[b];
-    const bool labels = h.sink_sc && h.sink_lb;
-    CUDA_TRY(e, cudaSetDevice(h.ordinal));
-    CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, hs.ev_d2h, 0));
-    if (!e->combine_nccl) {
-        for (Dev& d : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, d.slot[b].ev_walk, 0));
-        RingParts parts;
-        for (size_t r = 0; r < G; ++r) parts.p[r] = e->devs[(size_t)e->pos2dev[r]].slot[b].d_part + walked * C;   // ring order, host first
-        // word-wise ring: each class's score is the ring sum of that class's partials; C >= 2 labels come after it
-        const bool ring_labels = labels && C == 1;
-        CUDA_TRY(e, launch_ring_combine(parts, (int)G, hs.d_sc + walked * C, ring_labels ? hs.d_lb + walked : nullptr, cnt * C, h.sm_count, h.s_main));
-        h.kernel_launches++;
-        if (labels && C >= 2) CUDA_TRY(e, launch_labels(hs.d_sc + walked * C, hs.d_lb + walked, cnt, (uint32_t)C, h.s_main));
+    if (cells) {
+        for (Dev& d : e->devs) {
+            CUDA_TRY(e, cudaSetDevice(d.ordinal));
+            TRY(enqueue_results(e, d, d.slot[b], walked, cnt, false));
+        }
     } else {
-        TRY(nccl_combine(e, b, walked, cnt, labels));
+        Slot& hs = h.slot[b];
+        const bool labels = h.sink_sc && h.sink_lb;
+        CUDA_TRY(e, cudaSetDevice(h.ordinal));
+        CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, hs.ev_d2h, 0));
+        if (!e->combine_nccl) {
+            for (Dev& d : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, d.slot[b].ev_walk, 0));
+            RingParts parts;
+            for (size_t r = 0; r < G; ++r) parts.p[r] = e->devs[(size_t)e->pos2dev[r]].slot[b].d_part + walked * C;   // ring order, host first
+            // word-wise ring: each class's score is the ring sum of that class's partials; C >= 2 labels come after it
+            const bool ring_labels = labels && C == 1;
+            CUDA_TRY(e, launch_ring_combine(parts, (int)G, hs.d_sc + walked * C, ring_labels ? hs.d_lb + walked : nullptr, cnt * C,
+                                            h.sm_count, h.s_main));
+            h.kernel_launches++;
+            if (labels && C >= 2) CUDA_TRY(e, launch_labels(hs.d_sc + walked * C, hs.d_lb + walked, cnt, (uint32_t)C, h.s_main));
+        } else {
+            TRY(nccl_combine(e, b, walked, cnt, labels));
+        }
+        CUDA_TRY(e, cudaEventRecord(hs.ev_comb, h.s_main));
+        CUDA_TRY(e, cudaEventRecord(hs.ev_walk, h.s_main));       // results of this slot are final after the combine
+        TRY(enqueue_results(e, h, hs, walked, cnt, labels));
     }
-    CUDA_TRY(e, cudaEventRecord(hs.ev_comb, h.s_main));
-    CUDA_TRY(e, cudaEventRecord(hs.ev_walk, h.s_main));           // results of this slot are final after the combine
-    TRY(enqueue_results(e, h, hs, walked, cnt, labels));
     e->tuples_out += cnt;
     return DTE_OK;
 }
@@ -892,59 +876,28 @@ uint64_t global_prefix(const dte_engine* e, bool completed) {
     return cnt(host_dev(e));
 }
 
-int prepare_data_phase(dte_engine* e, bool need_ring) {
+// landing slots and result queue of a line-stream run
+int prepare_data_phase(dte_engine* e) {
     const uint32_t F = e->g.F();
     const size_t cap = default_chunk(e, F);
     for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
-    if (need_ring) {
-        // result queue: reg 207 says how many result lines the run produces; bounded either way
-        uint64_t lines = e->opt_queue_lines ? e->opt_queue_lines : (e->regs[7] & 0xFFFFFFFFull) + 64;
-        if (!e->opt_queue_lines) lines = std::max<uint64_t>(lines, 1u << 18);
-        lines = std::min<uint64_t>(std::max<uint64_t>(lines, 16), 1u << 26);
-        e->ring_cap = lines * 4;
-        const uint64_t G = e->devs.size();
-        for (Dev& d : e->devs) {
-            const bool has_results = e->part != Part::Chunked || &d == &host_dev(e);
-            if (!has_results) continue;
-            const uint64_t per = e->part == Part::Dealt ? e->ring_cap / G + 2 * dealing(e).bt + cap : e->ring_cap + cap;
-            TRY(ensure_ring(e, d, per));
-        }
+    // result queue: reg 207 says how many result lines the run produces; bounded either way
+    uint64_t lines = e->opt_queue_lines ? e->opt_queue_lines : (e->regs[7] & 0xFFFFFFFFull) + 64;
+    if (!e->opt_queue_lines) lines = std::max<uint64_t>(lines, 1u << 18);
+    lines = std::min<uint64_t>(std::max<uint64_t>(lines, 16), 1u << 26);
+    e->ring_cap = lines * 4;
+    const uint64_t G = e->devs.size();
+    for (Dev& d : e->devs) {
+        const bool has_results = e->part != Part::Chunked || &d == &host_dev(e);
+        if (!has_results) continue;
+        const uint64_t per = e->part == Part::Dealt ? e->ring_cap / G + 2 * dealing(e).bt + cap : e->ring_cap + cap;
+        TRY(ensure_ring(e, d, per));
     }
     return DTE_OK;
 }
 
-int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
-                   uint16_t* h_leaves = nullptr);
-
-// Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
-// score buffer as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every
-// chunk broadcast to all of them (tree chunks + ring combine).  bin: h_tuples are u8 bins [n][F] (F bytes per tuple
-// through the same landing slots), walked against the binned layout.
-int infer_host(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels, bool bin) {
-    Geom g;
-    TRY(decode_geom(e, g));
-    if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "infer_host while the tree stream is being received");
-    if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
-    TRY(drain_all(e));
-    if (e->multi()) TRY(decide_partition(e, g));
-    TRY(check_resident(e, g, bin));
-    if (n == 0) return DTE_OK;
-    e->g = g;
-    for (Dev& d : e->devs)                           // every chunk of this call starts on a fresh landing buffer
-        if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
-    TRY(prepare_data_phase(e, false));
-    if (!bin) return infer_host_run(e, h_tuples, n, h_scores, h_labels);
-    for (Dev& d : e->devs) d.run_bin = true;
-    const int rc = infer_host_run(e, h_tuples, n, h_scores, h_labels);
-    for (Dev& d : e->devs) {                         // the slots carry fp32 tuples again: leave none partly filled
-        if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
-        d.run_bin = false;
-    }
-    return rc;
-}
-
 // The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.
-// h_leaves (leaf calls, Dev::run_leaf set): [n][columns] cells, every device's rows landing in its own columns.
+// h_leaves (leaf calls): [n][columns] cells, every device's rows landing in its own columns.
 int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
                    uint16_t* h_leaves) {
     const size_t tb = e->devs[0].run_tuple_bytes();
@@ -1030,33 +983,41 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
     return DTE_OK;
 }
 
-// dte_infer_host_leaves: infer_host's landing pipeline with the leaf walk; no scores, no labels.
-int infer_host_leaves(dte_engine* e, const unsigned char* h_tuples, size_t n, uint16_t* h_leaves) {
+// Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
+// buffers as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every chunk
+// broadcast to all of them (tree chunks + ring combine).  A binned walk lands u8 bins [n][F] (F bytes per tuple through
+// the same landing slots); a leaf walk returns cells into h_leaves, no scores, no labels.  `what` names the call.
+int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_tuples, size_t n, float* h_scores,
+               uint8_t* h_labels, uint16_t* h_leaves) {
     Geom g;
     TRY(decode_geom(e, g));
-    if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "infer_host_leaves while the tree stream is being received");
+    if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "%s while the tree stream is being received", what);
     if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
-    TRY(check_resident(e, g, false, true));
+    TRY(check_resident(e, g, w));
     if (n == 0) return DTE_OK;
     e->g = g;
-    for (Dev& d : e->devs)
+    for (Dev& d : e->devs)                           // every chunk of this call starts on a fresh landing buffer
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
-    // The landing slots hold default_chunk tuples; their cells (2T bytes per tuple) may take at most twice the tuple
-    // budget, so a many-tree, few-feature ensemble lands fewer tuples per slot instead of allocating GiBs of cells.
     const uint32_t F = g.F();
-    uint32_t tmax = 1;
-    for (const Dev& d : e->devs) tmax = std::max(tmax, d.shape.T);
-    const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
-    const size_t cap = std::min(default_chunk(e, F), std::max<size_t>(4, budget / (2 * (size_t)tmax)) & ~(size_t)3);
+    size_t cap = default_chunk(e, F);
+    if (w == Walk::Leaf) {
+        // The cells of a slot (2T bytes per tuple) may take at most twice the tuple budget, so a many-tree, few-feature
+        // ensemble lands fewer tuples per slot instead of allocating GiBs of cells.
+        uint32_t tmax = 1;
+        for (const Dev& d : e->devs) tmax = std::max(tmax, d.shape.T);
+        const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
+        cap = std::min(cap, std::max<size_t>(4, budget / (2 * (size_t)tmax)) & ~(size_t)3);
+    }
     for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
-    for (Dev& d : e->devs) TRY(ensure_leaf_slots(e, d));
-    for (Dev& d : e->devs) d.run_leaf = true;
-    const int rc = infer_host_run(e, h_tuples, n, nullptr, nullptr, h_leaves);
-    for (Dev& d : e->devs) {
+    if (w == Walk::Leaf)
+        for (Dev& d : e->devs) TRY(ensure_leaf_slots(e, d));
+    for (Dev& d : e->devs) d.walk = w;
+    const int rc = infer_host_run(e, h_tuples, n, h_scores, h_labels, h_leaves);
+    for (Dev& d : e->devs) {                         // the next call may land another kind: leave no slot partly filled
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
-        d.run_leaf = false;
+        d.walk = Walk::Fp32;
     }
     return rc;
 }
@@ -1203,7 +1164,7 @@ int receive_tree_lines(dte_engine* e, const unsigned char*& p, size_t& n_lines) 
         int rc = program_devices(e, e->g);
         for (auto& v : e->tree_w) { v.clear(); v.shrink_to_fit(); }
         for (auto& v : e->tree_f) { v.clear(); v.shrink_to_fit(); }
-        if (!rc) rc = prepare_data_phase(e, true);
+        if (!rc) rc = prepare_data_phase(e);
         e->t_prog1 = Clock::now();
         e->prog_open = false;
         if (rc) { e->state = dte_engine::ST_IDLE; e->running = false; return rc; }
@@ -1391,7 +1352,7 @@ int dte_softreg_write(dte_t* e, uint32_t addr, uint64_t data) {
         if (!rc && classes_of(e) >= 2)
             rc = fail(e, DTE_ERR_CONFIG, "the resident ensemble has %u classes: the line stream carries one score per tuple "
                       "(use dte_infer_host / dte_infer_device, or stream a single-class ensemble)", classes_of(e));
-        if (!rc) { e->g = g; rc = prepare_data_phase(e, true); }
+        if (!rc) { e->g = g; rc = prepare_data_phase(e); }
     }
     if (rc) { e->state = dte_engine::ST_IDLE; e->running = false; return rc; }
     e->g = g;
@@ -1521,10 +1482,10 @@ int dte_process_done(dte_t* e, int* done) {
     return DTE_OK;
 }
 
-// dte_load_ensemble_classes, and with `binned` dte_load_ensemble_binned: the edge table over every tree of the streams
+// dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
 // is built, and refused, before anything is packed or uploaded.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
-                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool binned) {
+                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1535,7 +1496,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
     const unsigned char* wl = static_cast<const unsigned char*>(weight_cls);
     const unsigned char* fl = static_cast<const unsigned char*>(findex_cls);
     BinEdges bins;
-    if (binned) {
+    if (with_bins) {
         std::string msg;
         const int rc = bin_edges(g, wl, n_weight_cls, fl, n_findex_cls, bins, msg);
         if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
@@ -1558,7 +1519,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes, binned ? &bins : nullptr));
+    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
@@ -1580,23 +1541,29 @@ int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, con
     return dte_load_ensemble_classes(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, 1);
 }
 
-static int infer_device_common(dte_t* e, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream,
-                               bool accumulate, const char* what, bool bin = false) {
-    // the tile kernels read tuple rows as 16-byte vectors and every kernel stores 4-byte score words: a misaligned
-    // pointer would fault the walk and leave the caller's CUDA context unusable, so it is refused here
-    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "%s: %s not 16-byte aligned", what, bin ? "d_bins" : "d_tuples");
-    if (reinterpret_cast<uintptr_t>(d_scores) & 3u)
-        return fail(e, DTE_ERR_ARG, "%s: %s not 4-byte aligned", what, accumulate ? "d_scores_accum" : "d_scores");
+// Device buffers in, device buffers out on ONE device: the walk of kind w writes scores [n][C] (labels too when given)
+// or, for a leaf walk, cells [n][T] into `out`.  `what` names the call.
+static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples, size_t n, void* out, uint8_t* d_labels,
+                        void* cuda_stream, bool accumulate = false) {
+    // the tile kernels read tuple rows as 16-byte vectors, every score walk stores 4-byte words and the leaf walk stores
+    // the cells of a row in pieces of up to 16 bytes: a misaligned pointer would fault the walk and leave the caller's
+    // CUDA context unusable, so it is refused here
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u)
+        return fail(e, DTE_ERR_ARG, "%s: %s not 16-byte aligned", what, w == Walk::Binned ? "d_bins" : "d_tuples");
+    const int align = w == Walk::Leaf ? 16 : 4;
+    if (reinterpret_cast<uintptr_t>(out) & (align - 1))
+        return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what,
+                    w == Walk::Leaf ? "d_leaves" : accumulate ? "d_scores_accum" : "d_scores", align);
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));
-    TRY(check_resident(e, g, bin));
+    TRY(check_resident(e, g, w));
     Dev& d = e->devs[0];
     e->g = g;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     cudaStream_t st = pick_stream(d, cuda_stream);
     CUDA_TRY(e, cudaEventRecord(d.ev_t0, st));
-    TRY(walk_or_fail(e, d, d_tuples, n, d_scores, d_labels, st, accumulate, bin));
+    TRY(walk_or_fail(e, d, w, d_tuples, n, out, d_labels, st, accumulate));
     CUDA_TRY(e, cudaEventRecord(d.ev_t1, st));
     d.timing_pending = true;
     e->tuples_in += n;
@@ -1605,14 +1572,22 @@ static int infer_device_common(dte_t* e, const void* d_tuples, size_t n, float* 
     return DTE_OK;
 }
 
+// the kernel and plan the next walk of kind w would launch
+static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
+    if (!e || !buf || !len) return DTE_ERR_ARG;
+    if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
+    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, w);
+    return DTE_OK;
+}
+
 int dte_infer_device(dte_t* e, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream) {
     if (!e || (n && (!d_tuples || !d_scores))) return DTE_ERR_ARG;
-    return infer_device_common(e, d_tuples, n, d_scores, d_labels, cuda_stream, false, "dte_infer_device");
+    return infer_device(e, Walk::Fp32, "dte_infer_device", d_tuples, n, d_scores, d_labels, cuda_stream);
 }
 
 int dte_infer_device_accumulate(dte_t* e, const void* d_tuples, size_t n, float* d_scores_accum, void* cuda_stream) {
     if (!e || (n && (!d_tuples || !d_scores_accum))) return DTE_ERR_ARG;
-    return infer_device_common(e, d_tuples, n, d_scores_accum, nullptr, cuda_stream, true, "dte_infer_device_accumulate");
+    return infer_device(e, Walk::Fp32, "dte_infer_device_accumulate", d_tuples, n, d_scores_accum, nullptr, cuda_stream, true);
 }
 
 // ---- peer-visible buffers (CUDA IPC): partial-score buffers other processes' combine kernels read ----
@@ -1651,18 +1626,18 @@ int dte_ipc_close(dte_t* e, void* d_ptr, int owner) {
 
 int dte_infer_host(dte_t* e, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
     if (!e || (n && (!h_tuples || !h_scores))) return DTE_ERR_ARG;
-    return infer_host(e, static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels, false);
+    return infer_host(e, Walk::Fp32, "infer_host", static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels, nullptr);
 }
 
 // ---- binned inference (DESIGN.md §9) ----
 int dte_infer_host_binned(dte_t* e, const void* h_bins, size_t n, float* h_scores, uint8_t* h_labels) {
     if (!e || (n && (!h_bins || !h_scores))) return DTE_ERR_ARG;
-    return infer_host(e, static_cast<const unsigned char*>(h_bins), n, h_scores, h_labels, true);
+    return infer_host(e, Walk::Binned, "infer_host", static_cast<const unsigned char*>(h_bins), n, h_scores, h_labels, nullptr);
 }
 
 int dte_infer_device_binned(dte_t* e, const void* d_bins, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream) {
     if (!e || (n && (!d_bins || !d_scores))) return DTE_ERR_ARG;
-    return infer_device_common(e, d_bins, n, d_scores, d_labels, cuda_stream, false, "dte_infer_device_binned", true);
+    return infer_device(e, Walk::Binned, "dte_infer_device_binned", d_bins, n, d_scores, d_labels, cuda_stream);
 }
 
 int dte_bin_tuples_device(dte_t* e, const void* d_tuples, size_t n, uint8_t* d_bins, void* cuda_stream) {
@@ -1673,7 +1648,7 @@ int dte_bin_tuples_device(dte_t* e, const void* d_tuples, size_t n, uint8_t* d_b
     TRY(single_only(e, "dte_bin_tuples_device"));
     Geom g;
     TRY(decode_geom(e, g));
-    TRY(check_resident(e, g, true));
+    TRY(check_resident(e, g, Walk::Binned));
     if (!n) return DTE_OK;
     Dev& d = e->devs[0];
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
@@ -1699,49 +1674,20 @@ int dte_bin_edges(dte_t* e, uint32_t* offsets, uint32_t* edges, size_t cap, size
     return DTE_OK;
 }
 
-int dte_kernel_name_binned(dte_t* e, char* buf, size_t len) {
-    if (!e || !buf || !len) return DTE_ERR_ARG;
-    if (!e->devs[0].d_top_b) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
-    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, true);
-    return DTE_OK;
-}
+int dte_kernel_name_binned(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Binned, buf, len); }
 
 // ---- leaf-index inference (DESIGN.md §10) ----
 int dte_infer_device_leaves(dte_t* e, const void* d_tuples, size_t n, uint16_t* d_leaves, void* cuda_stream) {
     if (!e || (n && (!d_tuples || !d_leaves))) return DTE_ERR_ARG;
-    // tuple rows are read as 16-byte vectors and the cells of a row go out in stores of up to 16 bytes
-    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "dte_infer_device_leaves: d_tuples not 16-byte aligned");
-    if (reinterpret_cast<uintptr_t>(d_leaves) & 15u) return fail(e, DTE_ERR_ARG, "dte_infer_device_leaves: d_leaves not 16-byte aligned");
-    TRY(single_only(e, "dte_infer_device_leaves"));
-    Geom g;
-    TRY(decode_geom(e, g));
-    TRY(check_resident(e, g, false, true));
-    Dev& d = e->devs[0];
-    e->g = g;
-    CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    cudaStream_t st = pick_stream(d, cuda_stream);
-    CUDA_TRY(e, cudaEventRecord(d.ev_t0, st));
-    TRY(leaf_walk_or_fail(e, d, d_tuples, n, d_leaves, st));
-    CUDA_TRY(e, cudaEventRecord(d.ev_t1, st));
-    d.timing_pending = true;
-    e->tuples_in += n;
-    e->tuples_out += n;
-    if (!cuda_stream) CUDA_TRY(e, cudaStreamSynchronize(st));
-    return DTE_OK;
+    return infer_device(e, Walk::Leaf, "dte_infer_device_leaves", d_tuples, n, d_leaves, nullptr, cuda_stream);
 }
 
 int dte_infer_host_leaves(dte_t* e, const void* h_tuples, size_t n, uint16_t* h_leaves) {
     if (!e || (n && (!h_tuples || !h_leaves))) return DTE_ERR_ARG;
-    return infer_host_leaves(e, static_cast<const unsigned char*>(h_tuples), n, h_leaves);
+    return infer_host(e, Walk::Leaf, "infer_host_leaves", static_cast<const unsigned char*>(h_tuples), n, nullptr, nullptr, h_leaves);
 }
 
-int dte_kernel_name_leaves(dte_t* e, char* buf, size_t len) {
-    if (!e || !buf || !len) return DTE_ERR_ARG;
-    if (!e->devs[0].d_bottom_id)
-        return fail(e, DTE_ERR_STATE, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1");
-    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, false, true);
-    return DTE_OK;
-}
+int dte_kernel_name_leaves(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Leaf, buf, len); }
 
 int dte_host_alloc(dte_t* e, size_t bytes, void** h_ptr) {
     if (!e || !h_ptr || !bytes) return DTE_ERR_ARG;
@@ -1876,12 +1822,7 @@ int dte_get_info(dte_t* e, dte_info* info) {
     return DTE_OK;
 }
 
-int dte_kernel_name(dte_t* e, char* buf, size_t len) {
-    if (!e || !buf || !len) return DTE_ERR_ARG;
-    if (!e->devs[0].d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
-    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len);
-    return DTE_OK;
-}
+int dte_kernel_name(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Fp32, buf, len); }
 
 int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     if (!e) return DTE_ERR_ARG;

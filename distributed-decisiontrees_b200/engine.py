@@ -155,6 +155,14 @@ def _ptr(x):
     raise TypeError("cannot take the address of %r" % type(x))
 
 
+def _host_rows(x, dtype=None):
+    """(rows, n) of a host array [n, ...]: a numpy array made C-contiguous (and of `dtype` when given), or a pinned torch
+    CPU tensor as it is."""
+    if isinstance(x, np.ndarray):
+        x = np.ascontiguousarray(x, dtype=dtype)
+    return x, int(x.shape[0])
+
+
 class Engine:
     """One in-order engine on one GPU (the analogue of one FPGA role)."""
 
@@ -315,23 +323,27 @@ class Engine:
         self._check(self._lib.dte_infer_device(self._h, _ptr(d_tuples), int(n), _ptr(d_scores), _ptr(d_labels),
                                                _stream(stream)))
 
-    def infer_host(self, tuples, want_labels=True, out_scores=None, out_labels=None):
-        """tuples: host array (numpy, or a pinned torch CPU tensor) [n, F] fp32 -> (scores, labels).
-        scores is [n] for a single-class ensemble and [n, C] for a C-class one (out_scores must hold n*C words)."""
-        if isinstance(tuples, np.ndarray):
-            t = np.ascontiguousarray(tuples)
-            n = t.shape[0]
-        else:
-            t = tuples
-            n = int(tuples.shape[0])
+    def _infer_host(self, fn, rows, dtype, want_labels, out_scores, out_labels):
+        """Allocate the outputs of a host-buffer score call and run it -> (scores, labels)."""
+        t, n = _host_rows(rows, dtype)
         if out_scores is None:
             nc = self.num_classes()
             scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
         else:
             scores = out_scores
         labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
-        self._check(self._lib.dte_infer_host(self._h, _ptr(t), n, _ptr(scores), _ptr(labels)))
+        self._check(fn(self._h, _ptr(t), n, _ptr(scores), _ptr(labels)))
         return scores, labels
+
+    def _name(self, fn):
+        buf = C.create_string_buffer(256)
+        self._check(fn(self._h, buf, 256))
+        return buf.value.decode()
+
+    def infer_host(self, tuples, want_labels=True, out_scores=None, out_labels=None):
+        """tuples: host array (numpy, or a pinned torch CPU tensor) [n, F] fp32 -> (scores, labels).
+        scores is [n] for a single-class ensemble and [n, C] for a C-class one (out_scores must hold n*C words)."""
+        return self._infer_host(self._lib.dte_infer_host, tuples, None, want_labels, out_scores, out_labels)
 
     # -- binned inference (DESIGN.md §9) -----------------------------------------------------------
     def bin_edges(self):
@@ -356,25 +368,10 @@ class Engine:
 
     def infer_host_binned(self, bins, want_labels=True, out_scores=None, out_labels=None):
         """infer_host on u8 bins [n, F] in host memory (numpy, or a pinned torch CPU tensor) -> (scores, labels)."""
-        if isinstance(bins, np.ndarray):
-            b = np.ascontiguousarray(bins, dtype=np.uint8)
-            n = b.shape[0]
-        else:
-            b = bins
-            n = int(bins.shape[0])
-        if out_scores is None:
-            nc = self.num_classes()
-            scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
-        else:
-            scores = out_scores
-        labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
-        self._check(self._lib.dte_infer_host_binned(self._h, _ptr(b), n, _ptr(scores), _ptr(labels)))
-        return scores, labels
+        return self._infer_host(self._lib.dte_infer_host_binned, bins, np.uint8, want_labels, out_scores, out_labels)
 
     def kernel_name_binned(self):
-        buf = C.create_string_buffer(256)
-        self._check(self._lib.dte_kernel_name_binned(self._h, buf, 256))
-        return buf.value.decode()
+        return self._name(self._lib.dte_kernel_name_binned)
 
     # -- leaf-index inference (DESIGN.md §10) ----------------------------------------------------------
     def infer_device_leaves(self, d_tuples, n, d_leaves, stream=None):
@@ -384,20 +381,13 @@ class Engine:
     def infer_host_leaves(self, tuples, out=None):
         """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> [n, T] uint16: the cell, in tree t's
         own weight heap, of the leaf that local tree t sends each tuple to (T = info()["num_trees"])."""
-        if isinstance(tuples, np.ndarray):
-            t = np.ascontiguousarray(tuples)
-            n = t.shape[0]
-        else:
-            t = tuples
-            n = int(tuples.shape[0])
+        t, n = _host_rows(tuples)
         leaves = out if out is not None else np.empty((n, int(self.info()["num_trees"])), dtype=np.uint16)
         self._check(self._lib.dte_infer_host_leaves(self._h, _ptr(t), n, _ptr(leaves)))
         return leaves
 
     def kernel_name_leaves(self):
-        buf = C.create_string_buffer(256)
-        self._check(self._lib.dte_kernel_name_leaves(self._h, buf, 256))
-        return buf.value.decode()
+        return self._name(self._lib.dte_kernel_name_leaves)
 
     def infer_device_accumulate(self, d_tuples, n, d_scores_accum, stream=None):
         """Walk and ADD the partial scores into d_scores_accum (local or peer-GPU buffer), fused in the kernel."""
@@ -467,9 +457,7 @@ class Engine:
         return buf.value.decode()
 
     def kernel_name(self):
-        buf = C.create_string_buffer(256)
-        self._check(self._lib.dte_kernel_name(self._h, buf, 256))
-        return buf.value.decode()
+        return self._name(self._lib.dte_kernel_name)
 
     def info(self):
         i = DteInfo()

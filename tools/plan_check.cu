@@ -28,8 +28,8 @@ static const char* const kTunes[] = {
 };
 
 int main(int argc, char** argv) {
-    const bool bin = argc > 1 && !strcmp(argv[1], "bin");
-    const bool leaf = argc > 1 && !strcmp(argv[1], "leaf");
+    const char* kind = argc > 1 ? argv[1] : "";
+    const Walk walk = !strcmp(kind, "bin") ? Walk::Binned : !strcmp(kind, "leaf") ? Walk::Leaf : Walk::Fp32;
     const uint32_t Fs[] = {4, 8, 32, 64, 96, 128, 192, 256, 384, 512, 516, 768, 1024, 1536, 1796, 1800, 2048};
     for (const char* s : kTunes) {
         setenv("DTE_TUNE", s, 1);
@@ -54,8 +54,8 @@ int main(int argc, char** argv) {
                     sh.Tpad = C * sh.gpc * 8;
                     for (int want = KERNEL_AUTO; want <= KERNEL_TILE_STAGED; ++want) {
                         char name[256];
-                        kernel_name(d, tune, want, name, sizeof name, bin, leaf);
-                        const auto pl = make_plan(d, tune, want, bin);
+                        kernel_name(d, tune, want, name, sizeof name, walk);
+                        const auto pl = make_plan(d, tune, want, walk);
                         printf("%u %u %u %d %d %s\n", D, F, C, want, (int)phased_level(d, tune, pl), name);
                     }
                 }
