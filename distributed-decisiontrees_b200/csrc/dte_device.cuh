@@ -4,12 +4,14 @@
 // dte_kernels.cuh.  Reference behaviour cited per function (paths relative to the reference root).
 #pragma once
 #include "dte_kernels.cuh"
+#include "dte_shap.cuh"
 
 #include <algorithm>
 #include <array>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
 #include <deque>
 #include <string>
@@ -22,9 +24,9 @@ constexpr int kNumSlots = 3;          // landing slots per device: H2D of i+1, w
 
 enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED = 3 };
 
-// What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), or the leaf cell every
-// tree reaches (DESIGN.md §10)
-enum class Walk { Fp32, Binned, Leaf };
+// What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), the leaf cell every
+// tree reaches (DESIGN.md §10), or the TreeSHAP feature contributions (DESIGN.md §12)
+enum class Walk { Fp32, Binned, Leaf, Contrib };
 
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
@@ -133,6 +135,134 @@ inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& liv
     live.assign(n_int, 1);
     for (uint32_t i = 0; i < n_int; ++i)
         if ((!live[i] || (fi[i] & 0x4000u)) && 2 * i + 2 < n_int) live[2 * i + 1] = live[2 * i + 2] = 0;
+}
+
+// One path record, `stride` bytes (a multiple of 16):
+//   +0   double bz           the path's bias term v * prod(z)
+//   +8   float  v            leaf word W[t][cell]
+//   +12  u32    meta         cell | m << 16 | L << 24 (L = steps = depth of the cell, m = merged elements)
+//   +16  u64    stepmap      bits 4s..4s+3: the element (0-based) of step s, s = 0 the root step
+//   +24  u16    feat[Dmax]   feature of each element
+//   +zoff double z[Dmax]     zero fraction of each element
+// Nodes: per layout tree [2^D - 1] {thr word, fidx | missing_right << 16}; only the ancestors of end cells are read.
+struct ShapLayout {
+    uint32_t D = 0, M = 0;               // levels; longest merged path of the layout
+    uint32_t stride = 0, zoff = 0;       // bytes per path record, offset of z in it
+    uint32_t n_nodes = 0;                // 2^D - 1
+    uint32_t C = 1;
+    std::vector<uint2> nodes;            // [Tl][n_nodes], layout trees class-major, stream order inside a class
+    std::vector<unsigned long long> tree_path;   // [Tl + 1] first path of each layout tree
+    std::vector<uint32_t> cls_tree;      // [C + 1] first layout tree of each class
+    std::vector<unsigned char> paths;    // [paths][stride]
+    size_t bytes() const {
+        return nodes.size() * sizeof(uint2) + tree_path.size() * 8 + cls_tree.size() * 4 + paths.size();
+    }
+    size_t num_paths() const { return tree_path.empty() ? 0 : (size_t)tree_path.back(); }
+};
+
+// Builds the contribution layout of trees [first, first + count) of the streams (count = 0 with first = 0: all), class
+// of tree s = s % classes.  covers: fp32 [T_all][2^(D+1) - 1], indexed like the weight heap.  Only live internal nodes
+// and reachable end cells are read; each must be finite and > 0.  Returns 0, -1 (bad covers or streams; msg names the
+// tree and cell) or -4 (a feature index >= F).
+inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_cls, const unsigned char* wl, size_t n_wl,
+                             const unsigned char* fl, size_t n_fl, const float* covers, uint32_t first, uint32_t count,
+                             uint32_t classes, ShapLayout& out, std::string& msg) {
+    char buf[256];
+    if (classes < 1 || n_wl % w_cls || n_fl != (n_wl / w_cls) * f_cls) { msg = "tree streams: line counts do not match the geometry"; return -1; }
+    const size_t T_all = n_wl / w_cls;
+    if (count == 0 && first == 0) count = (uint32_t)T_all;
+    if ((size_t)first + count > T_all || count == 0) {
+        snprintf(buf, sizeof buf, "tree chunk [%u, %u) outside the %zu trees of the stream", first, first + count, T_all);
+        msg = buf; return -1;
+    }
+    const uint32_t n_int = (1u << D) - 1, n_all = (2u << D) - 1;
+    const size_t wstride = (size_t)w_cls * 4, fstride = (size_t)f_cls * 8;
+    const uint32_t* Wall = reinterpret_cast<const uint32_t*>(wl);
+    const uint16_t* Fall = reinterpret_cast<const uint16_t*>(fl);
+    out = ShapLayout();
+    out.D = D; out.C = classes; out.n_nodes = n_int;
+    out.zoff = (24u + 2u * D + 7u) & ~7u;
+    out.stride = (out.zoff + 8u * D + 15u) & ~15u;
+    std::vector<uint32_t> order;                     // layout tree -> local tree, class-major
+    out.cls_tree.assign(classes + 1, 0);
+    for (uint32_t c = 0; c < classes; ++c) {
+        out.cls_tree[c] = (uint32_t)order.size();
+        for (uint32_t t = 0; t < count; ++t)
+            if ((first + t) % classes == c) order.push_back(t);
+    }
+    out.cls_tree[classes] = (uint32_t)order.size();
+    out.nodes.resize((size_t)count * n_int);
+    out.tree_path.assign(1, 0);
+    std::vector<uint8_t> live;
+    std::vector<uint32_t> cells;
+    uint32_t anc[16], efeat[16];
+    double ez[16];
+    for (uint32_t k = 0; k < count; ++k) {
+        const uint32_t s = first + order[k];
+        const uint32_t* W = Wall + (size_t)s * wstride;
+        const uint16_t* FI = Fall + (size_t)s * fstride;
+        const float* cov = covers + (size_t)s * n_all;
+        live_nodes(FI, D, live);
+        auto bad_cover = [&](uint32_t cell) {
+            const float c = cov[cell];
+            if (std::isfinite(c) && c > 0.0f) return false;
+            snprintf(buf, sizeof buf, "covers: tree %u cell %u has cover %g: a live node or reachable leaf needs a finite cover > 0",
+                     s, cell, (double)c);
+            msg = buf;
+            return true;
+        };
+        cells.clear();
+        for (uint32_t i = 0; i < n_int; ++i) {
+            out.nodes[(size_t)k * n_int + i] = make_uint2(W[i], (FI[i] & 0x7FFu) | (uint32_t)((FI[i] >> 13) & 1u) << 16);
+            if (!live[i]) continue;
+            if ((FI[i] & 0x7FFu) >= F) {
+                snprintf(buf, sizeof buf, "tree %u node %u: feature index %u >= %u features", s, i, FI[i] & 0x7FFu, F);
+                msg = buf; return -4;
+            }
+            if (bad_cover(i)) return -1;
+            if ((FI[i] & 0x4000u) || 2 * i + 1 >= n_int) { cells.push_back(2 * i + 1); cells.push_back(2 * i + 2); }
+        }
+        const size_t p0 = out.paths.size() / out.stride;
+        out.paths.resize(out.paths.size() + cells.size() * out.stride, 0);
+        for (size_t q = 0; q < cells.size(); ++q) {
+            const uint32_t cell = cells[q];
+            if (bad_cover(cell)) return -1;
+            uint32_t L = 0;
+            for (uint32_t n = cell; n; n = (n - 1) >> 1) anc[L++] = n;   // the cell and its ancestors below the root
+            // step s goes from node (s ? anc[L-s] : 0) to anc[L-1-s]
+            uint32_t m = 0;
+            unsigned long long stepmap = 0;
+            for (uint32_t st = 0; st < L; ++st) {
+                const uint32_t node = st ? anc[L - st] : 0, child = anc[L - 1 - st];
+                const uint32_t f = FI[node] & 0x7FFu;
+                const double frac = (double)cov[child] / (double)cov[node];
+                uint32_t e = 0;
+                while (e < m && efeat[e] != f) ++e;
+                if (e == m) { efeat[m] = f; ez[m] = frac; ++m; }
+                else ez[e] = ez[e] * frac;
+                stepmap |= (unsigned long long)e << (4 * st);
+            }
+            float v;
+            memcpy(&v, &W[cell], 4);
+            double zp = ez[0];
+            for (uint32_t e = 1; e < m; ++e) zp = zp * ez[e];
+            const double bz = (double)v * zp;
+            unsigned char* r = out.paths.data() + (p0 + q) * out.stride;
+            const uint32_t meta = cell | m << 16 | L << 24;
+            memcpy(r, &bz, 8);
+            memcpy(r + 8, &v, 4);
+            memcpy(r + 12, &meta, 4);
+            memcpy(r + 16, &stepmap, 8);
+            for (uint32_t e = 0; e < m; ++e) {
+                const uint16_t f16 = (uint16_t)efeat[e];
+                memcpy(r + 24 + 2 * e, &f16, 2);
+                memcpy(r + out.zoff + 8 * e, &ez[e], 8);
+            }
+            out.M = std::max(out.M, m);
+        }
+        out.tree_path.push_back(out.paths.size() / out.stride);
+    }
+    return 0;
 }
 
 // The edge table over EVERY tree of the streams (not one chunk), so that engines holding different tree chunks of one
@@ -354,6 +484,7 @@ struct Slot {
     float* d_part = nullptr;      // group (ensemble-sharded) mode: this device's partial scores
     uint8_t* d_lb = nullptr;
     uint16_t* d_leaf = nullptr;   // leaf calls: [cap][T] cells of this slot (allocated by the first leaf call)
+    float* d_contrib = nullptr;   // contribution calls: [cap][C][F + 1] of this slot (allocated by the first such call)
     // sparse host calls: the chunk's indptr slice and its entries, densified into d_tup (allocated by the first sparse call)
     long long* d_sp_ptr = nullptr;
     uint32_t* d_sp_idx = nullptr;
@@ -389,6 +520,17 @@ struct Dev {
     uint32_t* d_bin_edges = nullptr;
     // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
     uint4* d_bottom_id = nullptr;
+    // contribution layout (dte_load_ensemble_contribs only, DESIGN.md §12): the device copy of a ShapLayout
+    ShapLayout shap;                  // its shape; the host vectors are released after the upload
+    uint2* d_shap_nodes = nullptr;
+    unsigned char* d_shap_paths = nullptr;
+    unsigned long long* d_shap_tree_path = nullptr;
+    uint32_t* d_shap_cls_tree = nullptr;
+    // dt_shap_generic's fp64 accumulators, guarded by the event of the last walk using them; a launch of `rows` tuples uses
+    // [F + 1][rows] of them.  Sized in words, so a later ensemble with more features regrows it; a placement frees it.
+    double* d_shap_scratch = nullptr;
+    size_t shap_scratch_words = 0;
+    cudaEvent_t ev_shap = nullptr;
     Walk walk = Walk::Fp32;           // the walk the landing slots feed: binned calls land u8 bins (F bytes per tuple)
     size_t run_tuple_bytes() const { return walk == Walk::Binned ? shape.g.F() : shape.g.tuple_bytes(); }
 
@@ -407,6 +549,9 @@ struct Dev {
     uint16_t* sink_leaf = nullptr;
     size_t leaf_pitch = 0;
     size_t leaf_slot_cells = 0;       // cells allocated per Slot::d_leaf
+    // contribution calls (dte_infer_host_contribs): rows of C * (F + 1) words land in sink_contrib
+    float* sink_contrib = nullptr;
+    size_t contrib_slot_words = 0;    // words allocated per Slot::d_contrib
     size_t sparse_slot_nnz = 0;       // entries allocated per Slot::d_sp_idx / d_sp_val (d_sp_ptr holds cap_tuples + 1)
     // dte_infer_device_sparse: two [rows][F] buffers the chunks are densified into, each guarded by the event of its
     // last walk, so a call on another stream never overwrites rows a walk still reads
@@ -649,6 +794,113 @@ inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, i
     lp.first = d.shape.first % d.shape.C;
     return launch_plan(d, pl, pl.row < 0 ? kGenericLeafKernels[pl.wide] : kTileLeafKernels[pl.row][pl.wide](pl.thread_bound()), lp,
                        n, st, why);
+}
+
+// ---- feature contributions (DESIGN.md §12) ----
+// Shared memory of one dt_shap_tile tuple group: fp64 accumulators [F + 1][32], the rows [32] and the tuple tile [F][32]
+inline size_t shap_group_smem(uint32_t F) { return (size_t)(F + 2) * 32 * 8 + (size_t)F * 32 * 4; }
+// Tuple groups (warps) per dt_shap_tile CTA: as many as fit the opt-in shared memory, at most 4; 0: the tile does not fit
+inline int shap_tile_groups(const Dev& d) {
+    return (int)std::min<size_t>(4, (size_t)d.smem_optin / shap_group_smem(d.shape.g.F()));
+}
+// Tile warps resident per SM: whole CTAs of shap_tile_groups warps in the SM's shared memory (the opt-in size stands for it)
+inline int shap_tile_warps_per_sm(const Dev& d) {
+    const int G = shap_tile_groups(d);
+    return G < 1 ? 0 : G * (int)((size_t)d.smem_optin / ((size_t)G * shap_group_smem(d.shape.g.F())));
+}
+// AUTO takes the tile only when at least this many of its warps fit an SM (F <= 36 on the H100).  Both kernels are
+// latency-bound chains of dependent fp64 operations, so the one with more resident warps wins: measured on the H100 at
+// D = 8, the tile is 5 % faster at F = 20 (28 warps per SM), the generic kernel 1.2-1.4x faster at F = 48-72 (12 and 8
+// tile warps) and 1.4-3x faster from F = 128 (4 and 2 tile warps), DESIGN.md §12.
+constexpr int kShapTileMinWarps = 16;
+// Whether a contribution walk runs dt_shap_tile: never when GENERIC is forced; when TILE (or TILE_STAGED) is forced,
+// whenever a tuple group fits; under AUTO, when it also keeps kShapTileMinWarps warps per SM.
+inline bool shap_tile(const Dev& d, int want) {
+    if (want == KERNEL_GENERIC || shap_tile_groups(d) < 1) return false;
+    return want != KERNEL_AUTO || shap_tile_warps_per_sm(d) >= kShapTileMinWarps;
+}
+// The instantiated path-length bound that holds the layout's longest merged path
+inline int shap_bound(uint32_t M) { return M <= 3 ? 3 : M <= 7 ? 7 : 15; }
+using ShapKernel = void (*)(ShapParams);
+inline ShapKernel shap_kernel(bool tile, int bound) {
+    if (tile) return bound == 3 ? dt_shap_tile<3> : bound == 7 ? dt_shap_tile<7> : dt_shap_tile<15>;
+    return bound == 3 ? dt_shap_generic<3> : bound == 7 ? dt_shap_generic<7> : dt_shap_generic<15>;
+}
+constexpr size_t kShapScratchBytes = 256ull << 20;   // dt_shap_generic accumulators: rows per launch = this / (8 (F + 1))
+
+// Launch the contribution walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident
+// contribution layout: d_out [n][C][F + 1].  The single-class run adds the first min(T, 8 S K) trees of `run`, a
+// multi-class run every tree.  dt_shap_generic runs in launches of at most kShapScratchBytes / (8 (F + 1)) tuples through
+// the device's fp64 scratch, which waits for the previous walk using it.  Returns a cudaError_t.
+inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, const void* d_tuples, size_t n, float* d_out,
+                                  cudaStream_t st, const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const uint32_t F = d.shape.g.F(), C = d.shape.C;
+    ShapParams p = {};
+    p.nodes = d.d_shap_nodes;
+    p.paths = d.d_shap_paths;
+    p.tree_path = d.d_shap_tree_path;
+    p.cls_tree = d.d_shap_cls_tree;
+    p.F = F; p.C = C; p.missing = run.missing;
+    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff;
+    p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    const int bound = shap_bound(d.shap.M);
+    const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
+    const size_t row_words = (size_t)C * (F + 1);
+    cudaError_t rc;
+    if (shap_tile(d, want_variant)) {
+        const int G = shap_tile_groups(d);
+        const size_t smem = (size_t)G * shap_group_smem(F);
+        const unsigned long long blocks = ((n + 31) / 32 + G - 1) / G;
+        if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+        p.tuples = tuples; p.out = d_out; p.n = n; p.groups = (uint32_t)G;
+        const ShapKernel k = shap_kernel(true, bound);
+        if ((rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return rc;
+        k<<<(unsigned)blocks, 32 * G, smem, st>>>(p);
+        if ((rc = cudaGetLastError()) == cudaSuccess) d.kernel_launches++;
+        return rc;
+    }
+    const size_t cap = std::max<size_t>(32, (kShapScratchBytes / ((size_t)(F + 1) * 8)) & ~(size_t)31);
+    const size_t rows = std::min(cap, (n + 31) & ~(size_t)31);
+    if (!d.ev_shap && (rc = cudaEventCreateWithFlags(&d.ev_shap, cudaEventDisableTiming)) != cudaSuccess) return rc;
+    const size_t words = rows * (F + 1);             // what the kernel indexes: phi[f * rows + row], f <= F, row < rows
+    if (d.shap_scratch_words < words) {               // grow: no walk on any stream may still use the old scratch
+        if ((rc = cudaDeviceSynchronize()) != cudaSuccess) return rc;
+        if (d.d_shap_scratch) cudaFree(d.d_shap_scratch);
+        d.d_shap_scratch = nullptr;
+        d.shap_scratch_words = 0;
+        if ((rc = cudaMalloc(&d.d_shap_scratch, words * 8)) != cudaSuccess) return rc;
+        d.shap_scratch_words = words;
+    }
+    if ((rc = cudaStreamWaitEvent(st, d.ev_shap, 0)) != cudaSuccess) return rc;
+    p.scratch = d.d_shap_scratch;
+    p.scratch_rows = rows;
+    const ShapKernel k = shap_kernel(false, bound);
+    for (size_t off = 0; off < n; off += rows) {
+        p.n = std::min(rows, n - off);
+        p.tuples = tuples + off * F;
+        p.out = d_out + off * row_words;
+        k<<<(unsigned)((p.n + 127) / 128), 128, 0, st>>>(p);
+        if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
+        d.kernel_launches++;
+    }
+    return cudaEventRecord(d.ev_shap, st);
+}
+
+// "dt_shap_tile<bound> warps=G smem=..." or "dt_shap_generic<bound>", as launch_contrib would launch it
+inline void contrib_kernel_name(const Dev& d, int want, char* buf, size_t len) {
+    const int bound = shap_bound(d.shap.M);
+    if (shap_tile(d, want)) {
+        const int G = shap_tile_groups(d);
+        snprintf(buf, len, "dt_shap_tile<%d> warps=%d smem=%zu", bound, G, (size_t)G * shap_group_smem(d.shape.g.F()));
+    } else {
+        snprintf(buf, len, "dt_shap_generic<%d>", bound);
+    }
+    if (d.shape.C >= 2) {
+        const size_t used = strlen(buf);
+        if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
+    }
 }
 
 // The plan of a walk of kind w, named dt_walk_generic / dt_walk_tile with the kind's suffix: _u8 binned, _leaf leaf

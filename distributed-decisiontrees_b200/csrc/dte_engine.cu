@@ -274,6 +274,7 @@ const char* missing_layout(const Dev& d, Walk w) {
     switch (w) {
         case Walk::Binned: return d.d_top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
         case Walk::Leaf: return d.d_bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
+        case Walk::Contrib: return d.d_shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
         default: return d.d_top ? nullptr : "no ensemble loaded";
     }
 }
@@ -310,9 +311,17 @@ uint32_t classes_of(const dte_engine* e) { return host_dev(e).shape.C; }
 void free_ensemble(Dev& d) {
     cudaSetDevice(d.ordinal);
     for (void* p : {(void*)d.d_top, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges,
-                    (void*)d.d_bottom_id})
+                    (void*)d.d_bottom_id, (void*)d.d_shap_nodes, (void*)d.d_shap_paths, (void*)d.d_shap_tree_path,
+                    (void*)d.d_shap_cls_tree, (void*)d.d_shap_scratch})
         if (p) cudaFree(p);
     d.d_bottom_id = nullptr;
+    d.d_shap_nodes = nullptr;
+    d.d_shap_paths = nullptr;
+    d.d_shap_tree_path = nullptr;
+    d.d_shap_cls_tree = nullptr;
+    d.d_shap_scratch = nullptr;                       // sized for the F of the ensemble it served
+    d.shap_scratch_words = 0;
+    d.shap = ShapLayout();
     d.d_top = nullptr;
     d.d_bottom = nullptr;
     d.d_top_b = nullptr;
@@ -329,8 +338,9 @@ int upload(dte_engine* e, T*& dst, const std::vector<T>& src) {
     return DTE_OK;
 }
 
-// `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr
-int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins) {
+// `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr.  `shap`: the contribution
+// layout of a dte_load_ensemble_contribs, else nullptr.
+int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap) {
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
     free_ensemble(d);
@@ -349,6 +359,18 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
         TRY(upload(e, d.d_bottom_id, pk.bottom_id));
         d.ensemble_bytes += pk.bottom_id.size() * sizeof(uint4);
     }
+    if (shap) {
+        double tab[4][kShapTab][kShapTab];
+        shap_tables(tab);
+        CUDA_TRY(e, cudaMemcpyToSymbol(c_shap_tab, tab, sizeof tab));
+        TRY(upload(e, d.d_shap_nodes, shap->nodes));
+        TRY(upload(e, d.d_shap_paths, shap->paths));
+        TRY(upload(e, d.d_shap_tree_path, shap->tree_path));
+        TRY(upload(e, d.d_shap_cls_tree, shap->cls_tree));
+        d.ensemble_bytes += shap->bytes();
+        d.shap.D = shap->D; d.shap.M = shap->M; d.shap.stride = shap->stride; d.shap.zoff = shap->zoff;
+        d.shap.n_nodes = shap->n_nodes; d.shap.C = shap->C;
+    }
     return DTE_OK;
 }
 
@@ -364,9 +386,20 @@ struct TreeShare {
 // share is packed class-major, the class of a tree taken from its global stream index (share.first counts from the
 // start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
 // binned layout is dropped.  With DTE_OPT_LEAF_LAYOUT the leaf-id layout is built and uploaded too; without it any
-// resident leaf-id layout is dropped.
-int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr) {
+// resident leaf-id layout is dropped.  `covers` (fp32 [T_all][2^(D+1)-1] for the trees of the streams): also build and
+// upload the contribution layout of every share, all of them built and checked before anything is uploaded; without it
+// any resident contribution layout is dropped.
+int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr,
+                   const float* covers = nullptr) {
     const bool chunked = e->part == Part::Chunked;
+    std::vector<ShapLayout> shap(covers ? (chunked ? e->devs.size() : 1) : 0);
+    for (size_t r = 0; r < shap.size(); ++r) {
+        const TreeShare& s = share[r];
+        std::string msg;
+        const int rc = build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
+                                         classes, shap[r], msg);
+        if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
+    }
     PackedEnsemble pk;
     for (size_t r = 0; r < e->devs.size(); ++r) {
         if (chunked || r == 0) {
@@ -375,7 +408,7 @@ int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_
             const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg, bins, e->opt_leaf);
             if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
         }
-        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins));
+        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins, covers ? &shap[chunked ? r : 0] : nullptr));
     }
     e->bins = bins ? *bins : BinEdges();
     e->placed = e->part;
@@ -418,12 +451,14 @@ void free_slots(Dev& d) {
         if (s.d_part) cudaFree(s.d_part);
         if (s.d_lb) cudaFree(s.d_lb);
         if (s.d_leaf) cudaFree(s.d_leaf);
-        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_leaf = nullptr;
+        if (s.d_contrib) cudaFree(s.d_contrib);
+        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_leaf = nullptr; s.d_contrib = nullptr;
         s.fill = s.walked = 0;
     }
     d.cap_tuples = 0;
     d.slot_parts = false;
     d.leaf_slot_cells = 0;
+    d.contrib_slot_words = 0;
 }
 
 // leaf calls: Slot::d_leaf of [cap][T] cells on every slot (score runs never allocate them)
@@ -439,6 +474,22 @@ int ensure_leaf_slots(dte_engine* e, Dev& d) {
     d.leaf_slot_cells = 0;
     for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_leaf, cells * sizeof(uint16_t)));
     d.leaf_slot_cells = cells;
+    return DTE_OK;
+}
+
+// contribution calls: Slot::d_contrib of [cap][C][F + 1] words on every slot (other runs never allocate them)
+int ensure_contrib_slots(dte_engine* e, Dev& d) {
+    const size_t words = d.cap_tuples * d.shape.C * (d.shape.g.F() + 1);
+    if (d.contrib_slot_words >= words) return DTE_OK;
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    CUDA_TRY(e, cudaDeviceSynchronize());
+    for (Slot& s : d.slot) {
+        if (s.d_contrib) cudaFree(s.d_contrib);
+        s.d_contrib = nullptr;
+    }
+    d.contrib_slot_words = 0;
+    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_contrib, words * sizeof(float)));
+    d.contrib_slot_words = words;
     return DTE_OK;
 }
 
@@ -531,6 +582,10 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
         const size_t T = d.shape.T;
         CUDA_TRY(e, cudaMemcpy2DAsync(d.sink_leaf, d.leaf_pitch * 2, s.d_leaf + from * T, T * 2, T * 2, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
         d.sink_leaf += cnt * d.leaf_pitch;
+    } else if (d.walk == Walk::Contrib) {
+        const size_t row = (size_t)d.shape.C * (d.shape.g.F() + 1);
+        CUDA_TRY(e, cudaMemcpyAsync(d.sink_contrib, s.d_contrib + from * row, cnt * row * 4, cudaMemcpyDeviceToHost, d.s_d2h));
+        d.sink_contrib += cnt * row;
     } else if (d.sink_sc) {
         const size_t C = d.slot_C;
         CUDA_TRY(e, cudaMemcpyAsync(d.sink_sc, s.d_sc + from * C, cnt * C * 4, cudaMemcpyDeviceToHost, d.s_d2h));
@@ -556,16 +611,18 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
 }
 
 // Launch the walk of kind w over n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.  `out`
-// receives the scores [n][C] (labels too when given), or for a leaf walk the cells [n][T].
+// receives the scores [n][C] (labels too when given), for a leaf walk the cells [n][T], for a contribution walk the
+// contributions [n][C][F + 1].
 int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, void* out, uint8_t* labels, cudaStream_t st,
                  bool accumulate = false) {
     const char* why = nullptr;
     const cudaError_t rc =
         w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
-                        : launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
+        : w == Walk::Contrib ? launch_contrib(d, e->g, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
+                             : launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
     if (rc != cudaSuccess)
-        return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s", w == Walk::Leaf ? "leaf walk" : "walk kernel",
-                    why ? why : cudaGetErrorString(rc));
+        return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s",
+                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : "walk kernel", why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
 
@@ -583,7 +640,9 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // result buffer of this slot drained
     const bool labels = d.sink_sc && d.sink_lb;
-    void* out = d.walk == Walk::Leaf ? (void*)(s.d_leaf + s.walked * d.shape.T) : (void*)(s.d_sc + s.walked * d.slot_C);
+    void* out = d.walk == Walk::Leaf      ? (void*)(s.d_leaf + s.walked * d.shape.T)
+                : d.walk == Walk::Contrib ? (void*)(s.d_contrib + s.walked * d.shape.C * (d.shape.g.F() + 1))
+                                          : (void*)(s.d_sc + s.walked * d.slot_C);
     TRY(walk_or_fail(e, d, d.walk, s.d_tup + s.walked * tb, cnt, out, labels ? s.d_lb + s.walked : nullptr, d.s_main));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
     TRY(enqueue_results(e, d, s, s.walked, cnt, labels));
@@ -1013,10 +1072,10 @@ int prepare_data_phase(dte_engine* e) {
 }
 
 // The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.
-// h_leaves (leaf calls): [n][columns] cells, every device's rows landing in its own columns.  sp (sparse calls): the rows
-// come from sp instead of h_tuples, one chunk per slot.
+// h_leaves (leaf calls): [n][columns] cells, every device's rows landing in its own columns.  h_contribs (contribution
+// calls, never Chunked): [n][C][F + 1].  sp (sparse calls): the rows come from sp instead of h_tuples, one chunk per slot.
 int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
-                   uint16_t* h_leaves, const SparseRows* sp) {
+                   uint16_t* h_leaves, float* h_contribs, const SparseRows* sp) {
     const size_t tb = e->devs[0].run_tuple_bytes();
     std::vector<uint64_t> enq0(e->devs.size());
     for (size_t i = 0; i < e->devs.size(); ++i) {
@@ -1065,6 +1124,7 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
                     d.sink_leaf = h_leaves + off * d.shape.T;
                     d.leaf_pitch = d.shape.T;
                 }
+                if (h_contribs) d.sink_contrib = h_contribs + off * d.shape.C * (d.shape.g.F() + 1);
                 r = sp ? land_sparse_dev(e, d, *sp, off, cnt) : land_dev(e, d, h_tuples + off * tb, cnt * tb);
                 if (!r && d.slot[d.cur].fill) {          // a short last chunk, or any sparse chunk
                     r = submit_dev(e, d, d.cur);
@@ -1096,7 +1156,7 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
         cudaSetDevice(d.ordinal);
         if (cudaEventElapsedTime(&ms, d.ev_t0, d.ev_t1) == cudaSuccess) d.last_walk_ms = ms;
         ms_max = std::max(ms_max, ms);
-        d.sink_sc = nullptr; d.sink_lb = nullptr; d.sink_leaf = nullptr;
+        d.sink_sc = nullptr; d.sink_lb = nullptr; d.sink_leaf = nullptr; d.sink_contrib = nullptr;
         d.res_enq = d.res_done = enq0[i];            // direct-sink results are not part of the line-stream queue
     }
     e->last_walk_ms = ms_max;
@@ -1108,8 +1168,9 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
 // Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
 // buffers as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every chunk
 // broadcast to all of them (tree chunks + ring combine).  A binned walk lands u8 bins [n][F] (F bytes per tuple through
-// the same landing slots); a leaf walk returns cells into h_leaves, no scores, no labels.  sp: fp32 rows densified on the
-// device from sparse rows (h_tuples unused).  `what` names the call.
+// the same landing slots); a leaf walk returns cells into h_leaves, no scores, no labels; a contribution walk returns
+// [n][C][F + 1] into h_scores, no labels.  sp: fp32 rows densified on the device from sparse rows (h_tuples unused).
+// `what` names the call.
 int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_tuples, size_t n, float* h_scores,
                uint8_t* h_labels, uint16_t* h_leaves, const SparseRows* sp = nullptr) {
     Geom g;
@@ -1118,6 +1179,9 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
     if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
+    // the contributions of a tree chunk are fp64 partials: combining them in ring order is not offered
+    if (w == Walk::Contrib && e->part == Part::Chunked)
+        return fail(e, DTE_ERR_CONFIG, "%s: an ensemble-sharded handle cannot return contributions; use a single-device or data-sharded handle", what);
     TRY(check_resident(e, g, w));
     if (n == 0) return DTE_OK;
     e->g = g;
@@ -1133,16 +1197,26 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
         const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
         cap = std::min(cap, std::max<size_t>(4, budget / (2 * (size_t)tmax)) & ~(size_t)3);
     }
+    if (w == Walk::Contrib) {
+        // the same bound on a slot's contribution rows (4 C (F + 1) bytes per tuple: 2 MiB at C = 256, F = 2048)
+        const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
+        const size_t row = (size_t)4 * classes_of(e) * (F + 1);
+        cap = std::min(cap, std::max<size_t>(4, budget / row) & ~(size_t)3);
+    }
     for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
     if (w == Walk::Leaf)
         for (Dev& d : e->devs) TRY(ensure_leaf_slots(e, d));
+    if (w == Walk::Contrib)
+        for (Dev& d : e->devs) TRY(ensure_contrib_slots(e, d));
     if (sp) {                                        // every chunk is a slot: the scratch holds the largest one's entries
         size_t nnz = 0;
         for (size_t r = 0; r < n; r += cap) nnz = std::max(nnz, (size_t)(sp->indptr[std::min(n, r + cap)] - sp->indptr[r]));
         for (Dev& d : e->devs) TRY(ensure_sparse_slots(e, d, nnz));
     }
     for (Dev& d : e->devs) d.walk = w;
-    const int rc = infer_host_run(e, h_tuples, n, h_scores, h_labels, h_leaves, sp);
+    const bool contrib = w == Walk::Contrib;
+    const int rc = infer_host_run(e, h_tuples, n, contrib ? nullptr : h_scores, contrib ? nullptr : h_labels, h_leaves,
+                                  contrib ? h_scores : nullptr, sp);
     for (Dev& d : e->devs) {                         // the next call may land another kind: leave no slot partly filled
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
         d.walk = Walk::Fp32;
@@ -1179,6 +1253,7 @@ void destroy_dev(Dev& d) {
     cudaDeviceSynchronize();
     free_ensemble(d);
     free_slots(d);
+    if (d.ev_shap) cudaEventDestroy(d.ev_shap);
     for (int j = 0; j < 2; ++j) {
         if (d.d_dense[j]) cudaFree(d.d_dense[j]);
         if (d.ev_dense[j]) cudaEventDestroy(d.ev_dense[j]);
@@ -1615,9 +1690,10 @@ int dte_process_done(dte_t* e, int* done) {
 }
 
 // dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
-// is built, and refused, before anything is packed or uploaded.
+// is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
-                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins) {
+                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins,
+                         const float* covers = nullptr) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1651,7 +1727,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr));
+    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
@@ -1666,6 +1742,14 @@ int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_
 int dte_load_ensemble_binned(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                              size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
     return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, true);
+}
+
+int dte_load_ensemble_contribs(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                               size_t n_findex_cls, const float* covers, uint32_t first_tree, uint32_t num_local_trees,
+                               uint32_t num_classes) {
+    if (!covers) return e ? fail(e, DTE_ERR_ARG, "dte_load_ensemble_contribs: covers is NULL") : DTE_ERR_ARG;
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
+                         covers);
 }
 
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1685,7 +1769,7 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
     const int align = w == Walk::Leaf ? 16 : 4;
     if (reinterpret_cast<uintptr_t>(out) & (align - 1))
         return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what,
-                    w == Walk::Leaf ? "d_leaves" : accumulate ? "d_scores_accum" : "d_scores", align);
+                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib ? "d_contribs" : accumulate ? "d_scores_accum" : "d_scores", align);
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));
@@ -1708,7 +1792,8 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
 static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
     if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
-    kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, w);
+    if (w == Walk::Contrib) contrib_kernel_name(e->devs[0], e->forced_variant, buf, len);
+    else kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, w);
     return DTE_OK;
 }
 
@@ -1820,6 +1905,20 @@ int dte_infer_host_leaves(dte_t* e, const void* h_tuples, size_t n, uint16_t* h_
 }
 
 int dte_kernel_name_leaves(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Leaf, buf, len); }
+
+// ---- feature contributions (DESIGN.md §12) ----
+int dte_infer_device_contribs(dte_t* e, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_contribs))) return DTE_ERR_ARG;
+    return infer_device(e, Walk::Contrib, "dte_infer_device_contribs", d_tuples, n, d_contribs, nullptr, cuda_stream);
+}
+
+int dte_infer_host_contribs(dte_t* e, const void* h_tuples, size_t n, float* h_contribs) {
+    if (!e || (n && (!h_tuples || !h_contribs))) return DTE_ERR_ARG;
+    return infer_host(e, Walk::Contrib, "infer_host_contribs", static_cast<const unsigned char*>(h_tuples), n, h_contribs, nullptr,
+                      nullptr);
+}
+
+int dte_kernel_name_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Contrib, buf, len); }
 
 // ---- sparse tuples (DESIGN.md §11) ----
 // The kernel reads indptr as 8-byte and the entries as 4-byte words: a misaligned pointer would fault it.

@@ -66,6 +66,11 @@ ABI = [
     ("dte_infer_device_leaves", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_leaves", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("dte_kernel_name_leaves", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_load_ensemble_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint32,
+                                             C.c_uint32, C.c_uint32]),
+    ("dte_infer_device_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_kernel_name_contribs", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
     ("dte_sparse_to_dense_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
                                              C.c_void_p, C.c_void_p]),
     ("dte_infer_device_sparse", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p,
@@ -295,12 +300,14 @@ class Engine:
 
     # -- fast paths -----------------------------------------------------------------------------
     def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False,
-                      leaves=False):
+                      leaves=False, covers=None):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
         call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
         binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
         feature), which the *_binned calls walk with u8 tuples.
-        leaves=True: DTE_OPT_LEAF_LAYOUT = 1 for this load, so the *_leaves calls can walk it."""
+        leaves=True: DTE_OPT_LEAF_LAYOUT = 1 for this load, so the *_leaves calls can walk it.
+        covers: fp32 [T_all, 2^(D+1)-1] node covers of every tree of the streams, indexed like the weight heap: also build
+        the contribution layout the *_contribs calls walk (dte_load_ensemble_contribs; not with binned=True)."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
@@ -308,10 +315,16 @@ class Engine:
             saved = getattr(self, "_leaf_opt", 0)
             self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
             try:
-                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned)
+                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers)
             finally:
                 self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
-        if binned:
+        if covers is not None:
+            if binned:
+                raise ValueError("covers and binned=True cannot be combined: the contribution calls take fp32 tuples")
+            cv = np.ascontiguousarray(covers, dtype=np.float32)
+            self._check(self._lib.dte_load_ensemble_contribs(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16, _ptr(cv),
+                                                             int(first_tree), int(num_local_trees), int(num_classes)))
+        elif binned:
             self._check(self._lib.dte_load_ensemble_binned(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
                                                            int(first_tree), int(num_local_trees), int(num_classes)))
         elif num_classes == 1:
@@ -400,6 +413,25 @@ class Engine:
 
     def kernel_name_leaves(self):
         return self._name(self._lib.dte_kernel_name_leaves)
+
+    # -- feature contributions (DESIGN.md §12) ---------------------------------------------------------
+    def infer_device_contribs(self, d_tuples, n, d_contribs, stream=None):
+        """[n, C, F + 1] fp32 TreeSHAP contributions (bias last) of fp32 tuples [n, F], both on the device (d_tuples 16-byte,
+        d_contribs 4-byte aligned)."""
+        self._check(self._lib.dte_infer_device_contribs(self._h, _ptr(d_tuples), int(n), _ptr(d_contribs), _stream(stream)))
+
+    def infer_host_contribs(self, tuples, out=None):
+        """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> contributions [n, F + 1] for a
+        single-class ensemble, [n, C, F + 1] for a C-class one: feature f's share of the class score, the bias last."""
+        t, n = _host_rows(tuples)
+        F, nc = int(self.info()["num_features"]), self.num_classes()
+        if out is None:
+            out = np.empty((n, F + 1) if nc == 1 else (n, nc, F + 1), dtype=np.float32)
+        self._check(self._lib.dte_infer_host_contribs(self._h, _ptr(t), n, _ptr(out)))
+        return out
+
+    def kernel_name_contribs(self):
+        return self._name(self._lib.dte_kernel_name_contribs)
 
     # -- sparse tuples (DESIGN.md §11) ------------------------------------------------------------------
     # absent=None: an absent feature is the run's missing pattern (XGBoost); a 32-bit word, e.g. 0, is used as it is.

@@ -113,6 +113,21 @@ def synth_ensemble(n_trees, depth_levels, num_features, seed=0xD7EE5, bias=0.02,
     return W.view(np.uint32).copy(), FI
 
 
+def synth_covers(FI, depth_levels, seed=0xC0BE5):
+    """Node covers [T, 2^(D+1)-1] fp32 for the trees of FI (uint16 [T, 2^D-1]), indexed like the weight heap: every cell of
+    the last level gets an integer count 1 .. 2^(23-D) from SplitMix64(seed), every other cell the sum of its two children
+    (so the early-leaf cells of any tree are covered too).  Sums stay below 2^24, so every cover is an exact fp32 integer."""
+    T, d = int(np.asarray(FI).shape[0]), int(depth_levels)
+    n_int, n_all = (1 << d) - 1, (2 << d) - 1
+    top = np.uint64(1 << max(0, 23 - d))
+    cov = np.zeros((T, n_all), dtype=np.int64)
+    z = splitmix64(seed, np.arange(T * (n_all - n_int), dtype=np.uint64)).reshape(T, n_all - n_int)
+    cov[:, n_int:] = (z % top).astype(np.int64) + 1
+    for i in range(n_int - 1, -1, -1):
+        cov[:, i] = cov[:, 2 * i + 1] + cov[:, 2 * i + 2]
+    return cov.astype(np.float32)
+
+
 def bin_tuples(x_words, offsets, edges, missing=MISSING_DEFAULT):
     """The binned tuple format, defined on the host: fp32 tuple words [n, F] -> u8 bins [n, F].
 

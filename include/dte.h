@@ -231,6 +231,38 @@ int dte_infer_host_leaves(dte_t* engine, const void* h_tuples, size_t n, uint16_
  * leaf-id layout. */
 int dte_kernel_name_leaves(dte_t* engine, char* buf, size_t len);
 
+/* ---- feature contributions (DESIGN.md §12) --------------------------------------------------- */
+/* Path-dependent TreeSHAP (XGBoost pred_contribs, LightGBM pred_contrib, shap's TreeExplainer): for each tuple and class,
+ * each feature's share of the score and the bias.  For tuple x and tree t, v_t(S) is the tree's output when the features
+ * in S follow x by the walk's decision rule (the run's missing pattern, int32 compare, bit 13) and every other node
+ * averages its two children weighted by cover(child) / cover(node).  Trees are the source trees of the streams: a node
+ * with bit 14 ends its paths at its two child cells, and D = 1 has one level.  contribs[i][c][f] for f < F is the
+ * Shapley value of feature f summed over the class-c trees, contribs[i][c][F] the bias sum_t v_t({}), so a row sums to the
+ * score up to rounding.  The trees are those the score walk adds: the first min(T, 8*S*K) local trees of a single-class
+ * ensemble, every tree of a multi-class one.  Computed in fp64 with every operation rounded on its own in the order
+ * DESIGN.md §12 fixes, then rounded once to fp32, so every word is reproducible.  Layout [n][C][F+1] fp32. */
+/* dte_load_ensemble_classes (same placement), and in addition the contribution layout.  covers: fp32
+ * [T_all][2^(D+1)-1] for every tree of the streams, indexed like the weight heap (XGBoost cover / sum_hessian, LightGBM
+ * internal_count / leaf_count, scikit-learn weighted_n_node_samples).  Only live internal nodes (not below an early leaf)
+ * and reachable end cells are read; each must be finite and > 0, else DTE_ERR_ARG naming the tree and cell, before
+ * anything is uploaded: the resident ensemble stays.  Every other placement (dte_load_ensemble*, a tree line stream) drops
+ * the contribution layout, after which the contribution calls return DTE_ERR_STATE. */
+int dte_load_ensemble_contribs(dte_t* engine, const void* weight_cls, size_t n_weight_cls,
+                               const void* findex_cls, size_t n_findex_cls, const float* covers,
+                               uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes);
+/* [n][C][F+1] contributions of n fp32 tuples in device memory.  Single-device handles; stream as dte_infer_device.
+ * d_tuples must be 16-byte aligned and d_contribs 4-byte aligned, else DTE_ERR_ARG before any launch.
+ * DTE_KERNEL_AUTO takes dt_shap_tile when at least 16 of its warps fit an SM (F <= 36 on the H100), else dt_shap_generic;
+ * dte_set_kernel_variant(DTE_KERNEL_GENERIC) forces dt_shap_generic, DTE_KERNEL_TILE / _STAGED force dt_shap_tile
+ * wherever its tile fits shared memory (F up to about 590). */
+int dte_infer_device_contribs(dte_t* engine, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream);
+/* The same from host memory through the landing pipeline: single-device and data-sharded handles (rows in global tuple
+ * order).  An ensemble-sharded handle returns DTE_ERR_CONFIG.  The contribution buffers of the landing slots are
+ * allocated by the first call; a slot lands fewer tuples when its rows would exceed the tuple landing budget. */
+int dte_infer_host_contribs(dte_t* engine, const void* h_tuples, size_t n, float* h_contribs);
+/* "dt_shap_tile<bound> warps=G smem=..." or "dt_shap_generic<bound>"; DTE_ERR_STATE without a contribution layout. */
+int dte_kernel_name_contribs(dte_t* engine, char* buf, size_t len);
+
 /* ---- sparse tuples (DESIGN.md §11) ------------------------------------------------------------- */
 /* n tuples as CSR rows: indptr int64 [n + 1], indices uint32 [nnz] (feature numbers), values [nnz] 32-bit words (fp32 bit
  * patterns).  Row i's entries are k in [indptr[i], indptr[i+1]), indexing indices and values absolutely, so indptr[0]

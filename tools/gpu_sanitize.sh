@@ -57,6 +57,13 @@ for T in tests/test_gpu_sparse.py::test_sparse_to_dense_device_bytes "tests/test
   stag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_sparse_${stag}.log"
 done
+# the contribution kernels (dt_shap_tile with two tuple groups per CTA, dt_shap_generic at a width only it serves and in
+# two launches through its fp64 scratch) and the ragged tail of a warp
+for T in tests/test_gpu_contribs.py::test_headline_geometry tests/test_gpu_contribs.py::test_generic_only_width \
+         tests/test_gpu_contribs.py::test_generic_launches_in_chunks "tests/test_gpu_contribs.py::test_tuple_counts[33]"; do
+  ctag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_contribs_${ctag}.log"
+done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1
 echo "racecheck [canonical textbook pipeline] rc=$? $(grep -E 'canonical|RACECHECK SUMMARY' $OUT/sanitizer_racecheck_canonical.log | tr '\n' ' ' | cut -c1-300)"
