@@ -483,8 +483,8 @@ struct Slot {
     float* d_sc = nullptr;        // final scores of this slot (single / data-sharded / host node of a group)
     float* d_part = nullptr;      // group (ensemble-sharded) mode: this device's partial scores
     uint8_t* d_lb = nullptr;
-    uint16_t* d_leaf = nullptr;   // leaf calls: [cap][T] cells of this slot (allocated by the first leaf call)
-    float* d_contrib = nullptr;   // contribution calls: [cap][C][F + 1] of this slot (allocated by the first such call)
+    // leaf and contribution calls: [cap] result rows of row_bytes each (allocated by the first such call)
+    unsigned char* d_rows = nullptr;
     // sparse host calls: the chunk's indptr slice and its entries, densified into d_tup (allocated by the first sparse call)
     long long* d_sp_ptr = nullptr;
     uint32_t* d_sp_idx = nullptr;
@@ -541,17 +541,12 @@ struct Dev {
     uint32_t slot_C = 1;              // score words per tuple in d_sc / d_part (the resident ensemble's classes)
     bool slot_parts = false;          // d_part allocated
     int cur = 0;                      // slot being filled
-    // result sink of the next submitted tuples: direct host pointers (fast path) or the pinned ring (line stream)
-    float* sink_sc = nullptr;
+    size_t slot_row_bytes = 0;        // bytes allocated per Slot::d_rows
+    // result sink of the next submitted tuples: the caller's host rows (fast path), sink_pitch bytes apart (an
+    // ensemble-sharded leaf call: this device's columns of the caller's rows), or, when null, the pinned ring (line stream)
+    unsigned char* sink = nullptr;
+    size_t sink_pitch = 0;
     uint8_t* sink_lb = nullptr;
-    // leaf calls (dte_infer_host_leaves): the walk writes cells into Slot::d_leaf and its rows land in sink_leaf, whose
-    // rows are leaf_pitch cells apart (this device's columns of the caller's rows)
-    uint16_t* sink_leaf = nullptr;
-    size_t leaf_pitch = 0;
-    size_t leaf_slot_cells = 0;       // cells allocated per Slot::d_leaf
-    // contribution calls (dte_infer_host_contribs): rows of C * (F + 1) words land in sink_contrib
-    float* sink_contrib = nullptr;
-    size_t contrib_slot_words = 0;    // words allocated per Slot::d_contrib
     size_t sparse_slot_nnz = 0;       // entries allocated per Slot::d_sp_idx / d_sp_val (d_sp_ptr holds cap_tuples + 1)
     // dte_infer_device_sparse: two [rows][F] buffers the chunks are densified into, each guarded by the event of its
     // last walk, so a call on another stream never overwrites rows a walk still reads
@@ -575,6 +570,17 @@ struct Dev {
     double last_walk_ms = 0;
     uint64_t tuples_landed = 0;       // whole tuples landed on this device since `start`
 };
+
+// Leaf and contribution walks write their rows into Slot::d_rows; score walks into d_sc / d_part, which the combines,
+// the labels and the line stream's ring read.
+inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib; }
+// Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes, or
+// C (F + 1) contribution words
+inline size_t row_bytes(const Dev& d, Walk w) {
+    if (w == Walk::Leaf) return 2 * (size_t)d.shape.T;
+    if (w == Walk::Contrib) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
+    return 4 * (size_t)d.slot_C;
+}
 
 // ---- launch planning ---------------------------------------------------------------------------
 // the binned walk stages 4-byte tree tops and holds one byte per feature in the tile
@@ -813,18 +819,32 @@ inline int shap_tile_warps_per_sm(const Dev& d) {
 // D = 8, the tile is 5 % faster at F = 20 (28 warps per SM), the generic kernel 1.2-1.4x faster at F = 48-72 (12 and 8
 // tile warps) and 1.4-3x faster from F = 128 (4 and 2 tile warps), DESIGN.md §12.
 constexpr int kShapTileMinWarps = 16;
-// Whether a contribution walk runs dt_shap_tile: never when GENERIC is forced; when TILE (or TILE_STAGED) is forced,
-// whenever a tuple group fits; under AUTO, when it also keeps kShapTileMinWarps warps per SM.
-inline bool shap_tile(const Dev& d, int want) {
-    if (want == KERNEL_GENERIC || shap_tile_groups(d) < 1) return false;
-    return want != KERNEL_AUTO || shap_tile_warps_per_sm(d) >= kShapTileMinWarps;
+// How a contribution walk runs, read by both launch_contrib and contrib_kernel_name: dt_shap_tile with `groups` warps
+// and `smem` bytes per CTA, or dt_shap_generic, instantiated with the path-length bound that holds the layout's longest
+// merged path.  The tile runs never when GENERIC is forced; when TILE (or TILE_STAGED) is forced, whenever a tuple group
+// fits; under AUTO, when it also keeps kShapTileMinWarps warps per SM.
+struct ShapPlan {
+    bool tile = false;
+    int groups = 0;
+    size_t smem = 0;
+    int bound = 3;
+};
+inline ShapPlan shap_plan(const Dev& d, int want) {
+    ShapPlan p;
+    const uint32_t M = d.shap.M;
+    p.bound = M <= 3 ? 3 : M <= 7 ? 7 : 15;
+    const int G = shap_tile_groups(d);
+    p.tile = want != KERNEL_GENERIC && G >= 1 && (want != KERNEL_AUTO || shap_tile_warps_per_sm(d) >= kShapTileMinWarps);
+    if (p.tile) {
+        p.groups = G;
+        p.smem = (size_t)G * shap_group_smem(d.shape.g.F());
+    }
+    return p;
 }
-// The instantiated path-length bound that holds the layout's longest merged path
-inline int shap_bound(uint32_t M) { return M <= 3 ? 3 : M <= 7 ? 7 : 15; }
 using ShapKernel = void (*)(ShapParams);
-inline ShapKernel shap_kernel(bool tile, int bound) {
-    if (tile) return bound == 3 ? dt_shap_tile<3> : bound == 7 ? dt_shap_tile<7> : dt_shap_tile<15>;
-    return bound == 3 ? dt_shap_generic<3> : bound == 7 ? dt_shap_generic<7> : dt_shap_generic<15>;
+inline ShapKernel shap_kernel(const ShapPlan& p) {
+    if (p.tile) return p.bound == 3 ? dt_shap_tile<3> : p.bound == 7 ? dt_shap_tile<7> : dt_shap_tile<15>;
+    return p.bound == 3 ? dt_shap_generic<3> : p.bound == 7 ? dt_shap_generic<7> : dt_shap_generic<15>;
 }
 constexpr size_t kShapScratchBytes = 256ull << 20;   // dt_shap_generic accumulators: rows per launch = this / (8 (F + 1))
 
@@ -845,19 +865,18 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     p.F = F; p.C = C; p.missing = run.missing;
     p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff;
     p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
-    const int bound = shap_bound(d.shap.M);
+    const ShapPlan pl = shap_plan(d, want_variant);
+    const ShapKernel k = shap_kernel(pl);
     const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
     const size_t row_words = (size_t)C * (F + 1);
     cudaError_t rc;
-    if (shap_tile(d, want_variant)) {
-        const int G = shap_tile_groups(d);
-        const size_t smem = (size_t)G * shap_group_smem(F);
+    if (pl.tile) {
+        const int G = pl.groups;
         const unsigned long long blocks = ((n + 31) / 32 + G - 1) / G;
         if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
         p.tuples = tuples; p.out = d_out; p.n = n; p.groups = (uint32_t)G;
-        const ShapKernel k = shap_kernel(true, bound);
-        if ((rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return rc;
-        k<<<(unsigned)blocks, 32 * G, smem, st>>>(p);
+        if ((rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem)) != cudaSuccess) return rc;
+        k<<<(unsigned)blocks, 32 * G, pl.smem, st>>>(p);
         if ((rc = cudaGetLastError()) == cudaSuccess) d.kernel_launches++;
         return rc;
     }
@@ -876,7 +895,6 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     if ((rc = cudaStreamWaitEvent(st, d.ev_shap, 0)) != cudaSuccess) return rc;
     p.scratch = d.d_shap_scratch;
     p.scratch_rows = rows;
-    const ShapKernel k = shap_kernel(false, bound);
     for (size_t off = 0; off < n; off += rows) {
         p.n = std::min(rows, n - off);
         p.tuples = tuples + off * F;
@@ -890,13 +908,9 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
 
 // "dt_shap_tile<bound> warps=G smem=..." or "dt_shap_generic<bound>", as launch_contrib would launch it
 inline void contrib_kernel_name(const Dev& d, int want, char* buf, size_t len) {
-    const int bound = shap_bound(d.shap.M);
-    if (shap_tile(d, want)) {
-        const int G = shap_tile_groups(d);
-        snprintf(buf, len, "dt_shap_tile<%d> warps=%d smem=%zu", bound, G, (size_t)G * shap_group_smem(d.shape.g.F()));
-    } else {
-        snprintf(buf, len, "dt_shap_generic<%d>", bound);
-    }
+    const ShapPlan pl = shap_plan(d, want);
+    if (pl.tile) snprintf(buf, len, "dt_shap_tile<%d> warps=%d smem=%zu", pl.bound, pl.groups, pl.smem);
+    else snprintf(buf, len, "dt_shap_generic<%d>", pl.bound);
     if (d.shape.C >= 2) {
         const size_t used = strlen(buf);
         if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);

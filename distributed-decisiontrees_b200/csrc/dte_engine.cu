@@ -450,46 +450,28 @@ void free_slots(Dev& d) {
         if (s.d_sc) cudaFree(s.d_sc);
         if (s.d_part) cudaFree(s.d_part);
         if (s.d_lb) cudaFree(s.d_lb);
-        if (s.d_leaf) cudaFree(s.d_leaf);
-        if (s.d_contrib) cudaFree(s.d_contrib);
-        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_leaf = nullptr; s.d_contrib = nullptr;
+        if (s.d_rows) cudaFree(s.d_rows);
+        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_rows = nullptr;
         s.fill = s.walked = 0;
     }
     d.cap_tuples = 0;
     d.slot_parts = false;
-    d.leaf_slot_cells = 0;
-    d.contrib_slot_words = 0;
+    d.slot_row_bytes = 0;
 }
 
-// leaf calls: Slot::d_leaf of [cap][T] cells on every slot (score runs never allocate them)
-int ensure_leaf_slots(dte_engine* e, Dev& d) {
-    const size_t cells = d.cap_tuples * d.shape.T;
-    if (d.leaf_slot_cells >= cells) return DTE_OK;
+// leaf and contribution calls: Slot::d_rows of [cap] rows of walk w on every slot (score runs never allocate them)
+int ensure_row_slots(dte_engine* e, Dev& d, Walk w) {
+    const size_t bytes = d.cap_tuples * row_bytes(d, w);
+    if (d.slot_row_bytes >= bytes) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());
     for (Slot& s : d.slot) {
-        if (s.d_leaf) cudaFree(s.d_leaf);
-        s.d_leaf = nullptr;
+        if (s.d_rows) cudaFree(s.d_rows);
+        s.d_rows = nullptr;
     }
-    d.leaf_slot_cells = 0;
-    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_leaf, cells * sizeof(uint16_t)));
-    d.leaf_slot_cells = cells;
-    return DTE_OK;
-}
-
-// contribution calls: Slot::d_contrib of [cap][C][F + 1] words on every slot (other runs never allocate them)
-int ensure_contrib_slots(dte_engine* e, Dev& d) {
-    const size_t words = d.cap_tuples * d.shape.C * (d.shape.g.F() + 1);
-    if (d.contrib_slot_words >= words) return DTE_OK;
-    CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    CUDA_TRY(e, cudaDeviceSynchronize());
-    for (Slot& s : d.slot) {
-        if (s.d_contrib) cudaFree(s.d_contrib);
-        s.d_contrib = nullptr;
-    }
-    d.contrib_slot_words = 0;
-    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_contrib, words * sizeof(float)));
-    d.contrib_slot_words = words;
+    d.slot_row_bytes = 0;
+    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_rows, bytes));
+    d.slot_row_bytes = bytes;
     return DTE_OK;
 }
 
@@ -573,24 +555,25 @@ int poll_dev(dte_engine* e, Dev& d, uint64_t need) {
     return DTE_OK;
 }
 
-// D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink.  A leaf walk's
-// result is shape.T cells, its rows leaf_pitch cells apart on the host; a score is slot_C words (the direct sink only:
-// the line stream's pinned ring always carries one word per tuple).
+// The result rows of slot s for the device's walk: d_rows, or the final scores d_sc
+unsigned char* slot_rows(const Dev& d, const Slot& s) {
+    return row_walk(d.walk) ? s.d_rows : reinterpret_cast<unsigned char*>(s.d_sc);
+}
+
+// D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink: rows of row_bytes,
+// sink_pitch bytes apart on the host, and their labels when asked.  Without a sink, into the line stream's pinned ring,
+// which always carries one score word per tuple.
 int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, bool labels) {
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_d2h, s.ev_walk, 0));
-    if (d.walk == Walk::Leaf) {
-        const size_t T = d.shape.T;
-        CUDA_TRY(e, cudaMemcpy2DAsync(d.sink_leaf, d.leaf_pitch * 2, s.d_leaf + from * T, T * 2, T * 2, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
-        d.sink_leaf += cnt * d.leaf_pitch;
-    } else if (d.walk == Walk::Contrib) {
-        const size_t row = (size_t)d.shape.C * (d.shape.g.F() + 1);
-        CUDA_TRY(e, cudaMemcpyAsync(d.sink_contrib, s.d_contrib + from * row, cnt * row * 4, cudaMemcpyDeviceToHost, d.s_d2h));
-        d.sink_contrib += cnt * row;
-    } else if (d.sink_sc) {
-        const size_t C = d.slot_C;
-        CUDA_TRY(e, cudaMemcpyAsync(d.sink_sc, s.d_sc + from * C, cnt * C * 4, cudaMemcpyDeviceToHost, d.s_d2h));
-        d.sink_sc += cnt * C;
-        if (labels && d.sink_lb) {
+    if (d.sink) {
+        const size_t row = row_bytes(d, d.walk);
+        const unsigned char* src = slot_rows(d, s) + from * row;
+        if (d.sink_pitch == row)
+            CUDA_TRY(e, cudaMemcpyAsync(d.sink, src, cnt * row, cudaMemcpyDeviceToHost, d.s_d2h));
+        else
+            CUDA_TRY(e, cudaMemcpy2DAsync(d.sink, d.sink_pitch, src, row, row, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
+        d.sink += cnt * d.sink_pitch;
+        if (labels) {
             CUDA_TRY(e, cudaMemcpyAsync(d.sink_lb, s.d_lb + from, cnt, cudaMemcpyDeviceToHost, d.s_d2h));
             d.sink_lb += cnt;
         }
@@ -639,10 +622,8 @@ int submit_dev(dte_engine* e, Dev& d, int b) {
     CUDA_TRY(e, cudaEventRecord(s.ev_land, d.s_h2d));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_land, 0));
     CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, s.ev_d2h, 0));        // result buffer of this slot drained
-    const bool labels = d.sink_sc && d.sink_lb;
-    void* out = d.walk == Walk::Leaf      ? (void*)(s.d_leaf + s.walked * d.shape.T)
-                : d.walk == Walk::Contrib ? (void*)(s.d_contrib + s.walked * d.shape.C * (d.shape.g.F() + 1))
-                                          : (void*)(s.d_sc + s.walked * d.slot_C);
+    const bool labels = d.sink && d.sink_lb;
+    unsigned char* out = slot_rows(d, s) + s.walked * row_bytes(d, d.walk);
     TRY(walk_or_fail(e, d, d.walk, s.d_tup + s.walked * tb, cnt, out, labels ? s.d_lb + s.walked : nullptr, d.s_main));
     CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
     TRY(enqueue_results(e, d, s, s.walked, cnt, labels));
@@ -864,7 +845,7 @@ int submit_group(dte_engine* e, int b) {
         for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));   // every piece has landed here
         // the cells of this slot have been copied out / the previous combine is done with our partials
         CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, cells ? s.ev_d2h : h.slot[b].ev_comb, 0));
-        void* out = cells ? (void*)(s.d_leaf + walked * d.shape.T) : (void*)(s.d_part + walked * C);
+        void* out = cells ? (void*)(s.d_rows + walked * row_bytes(d, Walk::Leaf)) : (void*)(s.d_part + walked * C);
         TRY(walk_or_fail(e, d, h.walk, s.d_tup + walked * tb, cnt, out, nullptr, d.s_main));
         CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
         s.walked = whole;
@@ -876,7 +857,7 @@ int submit_group(dte_engine* e, int b) {
         }
     } else {
         Slot& hs = h.slot[b];
-        const bool labels = h.sink_sc && h.sink_lb;
+        const bool labels = h.sink && h.sink_lb;
         CUDA_TRY(e, cudaSetDevice(h.ordinal));
         CUDA_TRY(e, cudaStreamWaitEvent(h.s_main, hs.ev_d2h, 0));
         if (!e->combine_nccl) {
@@ -1021,7 +1002,7 @@ bool fragment_pending(const dte_engine* e) {
 void reset_pipeline(Dev& d) {
     for (Slot& s : d.slot) { s.fill = 0; s.walked = 0; }
     d.cur = 0;
-    d.sink_sc = nullptr;
+    d.sink = nullptr;
     d.sink_lb = nullptr;
     d.res_enq = d.res_done = 0;
     d.tuples_landed = 0;
@@ -1071,11 +1052,11 @@ int prepare_data_phase(dte_engine* e) {
     return DTE_OK;
 }
 
-// The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.
-// h_leaves (leaf calls): [n][columns] cells, every device's rows landing in its own columns.  h_contribs (contribution
-// calls, never Chunked): [n][C][F + 1].  sp (sparse calls): the rows come from sp instead of h_tuples, one chunk per slot.
-int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float* h_scores, uint8_t* h_labels,
-                   uint16_t* h_leaves, float* h_contribs, const SparseRows* sp) {
+// The landing pipeline of one infer_host call, set up by infer_host: n tuples of Dev::run_tuple_bytes() each.  h_out
+// receives n result rows of the walk (row_bytes), an ensemble-sharded leaf call's rows [n][columns] with every device's
+// cells landing in its own columns.  sp (sparse calls): the rows come from sp instead of h_tuples, one chunk per slot.
+int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, unsigned char* h_out, uint8_t* h_labels,
+                   const SparseRows* sp) {
     const size_t tb = e->devs[0].run_tuple_bytes();
     std::vector<uint64_t> enq0(e->devs.size());
     for (size_t i = 0; i < e->devs.size(); ++i) {
@@ -1087,17 +1068,19 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
     int rc = DTE_OK;
     if (e->part == Part::Chunked) {
         Dev& h = host_dev(e);
-        h.sink_sc = h_scores;
         h.sink_lb = h_labels;
-        if (h_leaves) {                                  // ring position r owns columns [sum of T before r, + T_r)
-            size_t cols = 0, off = 0;
-            for (const Dev& d : e->devs) cols += d.shape.T;
+        if (h.walk == Walk::Leaf) {                      // ring position r owns columns [sum of T before r, + T_r)
+            size_t pitch = 0, off = 0;
+            for (const Dev& d : e->devs) pitch += row_bytes(d, Walk::Leaf);
             for (size_t r = 0; r < e->devs.size(); ++r) {
                 Dev& d = e->devs[(size_t)e->pos2dev[r]];
-                d.sink_leaf = h_leaves + off;
-                d.leaf_pitch = cols;
-                off += d.shape.T;
+                d.sink = h_out + off;
+                d.sink_pitch = pitch;
+                off += row_bytes(d, Walk::Leaf);
             }
+        } else {                                         // the scores are combined on the host device
+            h.sink = h_out;
+            h.sink_pitch = row_bytes(h, h.walk);
         }
         if (sp) {
             const size_t chunk = h.cap_tuples;
@@ -1111,20 +1094,17 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
     } else {
         // chunks round-robin over the devices; with several devices each one is fed by its own host thread (one
         // thread cannot issue the ~25 runtime calls per chunk fast enough for 8 PCIe links)
-        const size_t chunk = e->devs[0].cap_tuples, G = e->devs.size(), C = classes_of(e);
+        const size_t chunk = e->devs[0].cap_tuples, G = e->devs.size();
         auto feed = [&](size_t g) -> int {
             Dev& d = e->devs[g];
+            const size_t row = row_bytes(d, d.walk);
             int r = DTE_OK;
             size_t i = g;
             for (size_t off = g * chunk; off < n && !r; off += G * chunk, i += G) {
                 const size_t cnt = std::min(chunk, n - off);
-                d.sink_sc = h_scores ? h_scores + off * C : nullptr;      // scores are [n][C]
+                d.sink = h_out + off * row;
+                d.sink_pitch = row;
                 d.sink_lb = h_labels ? h_labels + off : nullptr;
-                if (h_leaves) {
-                    d.sink_leaf = h_leaves + off * d.shape.T;
-                    d.leaf_pitch = d.shape.T;
-                }
-                if (h_contribs) d.sink_contrib = h_contribs + off * d.shape.C * (d.shape.g.F() + 1);
                 r = sp ? land_sparse_dev(e, d, *sp, off, cnt) : land_dev(e, d, h_tuples + off * tb, cnt * tb);
                 if (!r && d.slot[d.cur].fill) {          // a short last chunk, or any sparse chunk
                     r = submit_dev(e, d, d.cur);
@@ -1156,7 +1136,7 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
         cudaSetDevice(d.ordinal);
         if (cudaEventElapsedTime(&ms, d.ev_t0, d.ev_t1) == cudaSuccess) d.last_walk_ms = ms;
         ms_max = std::max(ms_max, ms);
-        d.sink_sc = nullptr; d.sink_lb = nullptr; d.sink_leaf = nullptr; d.sink_contrib = nullptr;
+        d.sink = nullptr; d.sink_lb = nullptr;
         d.res_enq = d.res_done = enq0[i];            // direct-sink results are not part of the line-stream queue
     }
     e->last_walk_ms = ms_max;
@@ -1168,11 +1148,11 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, float
 // Host buffers in, host buffers out (fast path, no line framing): the same landing pipeline with the caller's
 // buffers as the direct sink.  Multi-device: chunks round-robin over the devices (trees replicated) or every chunk
 // broadcast to all of them (tree chunks + ring combine).  A binned walk lands u8 bins [n][F] (F bytes per tuple through
-// the same landing slots); a leaf walk returns cells into h_leaves, no scores, no labels; a contribution walk returns
-// [n][C][F + 1] into h_scores, no labels.  sp: fp32 rows densified on the device from sparse rows (h_tuples unused).
-// `what` names the call.
-int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_tuples, size_t n, float* h_scores,
-               uint8_t* h_labels, uint16_t* h_leaves, const SparseRows* sp = nullptr) {
+// the same landing slots).  h_out receives the walk's rows: scores [n][C], leaf cells [n][T] or contributions
+// [n][C][F + 1]; only score walks return labels.  sp: fp32 rows densified on the device from sparse rows (h_tuples
+// unused).  `what` names the call.
+int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_tuples, size_t n, void* h_out,
+               uint8_t* h_labels, const SparseRows* sp = nullptr) {
     Geom g;
     TRY(decode_geom(e, g));
     if (e->state == dte_engine::ST_TREES) return fail(e, DTE_ERR_STATE, "%s while the tree stream is being received", what);
@@ -1189,34 +1169,25 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
     const uint32_t F = g.F();
     size_t cap = default_chunk(e, F);
-    if (w == Walk::Leaf) {
-        // The cells of a slot (2T bytes per tuple) may take at most twice the tuple budget, so a many-tree, few-feature
-        // ensemble lands fewer tuples per slot instead of allocating GiBs of cells.
-        uint32_t tmax = 1;
-        for (const Dev& d : e->devs) tmax = std::max(tmax, d.shape.T);
+    if (row_walk(w)) {
+        // The rows of a slot (2T bytes per tuple for leaf cells, 4 C (F + 1) for contributions: 2 MiB at C = 256,
+        // F = 2048) may take at most twice the tuple budget, so a many-tree or many-feature ensemble lands fewer tuples
+        // per slot instead of allocating GiBs of rows.
+        size_t row = 1;
+        for (const Dev& d : e->devs) row = std::max(row, row_bytes(d, w));
         const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
-        cap = std::min(cap, std::max<size_t>(4, budget / (2 * (size_t)tmax)) & ~(size_t)3);
-    }
-    if (w == Walk::Contrib) {
-        // the same bound on a slot's contribution rows (4 C (F + 1) bytes per tuple: 2 MiB at C = 256, F = 2048)
-        const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
-        const size_t row = (size_t)4 * classes_of(e) * (F + 1);
         cap = std::min(cap, std::max<size_t>(4, budget / row) & ~(size_t)3);
     }
     for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
-    if (w == Walk::Leaf)
-        for (Dev& d : e->devs) TRY(ensure_leaf_slots(e, d));
-    if (w == Walk::Contrib)
-        for (Dev& d : e->devs) TRY(ensure_contrib_slots(e, d));
+    if (row_walk(w))
+        for (Dev& d : e->devs) TRY(ensure_row_slots(e, d, w));
     if (sp) {                                        // every chunk is a slot: the scratch holds the largest one's entries
         size_t nnz = 0;
         for (size_t r = 0; r < n; r += cap) nnz = std::max(nnz, (size_t)(sp->indptr[std::min(n, r + cap)] - sp->indptr[r]));
         for (Dev& d : e->devs) TRY(ensure_sparse_slots(e, d, nnz));
     }
     for (Dev& d : e->devs) d.walk = w;
-    const bool contrib = w == Walk::Contrib;
-    const int rc = infer_host_run(e, h_tuples, n, contrib ? nullptr : h_scores, contrib ? nullptr : h_labels, h_leaves,
-                                  contrib ? h_scores : nullptr, sp);
+    const int rc = infer_host_run(e, h_tuples, n, static_cast<unsigned char*>(h_out), h_labels, sp);
     for (Dev& d : e->devs) {                         // the next call may land another kind: leave no slot partly filled
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
         d.walk = Walk::Fp32;
@@ -1843,13 +1814,13 @@ int dte_ipc_close(dte_t* e, void* d_ptr, int owner) {
 
 int dte_infer_host(dte_t* e, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
     if (!e || (n && (!h_tuples || !h_scores))) return DTE_ERR_ARG;
-    return infer_host(e, Walk::Fp32, "infer_host", static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels, nullptr);
+    return infer_host(e, Walk::Fp32, "infer_host", static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels);
 }
 
 // ---- binned inference (DESIGN.md §9) ----
 int dte_infer_host_binned(dte_t* e, const void* h_bins, size_t n, float* h_scores, uint8_t* h_labels) {
     if (!e || (n && (!h_bins || !h_scores))) return DTE_ERR_ARG;
-    return infer_host(e, Walk::Binned, "infer_host", static_cast<const unsigned char*>(h_bins), n, h_scores, h_labels, nullptr);
+    return infer_host(e, Walk::Binned, "infer_host", static_cast<const unsigned char*>(h_bins), n, h_scores, h_labels);
 }
 
 int dte_infer_device_binned(dte_t* e, const void* d_bins, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream) {
@@ -1901,7 +1872,7 @@ int dte_infer_device_leaves(dte_t* e, const void* d_tuples, size_t n, uint16_t* 
 
 int dte_infer_host_leaves(dte_t* e, const void* h_tuples, size_t n, uint16_t* h_leaves) {
     if (!e || (n && (!h_tuples || !h_leaves))) return DTE_ERR_ARG;
-    return infer_host(e, Walk::Leaf, "infer_host_leaves", static_cast<const unsigned char*>(h_tuples), n, nullptr, nullptr, h_leaves);
+    return infer_host(e, Walk::Leaf, "infer_host_leaves", static_cast<const unsigned char*>(h_tuples), n, h_leaves, nullptr);
 }
 
 int dte_kernel_name_leaves(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Leaf, buf, len); }
@@ -1914,8 +1885,7 @@ int dte_infer_device_contribs(dte_t* e, const void* d_tuples, size_t n, float* d
 
 int dte_infer_host_contribs(dte_t* e, const void* h_tuples, size_t n, float* h_contribs) {
     if (!e || (n && (!h_tuples || !h_contribs))) return DTE_ERR_ARG;
-    return infer_host(e, Walk::Contrib, "infer_host_contribs", static_cast<const unsigned char*>(h_tuples), n, h_contribs, nullptr,
-                      nullptr);
+    return infer_host(e, Walk::Contrib, "infer_host_contribs", static_cast<const unsigned char*>(h_tuples), n, h_contribs, nullptr);
 }
 
 int dte_kernel_name_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Contrib, buf, len); }
@@ -2037,7 +2007,7 @@ int dte_infer_host_sparse(dte_t* e, const int64_t* h_indptr, const uint32_t* h_i
     TRY(decode_geom(e, g));
     SparseRows sp{indptr, h_indices, h_values, 0, {is_pageable(h_indptr), is_pageable(h_indices), is_pageable(h_values)}};
     TRY(absent_word(e, what, absent, g, sp.absent));
-    return infer_host(e, Walk::Fp32, what, nullptr, n, h_scores, h_labels, nullptr, &sp);
+    return infer_host(e, Walk::Fp32, what, nullptr, n, h_scores, h_labels, &sp);
 }
 
 int dte_host_alloc(dte_t* e, size_t bytes, void** h_ptr) {

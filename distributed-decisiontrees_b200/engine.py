@@ -348,15 +348,19 @@ class Engine:
         self._check(self._lib.dte_infer_device(self._h, _ptr(d_tuples), int(n), _ptr(d_scores), _ptr(d_labels),
                                                _stream(stream)))
 
+    def _score_outputs(self, n, want_labels, out_scores, out_labels):
+        """The (scores, labels) a host-buffer score call of n tuples writes: the caller's arrays, else new ones."""
+        if out_scores is None:
+            nc = self.num_classes()
+            out_scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
+        if out_labels is None and want_labels:
+            out_labels = np.empty(n, dtype=np.uint8)
+        return out_scores, out_labels
+
     def _infer_host(self, fn, rows, dtype, want_labels, out_scores, out_labels):
         """Allocate the outputs of a host-buffer score call and run it -> (scores, labels)."""
         t, n = _host_rows(rows, dtype)
-        if out_scores is None:
-            nc = self.num_classes()
-            scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
-        else:
-            scores = out_scores
-        labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
+        scores, labels = self._score_outputs(n, want_labels, out_scores, out_labels)
         self._check(fn(self._h, _ptr(t), n, _ptr(scores), _ptr(labels)))
         return scores, labels
 
@@ -442,12 +446,7 @@ class Engine:
         from . import layout
         indptr, indices, values = layout.sparse_arrays(X)
         n = int(indptr.shape[0]) - 1
-        if out_scores is None:
-            nc = self.num_classes()
-            scores = np.empty(n, dtype=np.float32) if nc == 1 else np.empty((n, nc), dtype=np.float32)
-        else:
-            scores = out_scores
-        labels = out_labels if out_labels is not None else (np.empty(n, dtype=np.uint8) if want_labels else None)
+        scores, labels = self._score_outputs(n, want_labels, out_scores, out_labels)
         self._check(self._lib.dte_infer_host_sparse(self._h, _ptr(indptr), _ptr(indices), _ptr(values), n, _absent(absent),
                                                     _ptr(scores), _ptr(labels)))
         return scores, labels

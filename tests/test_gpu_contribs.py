@@ -211,6 +211,25 @@ def test_tuple_counts(torch_cuda, n):
         check_all(torch_cuda, e, x, want, 1, F, what="n=%d" % n)
 
 
+def test_many_classes_wide_rows(torch_cuda):
+    """C = 16, F = 512: a tuple's contributions take 32,832 bytes, so the host call lands at most twice the tuple budget
+    in rows per slot (4,088 tuples), and the rows of 9,000 tuples come back from three slots in order, word for word
+    those of the device call."""
+    C, T, D, F, n = 16, 32, 3, 512, 9000
+    W, FI = L.synth_ensemble(T, D, F, seed=795)
+    cov = L.synth_covers(FI, D, seed=796)
+    x = L.synth_tuples(0, n, F, seed=797, missing_ppm=20000)
+    wl, fl = L.pack_streams(W, FI, D)
+    with make_engine(T, D, F) as e:
+        e.load_ensemble(wl, fl, num_classes=C, covers=cov)
+        assert e.kernel_name_contribs().startswith("dt_shap_generic<")
+        want = device_contribs(torch_cuda, e, x, C, F)
+        launches = e.info()["kernel_launches"]
+        got = e.infer_host_contribs(x)
+        assert e.info()["kernel_launches"] - launches == 3       # one dt_shap_generic launch per slot
+        assert_words(got, want, "C=16 F=512 host")
+
+
 @pytest.mark.parametrize("mode", ["data", "ensemble"])
 def test_multi_device_handles(torch_cuda, mode):
     """[0, 0, 0]: a Dealt handle returns the single handle's rows in global order; a Chunked handle refuses."""
