@@ -144,10 +144,11 @@ inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& liv
 //   +16  u64    stepmap      bits 4s..4s+3: the element (0-based) of step s, s = 0 the root step
 //   +24  u16    feat[Dmax]   feature of each element
 //   +zoff double z[Dmax]     zero fraction of each element
+//   +izoff double iz[Dmax]   1 / z of each element (read only where z > 1, by the bottom-up unwinding)
 // Nodes: per layout tree [2^D - 1] {thr word, fidx | missing_right << 16}; only the ancestors of end cells are read.
 struct ShapLayout {
     uint32_t D = 0, M = 0;               // levels; longest merged path of the layout
-    uint32_t stride = 0, zoff = 0;       // bytes per path record, offset of z in it
+    uint32_t stride = 0, zoff = 0, izoff = 0;   // bytes per path record, offsets of z and 1 / z in it
     uint32_t n_nodes = 0;                // 2^D - 1
     uint32_t C = 1;
     std::vector<uint2> nodes;            // [Tl][n_nodes], layout trees class-major, stream order inside a class
@@ -182,7 +183,8 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
     out = ShapLayout();
     out.D = D; out.C = classes; out.n_nodes = n_int;
     out.zoff = (24u + 2u * D + 7u) & ~7u;
-    out.stride = (out.zoff + 8u * D + 15u) & ~15u;
+    out.izoff = out.zoff + 8u * D;
+    out.stride = (out.izoff + 8u * D + 15u) & ~15u;
     std::vector<uint32_t> order;                     // layout tree -> local tree, class-major
     out.cls_tree.assign(classes + 1, 0);
     for (uint32_t c = 0; c < classes; ++c) {
@@ -256,7 +258,9 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
             for (uint32_t e = 0; e < m; ++e) {
                 const uint16_t f16 = (uint16_t)efeat[e];
                 memcpy(r + 24 + 2 * e, &f16, 2);
+                const double iz = 1.0 / ez[e];
                 memcpy(r + out.zoff + 8 * e, &ez[e], 8);
+                memcpy(r + out.izoff + 8 * e, &iz, 8);
             }
             out.M = std::max(out.M, m);
         }
@@ -863,7 +867,7 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     p.tree_path = d.d_shap_tree_path;
     p.cls_tree = d.d_shap_cls_tree;
     p.F = F; p.C = C; p.missing = run.missing;
-    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff;
+    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff; p.izoff = d.shap.izoff;
     p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
     const ShapPlan pl = shap_plan(d, want_variant);
     const ShapKernel k = shap_kernel(pl);

@@ -369,6 +369,7 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
         TRY(upload(e, d.d_shap_cls_tree, shap->cls_tree));
         d.ensemble_bytes += shap->bytes();
         d.shap.D = shap->D; d.shap.M = shap->M; d.shap.stride = shap->stride; d.shap.zoff = shap->zoff;
+        d.shap.izoff = shap->izoff;
         d.shap.n_nodes = shap->n_nodes; d.shap.C = shap->C;
     }
     return DTE_OK;

@@ -17,16 +17,21 @@
 //       if o_l: w[j+1] = w[j+1] + w[j] * Q[l][j]                 Q[l][j]  = (j+1) / (l+1)
 //       w[j] = (z_l * w[j]) * R[l][j]                             R[l][j]  = (l-j) / (l+1)
 //   for i = 1..m (element order), l = m:
-//       o_i = 1: next = w[m]; total = 0; for j = m-1..0:
+//       o_i = 1, z_i <= 1: next = w[m]; total = 0; for j = m-1..0:
 //                  tmp = next * IQ[m][j]; total = total + tmp;    IQ[l][j] = (l+1) / (j+1)
 //                  next = w[j] - (tmp * z_i) * R[m][j]
-//                contrib = (total * (1 - z_i)) * v
+//       o_i = 1, z_i > 1: u = 0; total = 0; for j = 0..m-1:
+//                  u = ((j ? w[j] - Q[m][j-1] * u : w[0]) * iz_i) * IR[m][j]; total = total + u
+//                contrib = (total * (1 - z_i)) * v                 (both o_i = 1 forms)
 //       o_i = 0: total = 0; for j = m-1..0: total = total + w[j] * IR[m][j]     IR[l][j] = (l+1) / (l-j)
 //                contrib = total * (-v)
 //       phi[f_i] = phi[f_i] + contrib
 //   phi[F] = phi[F] + bz, bz = v * (((z_1 * z_2) * ...) * z_m) computed on the host at load time
-// v = the fp32 leaf word W[t][cell] as double.  Lundberg's UNWOUND_SUM with o in {0, 1}: the o = 0 branch is
-// (w[j] / z) / ((l-j)/(l+1)) times (0 - z), which is exactly -w[j] * (l+1)/(l-j) before rounding, so z cancels there.
+// v = the fp32 leaf word W[t][cell] as double, iz_i = 1 / z_i rounded once on the host.  Lundberg's UNWOUND_SUM with o
+// in {0, 1}: the o = 0 branch is (w[j] / z) / ((l-j)/(l+1)) times (0 - z), which is exactly -w[j] * (l+1)/(l-j) before
+// rounding, so z cancels there.  For o = 1 both forms undo the extension w[j] = z R[m][j] u[j] + Q[m][j-1] u[j-1]: from
+// the top each step scales the error of u by z (m-j)/(j+1), from the bottom by j / (z (m-j)), so the top-down division is
+// stable for z <= 1 and the bottom-up one for z > 1 (a child whose cover exceeds its parent's); DESIGN.md §12.
 // Order: trees in stream order (class-major for C >= 2), a tree's paths in increasing end cell, elements in path order;
 // one __double2float_rn per word at the end.
 #pragma once
@@ -62,7 +67,7 @@ struct ShapParams {
     unsigned long long n;
     unsigned long long scratch_rows;
     uint32_t F, C, missing;
-    uint32_t n_nodes, stride, zoff;
+    uint32_t n_nodes, stride, zoff, izoff;
     uint32_t trees0;                    // C = 1: layout trees the run adds (min(T, 8 S K))
     uint32_t groups;                    // tile: tuple groups (warps) per CTA
 };
@@ -115,6 +120,7 @@ __device__ __forceinline__ void shap_group(const ShapParams& p, const Acc& phi, 
                 const uint32_t m = (vm.y >> 16) & 0xFFu, L = vm.y >> 24;
                 const uint16_t* feat = reinterpret_cast<const uint16_t*>(rec + 24);
                 const double* zs = reinterpret_cast<const double*>(rec + p.zoff);
+                const double* izs = reinterpret_cast<const double*>(rec + p.izoff);
                 // o bits: clear element e where x leaves the path at a step of e
                 uint32_t ones = 0xFFFFu;
                 uint32_t n = vm.y & 0xFFFFu;
@@ -150,15 +156,27 @@ __device__ __forceinline__ void shap_group(const ShapParams& p, const Acc& phi, 
                     const double z = __ldg(zs + i);
                     const bool o = (ones >> i) & 1u;
                     double total = 0.0, next = wm;
+                    if (o && z > 1.0) {                     // z is the path's (warp-uniform), o the lane's
+                        const double iz = __ldg(izs + i);
 #pragma unroll
-                    for (int j = M - 1; j >= 0; --j) {
-                        if (j < (int)m) {
-                            if (o) {
-                                const double tmp = __dmul_rn(next, c_shap_tab[2][m][j]);
-                                total = __dadd_rn(total, tmp);
-                                next = __dsub_rn(w[j], __dmul_rn(__dmul_rn(tmp, z), c_shap_tab[1][m][j]));
-                            } else {
-                                total = __dadd_rn(total, __dmul_rn(w[j], c_shap_tab[3][m][j]));
+                        for (int j = 0; j < M; ++j) {
+                            if (j < (int)m) {
+                                const double num = j ? __dsub_rn(w[j], __dmul_rn(c_shap_tab[0][m][j ? j - 1 : 0], next)) : w[0];
+                                next = __dmul_rn(__dmul_rn(num, iz), c_shap_tab[3][m][j]);
+                                total = __dadd_rn(total, next);
+                            }
+                        }
+                    } else {
+#pragma unroll
+                        for (int j = M - 1; j >= 0; --j) {
+                            if (j < (int)m) {
+                                if (o) {
+                                    const double tmp = __dmul_rn(next, c_shap_tab[2][m][j]);
+                                    total = __dadd_rn(total, tmp);
+                                    next = __dsub_rn(w[j], __dmul_rn(__dmul_rn(tmp, z), c_shap_tab[1][m][j]));
+                                } else {
+                                    total = __dadd_rn(total, __dmul_rn(w[j], c_shap_tab[3][m][j]));
+                                }
                             }
                         }
                     }

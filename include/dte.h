@@ -240,7 +240,10 @@ int dte_kernel_name_leaves(dte_t* engine, char* buf, size_t len);
  * Shapley value of feature f summed over the class-c trees, contribs[i][c][F] the bias sum_t v_t({}), so a row sums to the
  * score up to rounding.  The trees are those the score walk adds: the first min(T, 8*S*K) local trees of a single-class
  * ensemble, every tree of a multi-class one.  Computed in fp64 with every operation rounded on its own in the order
- * DESIGN.md §12 fixes, then rounded once to fp32, so every word is reproducible.  Layout [n][C][F+1] fp32. */
+ * DESIGN.md §12 fixes, then rounded once to fp32, so every word is reproducible.  Before that rounding each value is
+ * within 2^-40 sum_p |v_p| prod_e max(1, z_e) of the exact one (p the class's end cells, v_p its leaf value, z_e the cover
+ * fraction of each feature on the path), for any positive covers, including children above their parent (§12).
+ * Layout [n][C][F+1] fp32. */
 /* dte_load_ensemble_classes (same placement), and in addition the contribution layout.  covers: fp32
  * [T_all][2^(D+1)-1] for every tree of the streams, indexed like the weight heap (XGBoost cover / sum_hessian, LightGBM
  * internal_count / leaf_count, scikit-learn weighted_n_node_samples).  Only live internal nodes (not below an early leaf)

@@ -165,8 +165,9 @@ def shap_tables():
 
 def tree_paths(W_t, FI_t, cov_t, D):
     """The path records of one tree, as the layout builder makes them, in increasing end cell:
-    dict(cells [P], v fp64 [P], m [P], L [P], feat [P, D], z fp64 [P, D], nodes [P, D] (the node of step s, root first,
-    -1 past L), right [P, D] (the path's direction at step s), elem [P, D] (element of step s), bz fp64 [P])."""
+    dict(cells [P], v fp64 [P], m [P], L [P], feat [P, D], z fp64 [P, D], iz fp64 [P, D] (1 / z), nodes [P, D] (the node
+    of step s, root first, -1 past L), right [P, D] (the path's direction at step s), elem [P, D] (element of step s),
+    bz fp64 [P])."""
     cells = np.array(end_cells(FI_t, D), dtype=np.int64)
     P = cells.size
     L = np.floor(np.log2(cells + 1)).astype(np.int64)                # depth of the cell = steps
@@ -204,7 +205,7 @@ def tree_paths(W_t, FI_t, cov_t, D):
     zp = z[:, 0].copy()
     for e in range(1, D):
         zp = np.where(e < m, zp * z[:, e], zp)
-    return dict(cells=cells, v=v, m=m, L=L, feat=feat, z=z, nodes=nodes, right=right, elem=elem, bz=v * zp)
+    return dict(cells=cells, v=v, m=m, L=L, feat=feat, z=z, iz=1.0 / z, nodes=nodes, right=right, elem=elem, bz=v * zp)
 
 
 def _tree_contribs(W_t, FI_t, cov_t, D, x, missing, tab):
@@ -246,6 +247,7 @@ def _tree_contribs(W_t, FI_t, cov_t, D, x, missing, tab):
             continue
         zi = z[:, i][None, :]
         o = ones[:, :, i]
+        up = o & (zi > 1.0)                                         # o = 1 and z > 1: the bottom-up division
         total = np.zeros((n, P))
         nxt = wm.copy()
         for j in range(D - 1, -1, -1):
@@ -254,8 +256,16 @@ def _tree_contribs(W_t, FI_t, cov_t, D, x, missing, tab):
             t1 = total + tmp
             n1 = w[:, :, j] - (tmp * zi) * tab[1, m, j][None, :]
             t0 = total + w[:, :, j] * tab[3, m, j][None, :]
-            total = np.where(a, np.where(o, t1, t0), total)
+            total = np.where(a & ~up, np.where(o, t1, t0), total)
             nxt = np.where(a & o, n1, nxt)
+        izi = pr["iz"][:, i][None, :]
+        u = np.zeros((n, P))
+        for j in range(D):
+            a = (j < m)[None, :] & up
+            num = w[:, :, j] - tab[0, m, j - 1][None, :] * u if j else w[:, :, 0]
+            u1 = (num * izi) * tab[3, m, j][None, :]
+            u = np.where(a, u1, u)
+            total = np.where(a, total + u1, total)
         c = np.where(o, (total * (1.0 - zi)) * v[None, :], total * (-v)[None, :])
         out[:, :, i] = np.where(act_i[None, :], c, 0.0)
     return out, pr["feat"], m, pr["bz"]

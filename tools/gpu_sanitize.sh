@@ -58,9 +58,11 @@ for T in tests/test_gpu_sparse.py::test_sparse_to_dense_device_bytes "tests/test
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_sparse_${stag}.log"
 done
 # the contribution kernels (dt_shap_tile with two tuple groups per CTA, dt_shap_generic at a width only it serves and in
-# two launches through its fp64 scratch) and the ragged tail of a warp
+# two launches through its fp64 scratch), the ragged tail of a warp, and both <15> kernels on D = 15 paths of 15 elements
+# with the bottom-up unwinding (covers above their parent's)
 for T in tests/test_gpu_contribs.py::test_headline_geometry tests/test_gpu_contribs.py::test_generic_only_width \
-         tests/test_gpu_contribs.py::test_generic_launches_in_chunks "tests/test_gpu_contribs.py::test_tuple_counts[33]"; do
+         tests/test_gpu_contribs.py::test_generic_launches_in_chunks "tests/test_gpu_contribs.py::test_tuple_counts[33]" \
+         "tests/test_gpu_contribs_deep.py::test_leafwise_merged_lengths[m15-D15-free]"; do
   ctag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_contribs_${ctag}.log"
 done
