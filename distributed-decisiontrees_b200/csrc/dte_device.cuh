@@ -670,6 +670,22 @@ inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
     return (phased && fits && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
+// make_plan scores plans by walks in flight; it cannot see that the bottom-record gather slows down once the tuple tile
+// leaves it too little L1 (DESIGN.md §4).  A handle configured for a large workload therefore times the staged
+// candidates at load and runs the fastest when it beats make_plan's choice by kPlanMargin (DESIGN.md §4, "Measured
+// plans").  The timing takes about half a second of GPU time at cfg3, so it waits for a workload hint of
+// kMeasureHintTuples tuples (reg 207).
+constexpr uint64_t kMeasureHintTuples = 8000000;
+constexpr double kPlanMargin = 0.02;
+inline bool tune_pinned(const Tune& t) {
+    return t.ilp || t.stages || t.warps || t.pair || t.fill || t.phased != -1;
+}
+// Whether loading an ensemble times the plans: only on a single-device handle whose plan no DTE_TUNE knob pins and no
+// forced kernel variant overrides, configured for at least kMeasureHintTuples tuples.
+inline bool measure_plan_at_load(const Tune& tune, int forced_variant, bool multi, uint64_t hint_tuples) {
+    return !multi && !tune_pinned(tune) && forced_variant == KERNEL_AUTO && hint_tuples >= kMeasureHintTuples;
+}
+
 using WalkKernel = void (*)(WalkParams);
 // The instantiation of family R with the given WIDE, MC and BIN flags and thread bound nt (Plan::thread_bound)
 template <int R, bool WIDE, bool MC, bool BIN>

@@ -73,7 +73,9 @@ struct dte_engine {
     std::vector<Dev> devs;            // devs[d] = device ID d of devices_list = d-th ordinal given at create
     int pos2dev[kMaxRing];            // ring position -> index into devs (registers 208-210), decoded at start
     uint32_t node_index = 0;          // single-device handle: the ring position this engine stands for (dte_set_node)
-    Tune tune;
+    Tune tune;                        // DTE_TUNE's knobs, or the plan dte_autotune pinned
+    std::optional<Tune> measured;     // the fp32 plan timed fastest at load, when it beat make_plan's (measure_plan_at_load)
+    bool autotuned = false;           // dte_autotune chose `tune`
     int forced_variant = KERNEL_AUTO;
     std::string err;
 
@@ -412,6 +414,7 @@ int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_
         TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins, covers ? &shap[chunked ? r : 0] : nullptr));
     }
     e->bins = bins ? *bins : BinEdges();
+    e->measured.reset();              // a plan measured on the previous ensemble says nothing about this one
     e->placed = e->part;
     memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
     return DTE_OK;
@@ -594,6 +597,12 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
     return DTE_OK;
 }
 
+// The knobs the next walk of kind w is planned with: the plan measured at load for an fp32 walk of the default variant,
+// else DTE_TUNE's (or dte_autotune's pin).  The measured plan was timed for the fp32 walk only.
+const Tune& walk_tune(const dte_engine* e, Walk w) {
+    return e->measured && w == Walk::Fp32 && e->forced_variant == KERNEL_AUTO ? *e->measured : e->tune;
+}
+
 // Launch the walk of kind w over n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.  `out`
 // receives the scores [n][C] (labels too when given), for a leaf walk the cells [n][T], for a contribution walk the
 // contributions [n][C][F + 1].
@@ -603,7 +612,7 @@ int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, vo
     const cudaError_t rc =
         w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
         : w == Walk::Contrib ? launch_contrib(d, e->g, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
-                             : launch_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
+                             : launch_walk(d, e->g, walk_tune(e, w), e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
     if (rc != cudaSuccess)
         return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s",
                     w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : "walk kernel", why ? why : cudaGetErrorString(rc));
@@ -1661,6 +1670,121 @@ int dte_process_done(dte_t* e, int* done) {
     return DTE_OK;
 }
 
+// A launch plan timed on the resident ensemble: its knobs, the kernel it launches and its median rate.
+struct PlanTiming {
+    Tune tune;
+    std::string name;
+    double tuples_per_ms = 0;
+};
+
+// Time the fp32 walk of the resident ensemble on device d under `base` and under each staged candidate that fits and
+// plans a launch not yet timed, on synthetic tuples generated on the device; out[0] is `base`.  Every plan walks the
+// largest whole number of its own waves of tiles that fits in max(n, 2 waves) tuples, since a partial last wave would
+// charge plans with smaller tiles for idle SMs.  One round of launches warms up, then kPlanReps rounds visit the plans
+// in turn; a plan's rate is its median.
+constexpr int kPlanReps = 3;
+static int time_plans(dte_t* e, Dev& d, const Tune& base, size_t n, std::vector<PlanTiming>& out) {
+    struct Cand { int row, stages, phased, warps; };            // warps = 10: the 384-thread (168-register) instantiation
+    const int r42 = tile_row(4, 2, true), r24 = tile_row(2, 4, true), r81 = tile_row(8, 1, true), r41 = tile_row(4, 1, true),
+              r22 = tile_row(2, 2, true);
+    // the last three cap the tuple tile at 4 or 5 groups, which leaves the bottom-record gather more L1 (DESIGN.md §4)
+    const Cand cands[] = {{r42, 1, 1, 0}, {r42, 1, 0, 0}, {r42, 1, 1, 10}, {r42, 1, 0, 10}, {r24, 1, 1, 0}, {r24, 1, 0, 0}, {r81, 1, 0, 0},
+                          {r81, 2, 0, 0}, {r41, 2, 0, 0}, {r22, 2, 0, 0}, {r22, 1, 0, 0}, {r42, 1, 1, 8}, {r22, 1, 1, 10},
+                          {r24, 1, 1, 16}};
+    char name[256];
+    out.clear();
+    out.push_back({base, "", 0});
+    for (const Cand& c : cands) {
+        const TileFamily& f = kTileFamilies[c.row];
+        // the planner stages a pinned family only with >= 2 consumer warps, and a cap is only worth timing when it
+        // removes a tuple group; a plan that stages can always refill phased (Dtop >= 3, at most 4 stages)
+        const int groups = tile_groups(d, f, c.stages, c.warps);
+        if (groups * f.pair < 2 || (c.warps && tile_groups(d, f, c.stages, 0) * f.pair <= c.warps)) continue;
+        Tune t = base;
+        t.ilp = f.ilp; t.pair = f.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps;
+        out.push_back({t, "", 0});
+    }
+    size_t wave_max = 0;
+    std::vector<size_t> waves;
+    for (PlanTiming& p : out) {
+        kernel_name(d, p.tune, KERNEL_AUTO, name, sizeof name);
+        p.name = name;
+        waves.push_back((size_t)make_plan(d, p.tune, KERNEL_AUTO).tuples_per_cta() * d.sm_count);
+        wave_max = std::max(wave_max, waves.back());
+    }
+    for (size_t i = out.size(); i-- > 1;)                    // the same launch twice is timed once (base stays)
+        for (size_t j = 0; j < i; ++j)
+            if (out[j].name == out[i].name) { out.erase(out.begin() + i); waves.erase(waves.begin() + i); break; }
+    n = std::max(n, 2 * wave_max);
+    const uint32_t F = d.shape.g.F();
+    CUDA_TRY(e, cudaSetDevice(d.ordinal));
+    void* d_x = nullptr;
+    float* d_s = nullptr;
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    std::vector<float> ms(out.size() * kPlanReps);
+    int rc = DTE_OK;
+    if (cudaMalloc(&d_x, n * F * 4) != cudaSuccess || cudaMalloc(&d_s, n * d.shape.C * 4) != cudaSuccess) {
+        cudaGetLastError();                              // not sticky: the next launch's check must not see it
+        rc = fail(e, DTE_ERR_NOMEM, "timing the launch plans: out of device memory for %zu tuples", n);
+    }
+    else if (cudaEventCreate(&ev[0]) != cudaSuccess || cudaEventCreate(&ev[1]) != cudaSuccess)
+        rc = fail(e, DTE_ERR_CUDA, "timing the launch plans: cudaEventCreate failed");
+    if (!rc)
+        synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n * F,
+                                                                             0x7091E5ull, 10000u, e->g.missing);
+    for (int round = -1; round < kPlanReps && !rc; ++round)
+        for (size_t i = 0; i < out.size() && !rc; ++i) {
+            const char* why = nullptr;
+            cudaEventRecord(ev[0], d.s_main);
+            const cudaError_t st = launch_walk(d, e->g, out[i].tune, KERNEL_AUTO, d_x, n / waves[i] * waves[i], d_s, nullptr,
+                                               d.s_main, false, &why);
+            cudaEventRecord(ev[1], d.s_main);
+            if (st != cudaSuccess || cudaEventSynchronize(ev[1]) != cudaSuccess) {
+                rc = fail(e, DTE_ERR_CUDA, "timing %s: launch failed: %s", out[i].name.c_str(), why ? why : cudaGetErrorString(st));
+                break;
+            }
+            if (round >= 0) cudaEventElapsedTime(&ms[i * kPlanReps + round], ev[0], ev[1]);
+        }
+    for (size_t i = 0; i < out.size() && !rc; ++i) {
+        float* m = &ms[i * kPlanReps];
+        std::sort(m, m + kPlanReps);
+        out[i].tuples_per_ms = (double)(n / waves[i] * waves[i]) / m[kPlanReps / 2];
+    }
+    for (cudaEvent_t x : ev)
+        if (x) cudaEventDestroy(x);
+    cudaFree(d_x);
+    cudaFree(d_s);
+    return rc;
+}
+
+// After a load on a handle that measure_plan_at_load admits: time the staged candidates on synthetic tuples and keep the
+// fastest for the fp32 walk when it beats make_plan's choice by kPlanMargin.  Reports the choice and its cost on stderr.
+static int choose_measured_plan(dte_t* e) {
+    const uint64_t hint = 4 * (e->regs[7] & 0xFFFFFFFFull);                    // reg 207[31:0]: result lines of 4 tuples
+    if (!measure_plan_at_load(e->tune, e->forced_variant, e->multi(), hint)) return DTE_OK;
+    Dev& d = e->devs[0];
+    if (make_plan(d, e->tune, KERNEL_AUTO).variant() != KERNEL_TILE_STAGED) return DTE_OK;   // nothing staged to choose
+    const Clock::time_point t0 = Clock::now();
+    std::vector<PlanTiming> t;
+    const size_t n = std::min<size_t>((size_t)1 << 19, ((size_t)512 << 20) / (d.shape.g.F() * 4));   // ~9 ms per launch at cfg3
+    const int rc = time_plans(e, d, e->tune, n, t);
+    if (rc == DTE_ERR_NOMEM) {                                                  // the built-in plan still runs
+        fprintf(stderr, "dte: launch plan kept: %s\n", e->err.c_str());
+        e->err.clear();
+        return DTE_OK;
+    }
+    TRY(rc);
+    const PlanTiming* best = &t[0];
+    for (const PlanTiming& p : t)
+        if (p.tuples_per_ms > best->tuples_per_ms) best = &p;
+    const bool better = best->tuples_per_ms >= t[0].tuples_per_ms * (1 + kPlanMargin);
+    if (better) e->measured = best->tune;
+    fprintf(stderr, "dte: launch plan %s %s (%.1f M tuples/s; built-in %.1f M) after timing %zu plans in %.0f ms\n",
+            better ? "measured" : "kept", (better ? best : &t[0])->name.c_str(), best->tuples_per_ms * 1e-3,
+            t[0].tuples_per_ms * 1e-3, t.size(), std::chrono::duration<double, std::milli>(Clock::now() - t0).count());
+    return DTE_OK;
+}
+
 // dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
 // is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
@@ -1703,7 +1827,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
-    return DTE_OK;
+    return choose_measured_plan(e);
 }
 
 int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1765,7 +1889,7 @@ static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
     if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
     if (w == Walk::Contrib) contrib_kernel_name(e->devs[0], e->forced_variant, buf, len);
-    else kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len, w);
+    else kernel_name(e->devs[0], walk_tune(e, w), e->forced_variant, buf, len, w);
     return DTE_OK;
 }
 
@@ -1967,7 +2091,7 @@ int dte_infer_device_sparse(dte_t* e, const int64_t* d_indptr, const uint32_t* d
     const uint32_t F = g.F(), C = d.shape.C;
     // whole waves of the walk's persistent CTAs per chunk: a partial last wave in every launch leaves SMs idle (a
     // 64 MiB chunk is 3.1 waves of the cfg3 plan, which then ran at 0.74x of one dense launch)
-    const size_t wave = (size_t)make_plan(d, e->tune, e->forced_variant).tuples_per_cta() * d.sm_count;
+    const size_t wave = (size_t)make_plan(d, walk_tune(e, Walk::Fp32), e->forced_variant).tuples_per_cta() * d.sm_count;
     size_t rows = default_chunk(e, F);
     if (rows > wave) rows -= rows % wave;
     rows = std::min(n, rows);
@@ -2137,10 +2261,11 @@ int dte_get_info(dte_t* e, dte_info* info) {
     info->tuples_out = e->tuples_out;
     info->num_classes = d0.d_top ? d0.shape.C : 0;
     if (d0.d_top) {
-        const Plan pl = make_plan(d0, e->tune, e->forced_variant);
+        const Plan pl = make_plan(d0, walk_tune(e, Walk::Fp32), e->forced_variant);
         info->kernel_variant = (uint32_t)pl.variant();
         info->tuples_per_cta = pl.tuples_per_cta();
     }
+    info->plan_source = e->autotuned || (e->measured && e->forced_variant == KERNEL_AUTO) ? DTE_PLAN_MEASURED : DTE_PLAN_STATIC;
     return DTE_OK;
 }
 
@@ -2154,52 +2279,21 @@ int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     TRY(decode_geom(e, g));
     TRY(check_resident(e, g));
     TRY(drain_all(e));
-    const uint32_t F = d.shape.g.F();
-    n_tuples = std::max<size_t>(n_tuples, (size_t)d.sm_count * 192 * 4);
-    CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    void* d_x = nullptr;
-    float* d_s = nullptr;
-    CUDA_TRY(e, cudaMalloc(&d_x, n_tuples * F * 4));
-    if (cudaMalloc(&d_s, n_tuples * d.shape.C * 4) != cudaSuccess) { cudaFree(d_x); return fail(e, DTE_ERR_NOMEM, "autotune: out of device memory"); }
-    synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n_tuples * F, 0x7091E5ull, 10000u, e->g.missing);
-    struct Cand { int row, stages, phased, warps; };            // warps = 10: the 384-thread (168-register) instantiation
-    const int r42 = tile_row(4, 2, true), r24 = tile_row(2, 4, true), r81 = tile_row(8, 1, true), r41 = tile_row(4, 1, true),
-              r22 = tile_row(2, 2, true);
-    const Cand cands[] = {{r42, 1, 1, 0}, {r42, 1, 0, 0}, {r42, 1, 1, 10}, {r42, 1, 0, 10}, {r24, 1, 1, 0}, {r24, 1, 0, 0}, {r81, 1, 0, 0},
-                          {r81, 2, 0, 0}, {r41, 2, 0, 0}, {r22, 2, 0, 0}, {r22, 1, 0, 0}};
-    const Tune saved = e->tune;
-    Tune best = saved;
-    float best_ms = 1e30f;
+    std::vector<PlanTiming> t;
+    TRY(time_plans(e, d, e->tune, n_tuples, t));
     std::string rep;
-    char name[256], line[400];
-    int rc = DTE_OK;
-    for (const Cand& c : cands) {
-        const TileFamily& f = kTileFamilies[c.row];
-        // the planner stages a pinned family only with >= 2 consumer warps, and a cap is only worth timing when it
-        // removes a tuple group; a plan that stages can always refill phased (Dtop >= 3, at most 4 stages)
-        const int groups = tile_groups(d, f, c.stages, c.warps);
-        if (groups * f.pair < 2 || (c.warps && tile_groups(d, f, c.stages, 0) * f.pair <= c.warps)) continue;
-        Tune t = saved;
-        t.ilp = f.ilp; t.pair = f.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps;
-        float ms = 0;
-        for (int rep_i = 0; rep_i < 2 && !rc; ++rep_i) {                     // the second launch is the measurement
-            const char* why = nullptr;
-            cudaEventRecord(d.ev_t0, d.s_main);
-            cudaError_t st = launch_walk(d, e->g, t, KERNEL_AUTO, d_x, n_tuples, d_s, nullptr, d.s_main, false, &why);
-            cudaEventRecord(d.ev_t1, d.s_main);
-            if (st != cudaSuccess || cudaEventSynchronize(d.ev_t1) != cudaSuccess) { rc = fail(e, DTE_ERR_CUDA, "autotune launch failed: %s", cudaGetErrorString(st)); break; }
-            cudaEventElapsedTime(&ms, d.ev_t0, d.ev_t1);
-        }
-        if (rc) break;
-        kernel_name(d, t, KERNEL_AUTO, name, sizeof name);
-        snprintf(line, sizeof line, "%8.3f ms  %7.2f M tuples/s  %s\n", ms, n_tuples / (ms * 1e3), name);
+    char line[400];
+    const PlanTiming* best = &t[0];
+    for (const PlanTiming& p : t) {
+        snprintf(line, sizeof line, "%8.3f ms per M tuples  %7.2f M tuples/s  %s%s\n", 1e3 / p.tuples_per_ms, p.tuples_per_ms * 1e-3,
+                 p.name.c_str(), &p == &t[0] ? "  (current)" : "");
         rep += line;
-        if (ms < best_ms) { best_ms = ms; best = t; }
+        if (p.tuples_per_ms > best->tuples_per_ms) best = &p;
     }
-    cudaFree(d_x);
-    cudaFree(d_s);
-    if (rc) { e->tune = saved; return rc; }
-    e->tune = best;
+    e->tune = best->tune;
+    e->measured.reset();
+    e->autotuned = true;
+    char name[256];
     kernel_name(d, e->tune, e->forced_variant, name, sizeof name);
     rep += std::string("chosen: ") + name + "\n";
     if (report && report_len) snprintf(report, report_len, "%s", rep.c_str());

@@ -87,8 +87,11 @@ class DteInfo(C.Structure):
         ("tuples_per_cta", C.c_uint32), ("sm_count", C.c_uint32), ("ensemble_bytes", C.c_uint64),
         ("kernel_launches", C.c_uint64), ("last_walk_ms", C.c_double),
         ("num_devices", C.c_uint32), ("partition", C.c_uint32), ("tuples_in", C.c_uint64), ("tuples_out", C.c_uint64),
-        ("num_classes", C.c_uint32),
+        ("num_classes", C.c_uint32), ("plan_source", C.c_uint32),
     ]
+
+
+PLAN_SOURCES = {0: "static", 1: "measured"}    # dte_plan_source
 
 
 DTE_OPT_CYCLE_MHZ, DTE_OPT_COMBINE, DTE_OPT_RESULT_QUEUE_LINES, DTE_OPT_CHUNK_TUPLES = 1, 2, 3, 4
@@ -535,4 +538,6 @@ class Engine:
     def info(self):
         i = DteInfo()
         self._check(self._lib.dte_get_info(self._h, C.byref(i)))
-        return {k: getattr(i, k) for k, _ in DteInfo._fields_}
+        info = {k: getattr(i, k) for k, _ in DteInfo._fields_}
+        info["plan_source"] = PLAN_SOURCES[info["plan_source"]]
+        return info

@@ -124,7 +124,12 @@ int dte_stream_flush(dte_t* engine);
  * written to registers 204/205.  Equivalent to `start` + streaming those lines.
  * first_tree/num_local_trees select the contiguous chunk this device keeps — the chunking
  * PCIeReceiver does by numcls_local_weights/findexes (PCIeReceiver.sv:241-264); pass 0 / all trees
- * for a single device or for the data-sharded (replicated) mode. */
+ * for a single device or for the data-sharded (replicated) mode.
+ * Every dte_load_ensemble* call on a single-device handle configured for at least 8 M tuples (reg 207, the n_tuples of
+ * dte_csr_from_profile), with no DTE_TUNE knob and no forced kernel variant, also times the fp32 walk's staged launch
+ * plans on synthetic tuples (dte_autotune's candidates; about half a second of GPU time at 1024 trees, D = 12) and runs
+ * the fastest when it beats the built-in plan by 2 %; one line on stderr reports the choice and its cost.  Every plan is
+ * bit-exact; only the speed differs.  dte_info.plan_source says which plan runs. */
 int dte_load_ensemble(dte_t* engine, const void* weight_cls, size_t n_weight_cls,
                       const void* findex_cls, size_t n_findex_cls,
                       uint32_t first_tree, uint32_t num_local_trees);
@@ -374,7 +379,12 @@ typedef struct {
     uint64_t tuples_in;        /* whole tuples received since create */
     uint64_t tuples_out;       /* results produced since create */
     uint32_t num_classes;      /* classes of the resident ensemble (1 = single score per tuple; 0 = none loaded) */
+    uint32_t plan_source;      /* how the fp32 walk's launch plan was chosen (dte_plan_source) */
 } dte_info;
+typedef enum {
+    DTE_PLAN_STATIC = 0,       /* the built-in planner, with any DTE_TUNE knobs */
+    DTE_PLAN_MEASURED = 1      /* timed on the device: at load (dte_load_ensemble) or by dte_autotune */
+} dte_plan_source;
 int dte_get_info(dte_t* engine, dte_info* info);
 
 /* Name and launch shape of the walk kernel the next dte_infer_* call will launch, e.g.
@@ -383,9 +393,10 @@ int dte_get_info(dte_t* engine, dte_info* info);
 int dte_kernel_name(dte_t* engine, char* buf, size_t len);
 
 /* Measure instead of guessing: times the planner's alternative launch plans (trees per warp x warps per tuple group x
- * ring stages x phased refill) of the resident ensemble on n_tuples synthetic tuples and pins the fastest for this
- * handle (every plan is bit-exact; only the speed differs).  The built-in choice is the plan measured best on the
- * BASELINE geometries; call this for other (trees, levels, features).  `report` (may be NULL) receives one line per plan. */
+ * ring stages x phased refill x consumer-warp cap) of the resident ensemble on synthetic tuples and pins the fastest for
+ * this handle and every walk kind (every plan is bit-exact; only the speed differs).  Each plan walks whole waves of its
+ * tiles within max(n_tuples, 2 waves), a warm-up launch and then the median of 3.  A load with a large workload hint
+ * already does this for the fp32 walk (dte_load_ensemble).  `report` (may be NULL) receives one line per plan. */
 int dte_autotune(dte_t* engine, size_t n_tuples, char* report, size_t report_len);
 
 typedef enum {

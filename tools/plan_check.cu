@@ -6,6 +6,8 @@
 // tests/test_plan_table.py compares the output with tests/golden/plan_table.txt.xz.  Test infrastructure.
 //   plan_check bin   the same grid for the binned walk (u8 tile, 4-byte tree tops): tests/golden/plan_table_binned.txt.xz
 //   plan_check leaf  the same grid for the leaf walk (dt_walk_*_leaf): tests/golden/plan_table_leaf.txt.xz
+//   plan_check trigger  whether a load times the launch plans (measure_plan_at_load), one line per case:
+//                       <DTE_TUNE> <forced variant> <multi-device> <workload hint> <1 = times them>
 #include "../distributed-decisiontrees_b200/csrc/dte_device.cuh"
 #include <cstdio>
 #include <cstdlib>
@@ -29,6 +31,19 @@ static const char* const kTunes[] = {
 
 int main(int argc, char** argv) {
     const char* kind = argc > 1 ? argv[1] : "";
+    if (!strcmp(kind, "trigger")) {
+        for (const char* s : {"", "chunk=65536", "ilp=4", "pair=2", "stages=1", "warps=8", "phased=1", "phased=0", "fill=1"}) {
+            setenv("DTE_TUNE", s, 1);
+            Tune tune;
+            parse_tune(tune);
+            for (int want = KERNEL_AUTO; want <= KERNEL_TILE_STAGED; ++want)
+                for (bool multi : {false, true})
+                    for (uint64_t hint : {0ull, 4000000ull, 7999996ull, 8000000ull, 50000000ull})
+                        printf("DTE_TUNE=%s %d %d %llu %d\n", s, want, (int)multi, (unsigned long long)hint,
+                               (int)measure_plan_at_load(tune, want, multi, hint));
+        }
+        return 0;
+    }
     const Walk walk = !strcmp(kind, "bin") ? Walk::Binned : !strcmp(kind, "leaf") ? Walk::Leaf : Walk::Fp32;
     const uint32_t Fs[] = {4, 8, 32, 64, 96, 128, 192, 256, 384, 512, 516, 768, 1024, 1536, 1796, 1800, 2048};
     for (const char* s : kTunes) {
