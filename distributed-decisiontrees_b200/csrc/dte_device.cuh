@@ -25,8 +25,8 @@ constexpr int kNumSlots = 3;          // landing slots per device: H2D of i+1, w
 enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED = 3 };
 
 // What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), the leaf cell every
-// tree reaches (DESIGN.md §10), or the TreeSHAP feature contributions (DESIGN.md §12)
-enum class Walk { Fp32, Binned, Leaf, Contrib };
+// tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12) or interaction values (DESIGN.md §13)
+enum class Walk { Fp32, Binned, Leaf, Contrib, Inter };
 
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
@@ -575,14 +575,15 @@ struct Dev {
     uint64_t tuples_landed = 0;       // whole tuples landed on this device since `start`
 };
 
-// Leaf and contribution walks write their rows into Slot::d_rows; score walks into d_sc / d_part, which the combines,
-// the labels and the line stream's ring read.
-inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib; }
-// Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes, or
-// C (F + 1) contribution words
+// Leaf, contribution and interaction walks write their rows into Slot::d_rows; score walks into d_sc / d_part, which the
+// combines, the labels and the line stream's ring read.
+inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib || w == Walk::Inter; }
+// Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes,
+// C (F + 1) contribution words or C (F + 1)^2 interaction words
 inline size_t row_bytes(const Dev& d, Walk w) {
     if (w == Walk::Leaf) return 2 * (size_t)d.shape.T;
     if (w == Walk::Contrib) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
+    if (w == Walk::Inter) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1) * (d.shape.g.F() + 1);
     return 4 * (size_t)d.slot_C;
 }
 
@@ -862,11 +863,28 @@ inline ShapPlan shap_plan(const Dev& d, int want) {
     return p;
 }
 using ShapKernel = void (*)(ShapParams);
+using InterKernel = void (*)(InterParams);
 inline ShapKernel shap_kernel(const ShapPlan& p) {
     if (p.tile) return p.bound == 3 ? dt_shap_tile<3> : p.bound == 7 ? dt_shap_tile<7> : dt_shap_tile<15>;
     return p.bound == 3 ? dt_shap_generic<3> : p.bound == 7 ? dt_shap_generic<7> : dt_shap_generic<15>;
 }
 constexpr size_t kShapScratchBytes = 256ull << 20;   // dt_shap_generic accumulators: rows per launch = this / (8 (F + 1))
+
+// The device's fp64 scratch of dt_shap_generic and dt_shap_inter, at least `words` long, made ready for a walk on st: it
+// waits for the previous walk using it (on any stream).  Grown after a device synchronise; every placement frees it.
+inline cudaError_t shap_scratch(Dev& d, size_t words, cudaStream_t st) {
+    cudaError_t rc;
+    if (!d.ev_shap && (rc = cudaEventCreateWithFlags(&d.ev_shap, cudaEventDisableTiming)) != cudaSuccess) return rc;
+    if (d.shap_scratch_words < words) {               // grow: no walk on any stream may still use the old scratch
+        if ((rc = cudaDeviceSynchronize()) != cudaSuccess) return rc;
+        if (d.d_shap_scratch) cudaFree(d.d_shap_scratch);
+        d.d_shap_scratch = nullptr;
+        d.shap_scratch_words = 0;
+        if ((rc = cudaMalloc(&d.d_shap_scratch, words * 8)) != cudaSuccess) return rc;
+        d.shap_scratch_words = words;
+    }
+    return cudaStreamWaitEvent(st, d.ev_shap, 0);
+}
 
 // Launch the contribution walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident
 // contribution layout: d_out [n][C][F + 1].  The single-class run adds the first min(T, 8 S K) trees of `run`, a
@@ -902,17 +920,8 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     }
     const size_t cap = std::max<size_t>(32, (kShapScratchBytes / ((size_t)(F + 1) * 8)) & ~(size_t)31);
     const size_t rows = std::min(cap, (n + 31) & ~(size_t)31);
-    if (!d.ev_shap && (rc = cudaEventCreateWithFlags(&d.ev_shap, cudaEventDisableTiming)) != cudaSuccess) return rc;
-    const size_t words = rows * (F + 1);             // what the kernel indexes: phi[f * rows + row], f <= F, row < rows
-    if (d.shap_scratch_words < words) {               // grow: no walk on any stream may still use the old scratch
-        if ((rc = cudaDeviceSynchronize()) != cudaSuccess) return rc;
-        if (d.d_shap_scratch) cudaFree(d.d_shap_scratch);
-        d.d_shap_scratch = nullptr;
-        d.shap_scratch_words = 0;
-        if ((rc = cudaMalloc(&d.d_shap_scratch, words * 8)) != cudaSuccess) return rc;
-        d.shap_scratch_words = words;
-    }
-    if ((rc = cudaStreamWaitEvent(st, d.ev_shap, 0)) != cudaSuccess) return rc;
+    // what the kernel indexes: phi[f * rows + row], f <= F, row < rows
+    if ((rc = shap_scratch(d, rows * (F + 1), st)) != cudaSuccess) return rc;
     p.scratch = d.d_shap_scratch;
     p.scratch_rows = rows;
     for (size_t off = 0; off < n; off += rows) {
@@ -931,6 +940,87 @@ inline void contrib_kernel_name(const Dev& d, int want, char* buf, size_t len) {
     const ShapPlan pl = shap_plan(d, want);
     if (pl.tile) snprintf(buf, len, "dt_shap_tile<%d> warps=%d smem=%zu", pl.bound, pl.groups, pl.smem);
     else snprintf(buf, len, "dt_shap_generic<%d>", pl.bound);
+    if (d.shape.C >= 2) {
+        const size_t used = strlen(buf);
+        if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
+    }
+}
+
+// ---- interaction values (DESIGN.md §13) ----
+// dt_shap_inter keeps fp64 accumulators acc(r, k) for B matrix rows of F words per tuple in the device's scratch, so one
+// pass over the paths computes rows [r0, r0 + B) and a launch chunk of `rows` tuples runs ceil((F + 1) / B) passes.  The
+// planner's B is the largest that lets min(n, kInterRowsPerSM per SM) tuples share kInterScratchBytes (a call of 135,168
+// tuples or more at F = 128 on 132 SMs: B = 7, 19 passes; a smaller call takes fewer, larger passes, since every pass
+// walks the paths again); DTE_OPT_INTERACTION_BLOCK forces another.  Every word is the same for any B and any chunking:
+// each accumulator belongs to one pass and one tuple and is added to in path order.
+constexpr size_t kInterScratchBytes = 1ull << 30;
+constexpr uint64_t kInterMaxRowWords = 1ull << 24;  // C (F + 1)^2 words of one tuple's row: 64 MiB
+constexpr size_t kInterRowsPerSM = 1024;            // two waves of 128-thread CTAs at four CTAs per SM
+struct InterPlan {
+    int bound = 3;                                   // the path-length bound M of dt_shap_inter<M>
+    uint32_t block = 1;                              // B: matrix rows per pass
+    size_t rows = 32;                                // tuples per launch chunk (a multiple of 32)
+};
+inline InterPlan inter_plan(const Dev& d, uint32_t forced_block, size_t n) {
+    InterPlan p;
+    const uint32_t F = d.shape.g.F();
+    p.bound = d.shap.M <= 3 ? 3 : d.shap.M <= 7 ? 7 : 15;
+    const size_t row_bytes = (size_t)8 * F;          // one matrix row of one tuple
+    const size_t tuples = std::min((size_t)std::max(1, d.sm_count) * kInterRowsPerSM, (std::min<size_t>(n, 1ull << 40) + 31) & ~(size_t)31);
+    const size_t B = forced_block ? forced_block : kInterScratchBytes / (row_bytes * std::max<size_t>(tuples, 32));
+    p.block = (uint32_t)std::min<size_t>(std::max<size_t>(B, 1), F + 1);
+    p.rows = std::max<size_t>(32, (kInterScratchBytes / (row_bytes * std::min(p.block, F))) & ~(size_t)31);
+    return p;
+}
+inline InterKernel inter_kernel(int bound) {
+    return bound == 3 ? dt_shap_inter<3> : bound == 7 ? dt_shap_inter<7> : dt_shap_inter<15>;
+}
+
+// Launch the interaction walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident contribution
+// layout: d_out [n][C][F + 1][F + 1], the trees as launch_contrib's.  Chunks of the plan's rows, each in passes of B
+// matrix rows through the device's fp64 scratch.  Returns a cudaError_t.
+inline cudaError_t launch_inter(Dev& d, const Geom& run, uint32_t forced_block, const void* d_tuples, size_t n, float* d_out,
+                                cudaStream_t st, const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const uint32_t F = d.shape.g.F(), C = d.shape.C;
+    InterParams ip = {};
+    ShapParams& p = ip.s;
+    p.nodes = d.d_shap_nodes;
+    p.paths = d.d_shap_paths;
+    p.tree_path = d.d_shap_tree_path;
+    p.cls_tree = d.d_shap_cls_tree;
+    p.F = F; p.C = C; p.missing = run.missing;
+    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff; p.izoff = d.shap.izoff;
+    p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    const InterPlan pl = inter_plan(d, forced_block, n);
+    const InterKernel k = inter_kernel(pl.bound);
+    const size_t rows = std::min(pl.rows, (n + 31) & ~(size_t)31);
+    cudaError_t rc;
+    if ((rc = shap_scratch(d, rows * std::min(pl.block, F) * F, st)) != cudaSuccess) return rc;
+    p.scratch = d.d_shap_scratch;
+    p.scratch_rows = rows;
+    const size_t row_words = (size_t)C * (F + 1) * (F + 1);
+    const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
+    for (size_t off = 0; off < n; off += rows) {
+        p.n = std::min(rows, n - off);
+        p.tuples = tuples + off * F;
+        p.out = d_out + off * row_words;
+        for (uint32_t r0 = 0; r0 <= F; r0 += pl.block) {
+            ip.r0 = r0;
+            ip.r1 = std::min(F + 1, r0 + pl.block);
+            k<<<(unsigned)((p.n + 127) / 128), 128, 0, st>>>(ip);
+            if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
+            d.kernel_launches++;
+        }
+    }
+    return cudaEventRecord(d.ev_shap, st);
+}
+
+// "dt_shap_inter<bound> rows=B", as launch_inter would launch a call of a full machine's tuples (or more)
+inline void inter_kernel_name(const Dev& d, uint32_t forced_block, char* buf, size_t len) {
+    const InterPlan pl = inter_plan(d, forced_block, SIZE_MAX);
+    snprintf(buf, len, "dt_shap_inter<%d> rows=%u", pl.bound, pl.block);
     if (d.shape.C >= 2) {
         const size_t used = strlen(buf);
         if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);

@@ -88,6 +88,7 @@ struct dte_engine {
     int combine_nccl = 0;
     size_t opt_queue_lines = 0, opt_chunk_tuples = 0;
     bool opt_leaf = false;            // DTE_OPT_LEAF_LAYOUT: placements also build the leaf-id layout
+    uint32_t opt_inter_block = 0;     // DTE_OPT_INTERACTION_BLOCK: matrix rows per interaction pass (0 = the planner's)
 
     // ---- stream state (PCIeReceiver.sv FSM) ----
     enum { ST_IDLE = 0, ST_TREES = 1, ST_WAIT = 2, ST_DATA = 3 } state = ST_IDLE;
@@ -276,7 +277,8 @@ const char* missing_layout(const Dev& d, Walk w) {
     switch (w) {
         case Walk::Binned: return d.d_top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
         case Walk::Leaf: return d.d_bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
-        case Walk::Contrib: return d.d_shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
+        case Walk::Contrib:
+        case Walk::Inter: return d.d_shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
         default: return d.d_top ? nullptr : "no ensemble loaded";
     }
 }
@@ -298,6 +300,10 @@ int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
                         g.F(), g.D, d.shape.g.F(), d.shape.g.D);
+        const uint64_t F1 = d.shape.g.F() + 1;
+        if (w == Walk::Inter && d.shape.C * F1 * F1 > kInterMaxRowWords)
+            return fail(e, DTE_ERR_UNSUPPORTED, "an interaction row of %u classes x %llu x %llu words exceeds 64 MiB (2^24 words)",
+                        d.shape.C, (unsigned long long)F1, (unsigned long long)F1);
         // a multi-class walk covers every tree: the slots must hold the largest class (no silent truncation per class)
         if (w != Walk::Leaf && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
             return fail(e, DTE_ERR_CONFIG, "reg 205: S=%u x K=%u x 8 slots hold fewer trees than the largest of the %u classes (%u trees): "
@@ -612,10 +618,12 @@ int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, vo
     const cudaError_t rc =
         w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
         : w == Walk::Contrib ? launch_contrib(d, e->g, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
+        : w == Walk::Inter   ? launch_inter(d, e->g, e->opt_inter_block, tuples, n, static_cast<float*>(out), st, &why)
                              : launch_walk(d, e->g, walk_tune(e, w), e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
     if (rc != cudaSuccess)
         return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s",
-                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : "walk kernel", why ? why : cudaGetErrorString(rc));
+                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : w == Walk::Inter ? "interaction walk" : "walk kernel",
+                    why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
 
@@ -1169,9 +1177,10 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
     if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
-    // the contributions of a tree chunk are fp64 partials: combining them in ring order is not offered
-    if (w == Walk::Contrib && e->part == Part::Chunked)
-        return fail(e, DTE_ERR_CONFIG, "%s: an ensemble-sharded handle cannot return contributions; use a single-device or data-sharded handle", what);
+    // the contributions (interactions) of a tree chunk are fp64 partials: combining them in ring order is not offered
+    if ((w == Walk::Contrib || w == Walk::Inter) && e->part == Part::Chunked)
+        return fail(e, DTE_ERR_CONFIG, "%s: an ensemble-sharded handle cannot return %s; use a single-device or data-sharded handle", what,
+                    w == Walk::Inter ? "interaction values" : "contributions");
     TRY(check_resident(e, g, w));
     if (n == 0) return DTE_OK;
     e->g = g;
@@ -1181,8 +1190,9 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
     size_t cap = default_chunk(e, F);
     if (row_walk(w)) {
         // The rows of a slot (2T bytes per tuple for leaf cells, 4 C (F + 1) for contributions: 2 MiB at C = 256,
-        // F = 2048) may take at most twice the tuple budget, so a many-tree or many-feature ensemble lands fewer tuples
-        // per slot instead of allocating GiBs of rows.
+        // F = 2048, 4 C (F + 1)^2 for interactions: at most 64 MiB) may take at most twice the tuple budget, so a
+        // many-tree or many-feature ensemble lands fewer tuples per slot instead of allocating GiBs of rows; every slot
+        // still lands at least 4 tuples.
         size_t row = 1;
         for (const Dev& d : e->devs) row = std::max(row, row_bytes(d, w));
         const size_t budget = 2 * (64ull << 20) * std::min<size_t>(4, e->devs.size());
@@ -1490,6 +1500,7 @@ int dte_set_option(dte_t* e, int option, uint64_t value) {
             if (value > 1) return fail(e, DTE_ERR_ARG, "DTE_OPT_LEAF_LAYOUT: 0 (scores only) or 1 (also the leaf-id layout)");
             e->opt_leaf = value != 0;
             break;
+        case DTE_OPT_INTERACTION_BLOCK: e->opt_inter_block = (uint32_t)std::min<uint64_t>(value, 0xFFFFFFFFu); break;
         default: return fail(e, DTE_ERR_ARG, "unknown option %d", option);
     }
     return DTE_OK;
@@ -1865,7 +1876,8 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
     const int align = w == Walk::Leaf ? 16 : 4;
     if (reinterpret_cast<uintptr_t>(out) & (align - 1))
         return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what,
-                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib ? "d_contribs" : accumulate ? "d_scores_accum" : "d_scores", align);
+                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib ? "d_contribs" : w == Walk::Inter ? "d_inter"
+                    : accumulate ? "d_scores_accum" : "d_scores", align);
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));
@@ -1889,6 +1901,7 @@ static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
     if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
     if (w == Walk::Contrib) contrib_kernel_name(e->devs[0], e->forced_variant, buf, len);
+    else if (w == Walk::Inter) inter_kernel_name(e->devs[0], e->opt_inter_block, buf, len);
     else kernel_name(e->devs[0], walk_tune(e, w), e->forced_variant, buf, len, w);
     return DTE_OK;
 }
@@ -2014,6 +2027,19 @@ int dte_infer_host_contribs(dte_t* e, const void* h_tuples, size_t n, float* h_c
 }
 
 int dte_kernel_name_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Contrib, buf, len); }
+
+// ---- interaction values (DESIGN.md §13) ----
+int dte_infer_device_interactions(dte_t* e, const void* d_tuples, size_t n, float* d_inter, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_inter))) return DTE_ERR_ARG;
+    return infer_device(e, Walk::Inter, "dte_infer_device_interactions", d_tuples, n, d_inter, nullptr, cuda_stream);
+}
+
+int dte_infer_host_interactions(dte_t* e, const void* h_tuples, size_t n, float* h_inter) {
+    if (!e || (n && (!h_tuples || !h_inter))) return DTE_ERR_ARG;
+    return infer_host(e, Walk::Inter, "infer_host_interactions", static_cast<const unsigned char*>(h_tuples), n, h_inter, nullptr);
+}
+
+int dte_kernel_name_interactions(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Inter, buf, len); }
 
 // ---- sparse tuples (DESIGN.md §11) ----
 // The kernel reads indptr as 8-byte and the entries as 4-byte words: a misaligned pointer would fault it.

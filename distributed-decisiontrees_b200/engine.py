@@ -71,6 +71,9 @@ ABI = [
     ("dte_infer_device_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("dte_kernel_name_contribs", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_infer_device_interactions", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_interactions", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_kernel_name_interactions", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
     ("dte_sparse_to_dense_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
                                              C.c_void_p, C.c_void_p]),
     ("dte_infer_device_sparse", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p,
@@ -96,6 +99,7 @@ PLAN_SOURCES = {0: "static", 1: "measured"}    # dte_plan_source
 
 DTE_OPT_CYCLE_MHZ, DTE_OPT_COMBINE, DTE_OPT_RESULT_QUEUE_LINES, DTE_OPT_CHUNK_TUPLES = 1, 2, 3, 4
 DTE_OPT_LEAF_LAYOUT = 5
+DTE_OPT_INTERACTION_BLOCK = 6     # matrix rows per interaction pass (0 = the planner's)
 DTE_ERR_BACKPRESSURE = -7
 DTE_SPARSE_ABSENT_MISSING = 0xFFFFFFFFFFFFFFFF   # sparse calls: an absent feature is the run's missing pattern (reg 205)
 CUDA_STREAM_LEGACY = 0x1        # cudaStreamLegacy: the handle value that NAMES the legacy default stream
@@ -439,6 +443,26 @@ class Engine:
 
     def kernel_name_contribs(self):
         return self._name(self._lib.dte_kernel_name_contribs)
+
+    # -- interaction values (DESIGN.md §13) ------------------------------------------------------------
+    def infer_device_interactions(self, d_tuples, n, d_inter, stream=None):
+        """[n, C, F + 1, F + 1] fp32 SHAP interaction values (bias at [F, F]) of fp32 tuples [n, F], both on the device
+        (d_tuples 16-byte, d_inter 4-byte aligned)."""
+        self._check(self._lib.dte_infer_device_interactions(self._h, _ptr(d_tuples), int(n), _ptr(d_inter), _stream(stream)))
+
+    def infer_host_interactions(self, tuples, out=None):
+        """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> interaction values [n, F + 1, F + 1] for
+        a single-class ensemble, [n, C, F + 1, F + 1] for a C-class one: row f sums to feature f's contribution, [F, F] is
+        the bias."""
+        t, n = _host_rows(tuples)
+        F, nc = int(self.info()["num_features"]), self.num_classes()
+        if out is None:
+            out = np.empty((n, F + 1, F + 1) if nc == 1 else (n, nc, F + 1, F + 1), dtype=np.float32)
+        self._check(self._lib.dte_infer_host_interactions(self._h, _ptr(t), n, _ptr(out)))
+        return out
+
+    def kernel_name_interactions(self):
+        return self._name(self._lib.dte_kernel_name_interactions)
 
     # -- sparse tuples (DESIGN.md §11) ------------------------------------------------------------------
     # absent=None: an absent feature is the run's missing pattern (XGBoost); a 32-bit word, e.g. 0, is used as it is.

@@ -271,6 +271,32 @@ int dte_infer_host_contribs(dte_t* engine, const void* h_tuples, size_t n, float
 /* "dt_shap_tile<bound> warps=G smem=..." or "dt_shap_generic<bound>"; DTE_ERR_STATE without a contribution layout. */
 int dte_kernel_name_contribs(dte_t* engine, char* buf, size_t len);
 
+/* ---- interaction values (DESIGN.md §13) ------------------------------------------------------ */
+/* SHAP interaction values (XGBoost pred_interactions, shap's shap_interaction_values) of the path-dependent game of the
+ * contribution calls, on the same trees, decision rule and classes.  For each tuple and class an (F+1) x (F+1) matrix:
+ * inter[i][c][a][b] for a != b, both < F, is the Shapley interaction index of features a and b summed over the class-c
+ * trees, half the pair's total interaction, so the matrix is symmetric up to rounding; inter[i][c][a][a] = contribs[a]
+ * minus the other words of row a (every row a < F sums to the contribution of a); row F and column F are 0 except
+ * inter[i][c][F][F], the bias, bit for bit the contribution calls' bias word.  Computed in fp64 in the order DESIGN.md
+ * §13 fixes and rounded once to fp32 per word, so every word is reproducible and independent of batching, devices and
+ * DTE_OPT_INTERACTION_BLOCK.  Before that rounding an off-diagonal value is within 2^-40 sum_p |v_p| prod_e max(1, z_e)
+ * of the exact one, as for contributions.  Layout [n][C][F+1][F+1] fp32.  Needs the contribution layout
+ * (dte_load_ensemble_contribs), else DTE_ERR_STATE.  A tuple row over 64 MiB (C (F+1)^2 > 2^24 words) returns
+ * DTE_ERR_UNSUPPORTED before anything runs.  Binned and sparse tuples are not taken: densify first
+ * (dte_sparse_to_dense_device). */
+/* [n][C][F+1][F+1] interaction values of n fp32 tuples in device memory.  Single-device handles (a multi-device handle
+ * returns DTE_ERR_UNSUPPORTED); stream as dte_infer_device.  d_tuples must be 16-byte aligned and d_inter 4-byte aligned,
+ * else DTE_ERR_ARG before any launch.  The walk runs in chunks of tuples, each in passes of B matrix rows through a fp64
+ * scratch of at most about 1 GiB the handle keeps (every placement frees it). */
+int dte_infer_device_interactions(dte_t* engine, const void* d_tuples, size_t n, float* d_inter, void* cuda_stream);
+/* The same from host memory through the landing pipeline: single-device and data-sharded handles (rows in global tuple
+ * order).  An ensemble-sharded handle returns DTE_ERR_CONFIG.  The row buffers of the landing slots are allocated by the
+ * first call; a slot lands fewer tuples (at least 4) when its rows would exceed the tuple landing budget. */
+int dte_infer_host_interactions(dte_t* engine, const void* h_tuples, size_t n, float* h_inter);
+/* "dt_shap_inter<bound> rows=B" (B = matrix rows per pass), plus " classes=C" for C >= 2; DTE_ERR_STATE without a
+ * contribution layout. */
+int dte_kernel_name_interactions(dte_t* engine, char* buf, size_t len);
+
 /* ---- sparse tuples (DESIGN.md §11) ------------------------------------------------------------- */
 /* n tuples as CSR rows: indptr int64 [n + 1], indices uint32 [nnz] (feature numbers), values [nnz] 32-bit words (fp32 bit
  * patterns).  Row i's entries are k in [indptr[i], indptr[i+1]), indexing indices and values absolutely, so indptr[0]
@@ -345,9 +371,11 @@ typedef enum {
                                      1 = one ncclReduce(SUM) to the host device (order free: 1e-5 relative) */
     DTE_OPT_RESULT_QUEUE_LINES = 3, /* capacity of the result queue in 128-bit lines (0 = derive from reg 207) */
     DTE_OPT_CHUNK_TUPLES = 4,     /* tuples per landing buffer of the H2D | walk | D2H pipeline (0 = 64 MiB worth) */
-    DTE_OPT_LEAF_LAYOUT = 5       /* 1: every placement of an ensemble (dte_load_ensemble*, a tree line stream) also builds
+    DTE_OPT_LEAF_LAYOUT = 5,      /* 1: every placement of an ensemble (dte_load_ensemble*, a tree line stream) also builds
                                      and uploads the leaf-id layout the dte_*_leaves calls walk, and ensemble_bytes counts
                                      it; 0 (default): a placement builds none and drops a resident one */
+    DTE_OPT_INTERACTION_BLOCK = 6 /* matrix rows B per pass of the interaction walk: 0 (default) = the planner's, else
+                                     min(value, F + 1); the words do not depend on it, only the speed and the scratch */
 } dte_option;
 int dte_set_option(dte_t* engine, int option, uint64_t value);
 

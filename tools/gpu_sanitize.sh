@@ -66,6 +66,13 @@ for T in tests/test_gpu_contribs.py::test_headline_geometry tests/test_gpu_contr
   ctag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_contribs_${ctag}.log"
 done
+# the interaction kernel: several row blocks through the fp64 scratch, three launch chunks, the ragged tail of a warp and
+# the <15> kernel on D = 15 paths with the bottom-up unwinding
+for T in tests/test_gpu_interactions.py::test_row_blocks_give_the_same_bytes tests/test_gpu_interactions.py::test_several_launch_chunks \
+         "tests/test_gpu_interactions.py::test_tuple_counts[33]" "tests/test_gpu_interactions.py::test_deep_leafwise[free-15-15-15]"; do
+  itag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_inter_${itag}.log"
+done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1
 echo "racecheck [canonical textbook pipeline] rc=$? $(grep -E 'canonical|RACECHECK SUMMARY' $OUT/sanitizer_racecheck_canonical.log | tr '\n' ' ' | cut -c1-300)"
