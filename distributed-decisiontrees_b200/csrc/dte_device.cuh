@@ -28,13 +28,14 @@ enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED 
 // tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12) or interaction values (DESIGN.md §13)
 enum class Walk { Fp32, Binned, Leaf, Contrib, Inter };
 
-// experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536"
+// experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536,tops=6"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
 //  phased: 0 off / k>=1 on with part A ending k levels earlier, fill=1: one bulk copy per tree,
-//  chunk: tuples per landing slot)
+//  chunk: tuples per landing slot, tops=6: a staged single-class fp32 walk streams the 6-byte split tree tops)
 struct Tune {
     int ilp = 0, stages = 0, warps = 0, pair = 0, fill = 0, phased = -1;
     size_t chunk = 0;
+    int tops = 0;
 };
 
 inline void parse_tune(Tune& t) {
@@ -56,6 +57,7 @@ inline void parse_tune(Tune& t) {
             else if (k == "fill") t.fill = (int)v;
             else if (k == "phased") t.phased = (int)v;
             else if (k == "chunk") t.chunk = (size_t)v;
+            else if (k == "tops") t.tops = (int)v;
         }
         if (comma == std::string::npos) break;
         pos = comma + 1;
@@ -73,6 +75,7 @@ struct Plan {               // how the next walk will be launched
     int row = -1;           // kTileFamilies row of a tile plan; -1: dt_walk_generic
     int nstages = 0, nwarps = 0;                       // nwarps = consumer warps = groups * pair
     bool wide = false;
+    bool split = false;                                // staged with the 6-byte split tree tops (dt_walk_tile_split)
     Walk walk = Walk::Fp32;
     size_t smem = 0;
     const TileFamily& fam() const { return kTileFamilies[row]; }
@@ -95,6 +98,8 @@ struct EnsembleShape {
 
 // The ensemble in the device layout, still in host memory (built once, uploaded to one or many devices).
 //   top[t][2^(D-2)]    8-byte heap records {thr bits, fidx | (8 + 8*missing_right) << 16} for levels 0..D-3
+//   top_split[t]       the same records split in two runs, 6 bytes each: u32 thr[2^(D-2)], then u16 meta[2^(D-2)] =
+//                      fidx | missing_right << 15; what dt_walk_tile_split streams through its ring (DESIGN.md §3)
 //   bottom[t][2^(D-2)] one record per level-(D-2) node: that node, its two children and their four leaves;
 //                      32 bytes (= one L2 sector) when every feature index < 512, 64 bytes otherwise
 // Source layout (SURVEY R1): per tree W = heap array of 2^(D+1)-1 fp32 words padded to w_cls lines, FI = 2^D-1
@@ -109,6 +114,7 @@ struct EnsembleShape {
 struct PackedEnsemble {
     EnsembleShape shape;
     std::vector<uint2> top;
+    std::vector<uint16_t> top_split;     // 3 * top_stride u16 words per tree slot
     std::vector<uint4> bottom;
     std::vector<uint32_t> top_b;
     std::vector<uint4> bottom_b;
@@ -478,6 +484,16 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
             }
         }
     }
+    // the split tops: every record of `top`, padding and zero-trees included, in the same slot order
+    out.top_split.assign((size_t)Tpad * top_stride * 3, 0);
+    for (size_t t = 0; t < Tpad; ++t) {
+        const uint2* tp = out.top.data() + t * top_stride;
+        uint16_t* ts = out.top_split.data() + t * top_stride * 3;
+        for (uint32_t n = 0; n < top_stride; ++n) {
+            memcpy(ts + 2 * n, &tp[n].x, 4);
+            ts[2 * top_stride + n] = (uint16_t)((tp[n].y & 0x7FFu) | ((tp[n].y >> 16) == 16u ? 0x8000u : 0u));
+        }
+    }
     return 0;
 }
 
@@ -515,6 +531,7 @@ struct Dev {
     // ---- resident ensemble ----
     EnsembleShape shape;              // of the resident ensemble; a run's K, S and missing are passed to launch_walk
     uint2* d_top = nullptr;
+    uint16_t* d_top_split = nullptr;  // PackedEnsemble::top_split
     uint4* d_bottom = nullptr;
     uint64_t ensemble_bytes = 0;
     // binned layout (dte_load_ensemble_binned only): 4-byte tops, binned bottom records, the edge table (CSR)
@@ -588,9 +605,10 @@ inline size_t row_bytes(const Dev& d, Walk w) {
 }
 
 // ---- launch planning ---------------------------------------------------------------------------
-// the binned walk stages 4-byte tree tops and holds one byte per feature in the tile
-inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride, Walk w = Walk::Fp32) {
-    const size_t top = w == Walk::Binned ? 4 : 8, feature = w == Walk::Binned ? 1 : 4;
+// the binned walk stages 4-byte tree tops and holds one byte per feature in the tile; split tops are 6 bytes
+inline size_t tile_smem(uint32_t F, int groups, int trees_per_stage, int nstages, uint32_t top_stride, Walk w = Walk::Fp32,
+                        bool split = false) {
+    const size_t top = split ? 6 : w == Walk::Binned ? 4 : 8, feature = w == Walk::Binned ? 1 : 4;
     return (size_t)kHdrBytes + (size_t)nstages * trees_per_stage * top_stride * top + (size_t)F * 32 * groups * feature;
 }
 
@@ -607,27 +625,36 @@ inline int tile_row(int ilp, int pair, bool staged) {
     return first >= 0 ? first : tile_row(ilp, 1, staged);
 }
 
+// Whether family f has split-tops walks (dt_walk_tile_split): the staged families below ILP = 8, whose walks sit at the
+// 168-register cap and spill with the second node address.
+constexpr bool splits(const TileFamily& f) { return f.staged && f.ilp < 8; }
+
 // Tuple groups (32 tuples, F*128 B of shared memory each, F*32 B binned) of family f that fit next to a ring of nstages
-// stages, and at most `warps` consumer warps when warps > 0.
-inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps, Walk w = Walk::Fp32) {
+// stages (of split tops when `split`), and at most `warps` consumer warps when warps > 0.
+inline int tile_groups(const Dev& d, const TileFamily& f, int nstages, int warps, Walk w = Walk::Fp32, bool split = false) {
     if (f.staged && d.shape.Dtop < 3) return 0;        // below that there is nothing worth staging
     const uint32_t F = d.shape.g.F();
     const size_t budget = (size_t)d.smem_optin;
-    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride, w);
+    const size_t fixed = tile_smem(F, 0, f.ilp * f.pair, nstages, d.shape.top_stride, w, split && splits(f));
     if (fixed >= budget) return 0;
     int g = (int)std::min<size_t>((size_t)(tile_warp_cap(f.nt) / f.pair), (budget - fixed) / ((size_t)F * (w == Walk::Binned ? 32 : 128)));
     if (warps) g = std::min(g, std::max(1, warps / f.pair));
     return g;
 }
 
+// Whether a staged plan of walk kind w streams split tree tops: on the knob tops=6, for single-class fp32 walks.
+inline bool split_tops(const Dev& d, const Tune& tune, Walk w) { return tune.tops == 6 && w == Walk::Fp32 && d.shape.C == 1; }
+
 // The plan of a walk of kind w on the resident ensemble.  Every kind has the same candidates and rules; a binned plan
 // sizes the binned tile and tops, a leaf plan is the fp32 plan.
 inline Plan make_plan(const Dev& d, const Tune& tune, int want, Walk w = Walk::Fp32) {
+    const bool split = split_tops(d, tune, w);
     auto tile_plan = [&](int row, int nstages, int groups) {
         const TileFamily& f = kTileFamilies[row];
         Plan p;
         p.row = row; p.nstages = nstages; p.nwarps = groups * f.pair; p.wide = d.shape.wide; p.walk = w;
-        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride, w);
+        p.split = split && splits(f);
+        p.smem = tile_smem(d.shape.g.F(), groups, f.ilp * f.pair, nstages, d.shape.top_stride, w, p.split);
         return p;
     };
     Plan generic, staged;
@@ -641,7 +668,7 @@ inline Plan make_plan(const Dev& d, const Tune& tune, int want, Walk w = Walk::F
         const int row = tile_row(tune.ilp ? tune.ilp : c[0], tune.pair ? tune.pair : c[1], true);
         const int ilp = kTileFamilies[row].ilp, pair = kTileFamilies[row].pair;
         const int st = std::max(1, std::min(tune.stages ? tune.stages : c[2], 4));
-        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps, w);
+        const int g = tile_groups(d, kTileFamilies[row], st, tune.warps, w, split);
         const int score = g * pair * ilp * 8 + (pair == 2 ? 4 : 0) - (pair == 4 ? 4 : 0) + st;
         if (g >= 1 && score > best) { best = score; staged = tile_plan(row, st, g); }
         if (tune.ilp && tune.stages && tune.pair) break;
@@ -666,8 +693,9 @@ inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
     const bool phased = tune.phased >= 1 || (tune.phased == -1 && d.shape.Dtop >= 10);
     // part A = levels 0..Lw; DTE_TUNE phased=k moves the split k-1 levels further up (smaller part A)
     const uint32_t up = tune.phased > 1 ? (uint32_t)tune.phased - 1 : 0;
-    // a binned part A of 8 << Lw bytes is no whole number of 16-byte bulk-copy units at Lw = 0
-    const bool fits = d.shape.Dtop >= 3 + up + (pl.walk == Walk::Binned ? 1 : 0);
+    // a binned part A of 8 << Lw bytes is no whole number of 16-byte bulk-copy units at Lw = 0, nor the 4 << Lw bytes of
+    // the meta run of split tops below Lw = 2
+    const bool fits = d.shape.Dtop >= 3 + up + (pl.walk == Walk::Binned ? 1 : pl.split ? 2 : 0);
     return (phased && fits && pl.nstages <= 4) ? d.shape.Dtop - 3 - up : 0xFFFFFFFFu;
 }
 
@@ -679,7 +707,7 @@ inline uint32_t phased_level(const Dev& d, const Tune& tune, const Plan& pl) {
 constexpr uint64_t kMeasureHintTuples = 8000000;
 constexpr double kPlanMargin = 0.02;
 inline bool tune_pinned(const Tune& t) {
-    return t.ilp || t.stages || t.warps || t.pair || t.fill || t.phased != -1;
+    return t.ilp || t.stages || t.warps || t.pair || t.fill || t.phased != -1 || t.tops;
 }
 // Whether loading an ensemble times the plans: only on a single-device handle whose plan no DTE_TUNE knob pins and no
 // forced kernel variant overrides, configured for at least kMeasureHintTuples tuples.
@@ -709,6 +737,20 @@ constexpr auto tile_kernel_table(std::index_sequence<R...>) {
           tile_kernel<R, true, false, true>, tile_kernel<R, true, true, true>}...}};
 }
 inline constexpr auto kTileKernels = tile_kernel_table(std::make_index_sequence<kNumTileFamilies>());
+// The split-tops walk of family R (rows with splits()) with the given WIDE flag and thread bound nt
+template <int R, bool WIDE>
+WalkKernel tile_split_kernel(int nt) {
+    constexpr TileFamily f = kTileFamilies[R];
+    if constexpr (!splits(f)) return nullptr;
+    else return nt == f.nt ? dt_walk_tile_split<f.ilp, f.pair, WIDE, f.nt> : dt_walk_tile_split<f.ilp, f.pair, WIDE, std::min(f.nt, 384)>;
+}
+// [row][WIDE]
+template <size_t... R>
+constexpr auto tile_split_kernel_table(std::index_sequence<R...>) {
+    using Pick = WalkKernel (*)(int);
+    return std::array<std::array<Pick, 2>, sizeof...(R)>{{{tile_split_kernel<R, false>, tile_split_kernel<R, true>}...}};
+}
+inline constexpr auto kTileSplitKernels = tile_split_kernel_table(std::make_index_sequence<kNumTileFamilies>());
 // [4 * BIN + 2 * WIDE + MC]
 inline constexpr WalkKernel kGenericKernels[8] = {
     dt_walk_generic<false, false, false>, dt_walk_generic<false, true, false>, dt_walk_generic<true, false, false>,
@@ -719,7 +761,7 @@ inline constexpr WalkKernel kGenericKernels[8] = {
 // the missing pattern of `run`.  The launchers add what their walk reads and writes.
 inline WalkParams walk_params(const Dev& d, const Geom& run, const Tune& tune, const Plan& pl, const void* d_tuples, size_t n) {
     WalkParams wp = {};
-    wp.top = d.d_top;
+    wp.top = pl.split ? reinterpret_cast<const uint2*>(d.d_top_split) : d.d_top;
     wp.tuples = static_cast<const float*>(d_tuples);
     wp.n = n;
     wp.F = d.shape.g.F();
@@ -783,7 +825,10 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     if (u8) wp.missing = 255u;                       // the bin of the missing pattern
     wp.accumulate = accumulate ? 1u : 0u;
     const int v = 4 * u8 + 2 * pl.wide + mc;
-    return launch_plan(d, pl, pl.row < 0 ? kGenericKernels[v] : kTileKernels[pl.row][v](pl.thread_bound()), wp, n, st, why);
+    const WalkKernel k = pl.row < 0 ? kGenericKernels[v]
+                       : pl.split  ? kTileSplitKernels[pl.row][pl.wide](pl.thread_bound())
+                                   : kTileKernels[pl.row][v](pl.thread_bound());
+    return launch_plan(d, pl, k, wp, n, st, why);
 }
 
 using LeafKernel = void (*)(LeafParams);
@@ -1038,6 +1083,10 @@ inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, siz
         snprintf(buf, len, "dt_walk_tile%s<%d, %d, %d, %d, %d> warps=%d stages=%d phased=%d threads=%d smem=%zu",
                  sfx, f.ilp, f.pair, f.staged ? 1 : 0, pl.wide ? 1 : 0, pl.thread_bound(), pl.nwarps, pl.nstages,
                  phased_level(d, tune, pl) != 0xFFFFFFFFu ? 1 : 0, pl.threads(), pl.smem);
+        if (pl.split) {
+            const size_t used = strlen(buf);
+            if (used < len) snprintf(buf + used, len - used, " tops=6");
+        }
     }
     if (d.shape.C >= 2) {
         const size_t used = strlen(buf);

@@ -318,7 +318,7 @@ uint32_t classes_of(const dte_engine* e) { return host_dev(e).shape.C; }
 // ---- placement of the ensemble on the devices ---------------------------------------------------------
 void free_ensemble(Dev& d) {
     cudaSetDevice(d.ordinal);
-    for (void* p : {(void*)d.d_top, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges,
+    for (void* p : {(void*)d.d_top, (void*)d.d_top_split, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges,
                     (void*)d.d_bottom_id, (void*)d.d_shap_nodes, (void*)d.d_shap_paths, (void*)d.d_shap_tree_path,
                     (void*)d.d_shap_cls_tree, (void*)d.d_shap_scratch})
         if (p) cudaFree(p);
@@ -331,6 +331,7 @@ void free_ensemble(Dev& d) {
     d.shap_scratch_words = 0;
     d.shap = ShapLayout();
     d.d_top = nullptr;
+    d.d_top_split = nullptr;
     d.d_bottom = nullptr;
     d.d_top_b = nullptr;
     d.d_bottom_b = nullptr;
@@ -353,9 +354,10 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
     CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
     free_ensemble(d);
     TRY(upload(e, d.d_top, pk.top));
+    TRY(upload(e, d.d_top_split, pk.top_split));
     TRY(upload(e, d.d_bottom, pk.bottom));
     d.shape = pk.shape;
-    d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.bottom.size() * sizeof(uint4);
+    d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.top_split.size() * sizeof(uint16_t) + pk.bottom.size() * sizeof(uint4);
     if (bins) {
         TRY(upload(e, d.d_top_b, pk.top_b));
         TRY(upload(e, d.d_bottom_b, pk.bottom_b));
@@ -1689,7 +1691,8 @@ struct PlanTiming {
 };
 
 // Time the fp32 walk of the resident ensemble on device d under `base` and under each staged candidate that fits and
-// plans a launch not yet timed, on synthetic tuples generated on the device; out[0] is `base`.  Every plan walks the
+// plans a launch not yet timed, each with the 8-byte tree tops and with the 6-byte split tops (a single-class ensemble;
+// the smaller ring stage may fit a tuple group more), on synthetic tuples generated on the device; out[0] is `base`.  Every plan walks the
 // largest whole number of its own waves of tiles that fits in max(n, 2 waves) tuples, since a partial last wave would
 // charge plans with smaller tiles for idle SMs.  One round of launches warms up, then kPlanReps rounds visit the plans
 // in turn; a plan's rate is its median.
@@ -1698,23 +1701,26 @@ static int time_plans(dte_t* e, Dev& d, const Tune& base, size_t n, std::vector<
     struct Cand { int row, stages, phased, warps; };            // warps = 10: the 384-thread (168-register) instantiation
     const int r42 = tile_row(4, 2, true), r24 = tile_row(2, 4, true), r81 = tile_row(8, 1, true), r41 = tile_row(4, 1, true),
               r22 = tile_row(2, 2, true);
-    // the last three cap the tuple tile at 4 or 5 groups, which leaves the bottom-record gather more L1 (DESIGN.md §4)
+    // {r42, 1, 1, 8}, {r22, 1, 1, 10} and {r24, 1, 1, 16} cap the tuple tile at 4 or 5 groups, which leaves the
+    // bottom-record gather more L1 (DESIGN.md §4); the two-stage SP = 8 pair families fit 4 groups with split tops
     const Cand cands[] = {{r42, 1, 1, 0}, {r42, 1, 0, 0}, {r42, 1, 1, 10}, {r42, 1, 0, 10}, {r24, 1, 1, 0}, {r24, 1, 0, 0}, {r81, 1, 0, 0},
                           {r81, 2, 0, 0}, {r41, 2, 0, 0}, {r22, 2, 0, 0}, {r22, 1, 0, 0}, {r42, 1, 1, 8}, {r22, 1, 1, 10},
-                          {r24, 1, 1, 16}};
+                          {r24, 1, 1, 16}, {r42, 2, 0, 0}, {r24, 2, 0, 0}};
     char name[256];
     out.clear();
     out.push_back({base, "", 0});
-    for (const Cand& c : cands) {
-        const TileFamily& f = kTileFamilies[c.row];
-        // the planner stages a pinned family only with >= 2 consumer warps, and a cap is only worth timing when it
-        // removes a tuple group; a plan that stages can always refill phased (Dtop >= 3, at most 4 stages)
-        const int groups = tile_groups(d, f, c.stages, c.warps);
-        if (groups * f.pair < 2 || (c.warps && tile_groups(d, f, c.stages, 0) * f.pair <= c.warps)) continue;
-        Tune t = base;
-        t.ilp = f.ilp; t.pair = f.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps;
-        out.push_back({t, "", 0});
-    }
+    for (const int tops : {0, 6})
+        for (const Cand& c : cands) {
+            const TileFamily& f = kTileFamilies[c.row];
+            // the planner stages a pinned family only with >= 2 consumer warps, and a cap is only worth timing when it
+            // removes a tuple group; a plan that stages can always refill phased (Dtop >= 3, at most 4 stages)
+            const bool split = tops == 6 && d.shape.C == 1;
+            const int groups = tile_groups(d, f, c.stages, c.warps, Walk::Fp32, split);
+            if (groups * f.pair < 2 || (c.warps && tile_groups(d, f, c.stages, 0, Walk::Fp32, split) * f.pair <= c.warps)) continue;
+            Tune t = base;
+            t.ilp = f.ilp; t.pair = f.pair; t.stages = c.stages; t.phased = c.phased; t.warps = c.warps; t.tops = tops;
+            out.push_back({t, "", 0});
+        }
     size_t wave_max = 0;
     std::vector<size_t> waves;
     for (PlanTiming& p : out) {

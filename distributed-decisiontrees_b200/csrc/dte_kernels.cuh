@@ -35,7 +35,8 @@
 namespace dte {
 
 struct WalkParams {
-    const uint2* top;           // [trees_padded][top_stride] {thr bits, fidx | (8+8*missing_right)<<16}
+    const uint2* top;           // [trees_padded][top_stride] {thr bits, fidx | (8+8*missing_right)<<16};
+                                // dt_walk_tile_split: the split tops (PackedEnsemble::top_split) instead
     const uint4* bottom;        // [trees_padded][nb][BOT_VEC] see repack in dte_engine.cu
     const float* tuples;        // [n][F] row-major fp32 (the reference's tuple CLs)
     float* scores;              // [n]
@@ -99,6 +100,11 @@ __device__ __forceinline__ uint2 lds64(uint32_t addr) {
 __device__ __forceinline__ uint32_t lds8(uint32_t addr) {
     uint32_t v;
     asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
+}
+__device__ __forceinline__ uint32_t lds16(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(addr));
     return v;
 }
 __device__ __forceinline__ uint32_t lds32(uint32_t addr) {
@@ -236,6 +242,24 @@ __device__ __forceinline__ uint32_t step_select(uint32_t x, uint32_t thr, uint32
         "}"
         : "=r"(r) : "r"(x), "r"(thr), "r"(missing), "r"(meta), "r"(a_left), "r"(a_right));
     return r;
+}
+// step_select for the split tree tops (meta = fidx | missing_right << 15), which walk two addresses per level, one into
+// the threshold run and one into the meta run: one decision, two selects.
+__device__ __forceinline__ void step_select_split(uint32_t x, uint32_t thr, uint32_t meta, uint32_t missing, uint32_t a_left,
+                                                  uint32_t a_right, uint32_t b_left, uint32_t b_right, uint32_t& a, uint32_t& b) {
+    asm("{\n\t"
+        ".reg .pred pge, pm, pmr, t1, t2, npm, pr;\n\t"
+        "setp.ge.s32 pge, %2, %3;\n\t"
+        "setp.eq.u32 pm, %2, %4;\n\t"
+        "setp.ge.u32 pmr, %5, 32768;\n\t"       // bit 15: missing goes right
+        "and.pred t1, pm, pmr;\n\t"
+        "not.pred npm, pm;\n\t"
+        "and.pred t2, npm, pge;\n\t"
+        "or.pred pr, t1, t2;\n\t"
+        "selp.u32 %0, %7, %6, pr;\n\t"
+        "selp.u32 %1, %9, %8, pr;\n\t"
+        "}"
+        : "=r"(a), "=r"(b) : "r"(x), "r"(thr), "r"(missing), "r"(meta), "r"(a_left), "r"(a_right), "r"(b_left), "r"(b_right));
 }
 
 // Fields of a tree-top record as step_select() takes them.  fp32 (8 bytes): {thr bits, fidx | (8 + 8*missing_right) << 16}.
@@ -563,7 +587,10 @@ __device__ __forceinline__ void ring_init(const WalkParams& p, uint32_t sbase) {
 //   levels 0..Lw of step q+1, A of step q+1 under the last level + bottom records + leaf sums of step q.  Bulk copies
 //   move multiples of 16 bytes, and a binned part A of 8 << Lw bytes is none at Lw = 0, so the planner never phases a
 //   binned walk at Lw = 0.
-template <int SP>
+// SPLIT: split tree tops (dt_walk_tile_split), a run of 4-byte thresholds then a run of 2-byte metas, 6 bytes per record.
+//   Part A is then the first 8 << Lw bytes of the threshold run and the first 4 << Lw of the meta run (the same records),
+//   two copies per tree and part; the planner phases them only from Lw = 2, where both are whole 16-byte units.
+template <int SP, bool SPLIT = false>
 __device__ __forceinline__ void ring_produce(const WalkParams& p, uint32_t sbase, const void* tops, uint32_t tree_bytes,
                                              uint32_t stage_bytes, uint32_t steps, uint32_t my_tiles, uint32_t unitA) {
     const uint64_t total = (uint64_t)my_tiles * steps;
@@ -578,6 +605,20 @@ __device__ __forceinline__ void ring_produce(const WalkParams& p, uint32_t sbase
         const char* src = src0 + (size_t)q * stage_bytes;
         mbar_wait(sbase + 8 * (p.nstages + slot), par);
         const uint32_t full = sbase + 8 * slot;
+#ifdef DTE_FILL_SKIP_ABLATION
+        // Timing experiment, never defined by the library (DESIGN.md §4): after the first fill of every slot the producer
+        // only arrives, so the walk reads stale (still valid) tree tops and its scores are wrong by design.
+        if (it >= p.nstages) {
+            mbar_arrive(full);
+            if (phased) {
+                mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
+                mbar_arrive(sbase + 8 * (2 * p.nstages + slot));
+            }
+            if (++q == steps) q = 0;
+            if (++slot == p.nstages) { slot = 0; par ^= 1; }
+            continue;
+        }
+#endif
         if (!phased) {
             mbar_arrive_expect_tx(full, stage_bytes);
             if (p.fill_split == 0) {
@@ -585,6 +626,22 @@ __device__ __forceinline__ void ring_produce(const WalkParams& p, uint32_t sbase
             } else {
 #pragma unroll
                 for (int c = 0; c < SP; ++c) bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, tree_bytes, full);
+            }
+        } else if constexpr (SPLIT) {
+            const uint32_t runT = tree_bytes / 6u * 4u, aT = 8u << p.Lw, aM = 4u << p.Lw;   // threshold run, part A pieces
+            mbar_arrive_expect_tx(full, (uint32_t)SP * (aT + aM));
+#pragma unroll
+            for (int c = 0; c < SP; ++c) {
+                bulk_g2s(dst + c * tree_bytes, src + (size_t)c * tree_bytes, aT, full);
+                bulk_g2s(dst + c * tree_bytes + runT, src + (size_t)c * tree_bytes + runT, aM, full);
+            }
+            mbar_wait(sbase + 8 * (3 * p.nstages + slot), par);
+            const uint32_t fullB = sbase + 8 * (2 * p.nstages + slot);
+            mbar_arrive_expect_tx(fullB, (uint32_t)SP * (tree_bytes - aT - aM));
+#pragma unroll
+            for (int c = 0; c < SP; ++c) {
+                bulk_g2s(dst + c * tree_bytes + aT, src + (size_t)c * tree_bytes + aT, runT - aT, fullB);
+                bulk_g2s(dst + c * tree_bytes + runT + aM, src + (size_t)c * tree_bytes + runT + aM, tree_bytes - runT - aM, fullB);
             }
         } else {
             mbar_arrive_expect_tx(full, (uint32_t)SP * bytesA);
@@ -606,9 +663,11 @@ __device__ __forceinline__ void ring_produce(const WalkParams& p, uint32_t sbase
 // per-thread limit is set by ceil(warps / 4): 9..12 warps -> 168 registers, 13..16 warps -> 128.  The planner
 // picks the 384-thread instantiation whenever the plan fits in 12 warps (cfg3: 5 tuple groups x 2 + producer).
 // MC: multi-class walk (see dt_walk_generic); the producer warp is the same, only sub 0's accumulation changes.
-template <int ILP, int P, bool STAGED, bool WIDE, int NT, bool MC>
-__global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
+// SPLIT: the ring holds split tree tops (dt_walk_tile_split); the body of dt_walk_tile and dt_walk_tile_split.
+template <int ILP, int P, bool STAGED, bool WIDE, int NT, bool MC, bool SPLIT>
+__device__ __forceinline__ void tile_walk(const WalkParams& p) {
     static_assert(ILP * P == 8 || ILP * P == 4, "a step covers a tree8 group or half of one");
+    static_assert(STAGED || !SPLIT, "split tree tops are a ring format");
     constexpr int BV = WIDE ? 4 : 2;
     constexpr int SP = ILP * P;                         // trees per ring stage / per step
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -616,7 +675,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
     const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t G = p.nwarps / P;                    // tuple groups per CTA
     const uint32_t M = 32u * G;
-    const uint32_t tree_bytes = p.top_stride * 8u;
+    const uint32_t tree_bytes = p.top_stride * (SPLIT ? 6u : 8u);
     const uint32_t stage_bytes = (uint32_t)SP * tree_bytes;
     const uint32_t ring_bytes = STAGED ? p.nstages * stage_bytes : 0u;
     const uint32_t xs_base = sbase + kHdrBytes + ring_bytes;
@@ -627,7 +686,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
     if (STAGED) {
         ring_init(p, sbase);
         if (warp == p.nwarps) {                         // producer: stream tree tops through the ring
-            if (lane == 0) ring_produce<SP>(p, sbase, p.top, tree_bytes, stage_bytes, steps, my_tiles, 16u);
+            if (lane == 0) ring_produce<SP, SPLIT>(p, sbase, p.top, tree_bytes, stage_bytes, steps, my_tiles, SPLIT ? 12u : 16u);
             return;
         }
     }
@@ -751,9 +810,14 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
                 // Absolute shared-memory addresses: with A = tb_c + o the child address is
                 // A' = tb_c + 2o + 8 + 8*right = (2A + 8 - tb_c) + 8*right.  2A + (8 - tb_c) does not depend
                 // on the feature, so only {compare, select, add} sit between the feature and the next node.
-                uint32_t A[ILP], kb8[ILP];
+                // SPLIT: node n of a tree is thr at tb_c + 4n and meta at tm_c + 2n (tm_c = tb_c + 4 * top_stride);
+                // both addresses step the same way, A' = (2A + 4 - tb_c) + 4*right and B' = (2B + 2 - tm_c) + 2*right.
+                uint32_t A[ILP], kb8[ILP], B[ILP], kbm[ILP];
 #pragma unroll
-                for (int c = 0; c < ILP; ++c) { A[c] = tb + c * tree_bytes; kb8[c] = 8u - A[c]; }
+                for (int c = 0; c < ILP; ++c) {
+                    A[c] = tb + c * tree_bytes; kb8[c] = (SPLIT ? 4u : 8u) - A[c];
+                    if constexpr (SPLIT) { B[c] = A[c] + 4u * p.top_stride; kbm[c] = 2u - B[c]; }
+                }
                 // Skewed schedule inside the warp.  A walk step has three dependent stages:
                 //   S1 node record  = LDS.64 [A]            S2 feature = LDS [xs + fidx*row]
                 //   S3 compare + child address (ALU)
@@ -765,11 +829,19 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
                 constexpr int H = ILP / 2;
                 uint2 nd[ILP];
                 uint32_t xv[ILP];
-                auto S1 = [&](int c) { nd[c] = lds64(A[c]); };
-                auto S2 = [&](int c) { xv[c] = feat(nd[c].y & 0xFFFFu); };
+                auto S1 = [&](int c) {
+                    if constexpr (SPLIT) nd[c] = make_uint2(lds32(A[c]), lds16(B[c]));   // {thr, meta}: two independent loads
+                    else nd[c] = lds64(A[c]);
+                };
+                auto S2 = [&](int c) { xv[c] = feat(nd[c].y & (SPLIT ? 0x7FFFu : 0xFFFFu)); };
                 auto S3 = [&](int c) {
                     const uint32_t a2 = A[c] + A[c] + kb8[c];
-                    A[c] = step_select(xv[c], nd[c].x, nd[c].y, p.missing, a2, a2 + 8u);
+                    if constexpr (SPLIT) {
+                        const uint32_t b2 = B[c] + B[c] + kbm[c];
+                        step_select_split(xv[c], nd[c].x, nd[c].y, p.missing, a2, a2 + 4u, b2, b2 + 2u, A[c], B[c]);
+                    } else {
+                        A[c] = step_select(xv[c], nd[c].x, nd[c].y, p.missing, a2, a2 + 8u);
+                    }
                 };
 #pragma unroll
                 for (int c = 0; c < ILP; ++c) S1(c);                         // level 0 nodes
@@ -812,7 +884,7 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
             // bottom: last two comparison levels + leaves, ONE 32 B (64 B) record per walk
 #pragma unroll
             for (int c = 0; c < ILP; ++c) {
-                const uint32_t j = (o[c] >> 3) - (p.nb - 1);
+                const uint32_t j = (o[c] >> (SPLIT ? 2 : 3)) - (p.nb - 1);
                 if constexpr (WIDE) bot_load_tile(dst[c], p.bottom + ((size_t)(t0 + c) * p.nb + j) * BV);
                 else bot_load_pair<ILP < 8>(dst[c], p.bottom + (size_t)(t0 + c) * p.nb * BV, j);
             }
@@ -856,6 +928,19 @@ __global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
             }
         }
     }
+}
+
+template <int ILP, int P, bool STAGED, bool WIDE, int NT, bool MC>
+__global__ void __launch_bounds__(NT, 1) dt_walk_tile(const WalkParams p) {
+    tile_walk<ILP, P, STAGED, WIDE, NT, MC, false>(p);
+}
+// The staged walk with split tree tops: WalkParams::top points at the split layout (PackedEnsemble::top_split), a tree
+// top of thr[top_stride] (u32) then meta[top_stride] (u16, fidx | missing_right << 15), 6 bytes per record instead of 8.
+// The compare is the same, so the scores are those of dt_walk_tile word for word; the ring stage shrinks by a quarter,
+// which leaves that much more shared memory to L1 (DESIGN.md §4).  Single-class walks only.
+template <int ILP, int P, bool WIDE, int NT>
+__global__ void __launch_bounds__(NT, 1) dt_walk_tile_split(const WalkParams p) {
+    tile_walk<ILP, P, true, WIDE, NT, false, true>(p);
 }
 
 // The binned tile walk (DESIGN.md §9): dt_walk_tile on u8 bins (WalkParams::bins) and 4-byte tree tops (top4), with

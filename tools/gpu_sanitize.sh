@@ -2,7 +2,8 @@
 # compute-sanitizer over the walk kernel that SHIPS for the headline geometry (D = 12, F = 256, AUTO plan =
 # dt_walk_tile<4,2,1,0,384>, phased ring refill, CTAs with two tiles) and over the planner's alternatives.
 # Logs (with the kernel name printed by the test) go to <logdir>/sanitizer_<tool>_<plan>.log.
-#   bash tools/gpu_sanitize.sh [logdir=sanitizer_logs]   memcheck + synccheck over four launch plans, a 3-class
+#   bash tools/gpu_sanitize.sh [logdir=sanitizer_logs]   memcheck + synccheck over six launch plans (two of them
+#                                                        with split tree tops, DTE_TUNE tops=6), a 3-class
 #                                                        ensemble, seven kernel-matrix instantiations, the binned and
 #                                                        the leaf walks, memcheck over the sparse densify kernel,
 #                                                        racecheck
@@ -23,6 +24,8 @@ run() { # tool tune extra-args
 }
 for tool in memcheck synccheck; do
   for tune in "" "pair=4,stages=1" "pair=1,ilp=8,stages=1" "pair=2,ilp=2,stages=2"; do run $tool "$tune" ""; done
+  # split tree tops (dt_walk_tile_split): the two-stage plan the cfg3 handle measures fastest, and a phased one
+  for tune in "pair=4,stages=2,phased=0,tops=6" "pair=4,stages=1,phased=1,tops=6"; do run $tool "$tune" ""; done
 done
 # the multi-class epilogue (C = 3, class-boundary stores and the argmax read-back) in the same geometry
 T=tests/test_gpu_multiclass.py::test_multiclass_headline_geometry_multi_tile

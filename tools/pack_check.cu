@@ -10,6 +10,10 @@
 //   pack_check leaf <same arguments>
 //     ->  n*T uint16 leaf cells (binary, stdout): the leaf-id layout (bottom_id) packed as well and decoded as the leaf
 //         walks decode it, the cell in the stream tree's own heap that each (tuple, tree) ends in
+//   pack_check split <same arguments>
+//     ->  the leaf words, with the top levels walked through the split tree tops (top_split) as dt_walk_tile_split
+//         walks them
+// Every run also decodes every record of top_split and checks it against the same record of top (exit 7 otherwise).
 #include "../distributed-decisiontrees_b200/csrc/dte_device.cuh"
 #include <cstdio>
 #include <cstring>
@@ -28,20 +32,41 @@ static std::vector<unsigned char> slurp(const char* p) {
 
 // leaf word of tree slot `slot` of the packed layout for tuple x, decoded as the kernels decode it
 // `bottom`: pk.bottom (leaf words) or pk.bottom_id (leaf cells)
-static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x, uint32_t missing, const std::vector<uint4>& bottom) {
+// `split`: walk the top levels through top_split instead of top
+static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x, uint32_t missing, const std::vector<uint4>& bottom,
+                     bool split = false) {
     const EnsembleShape& sh = pk.shape;
     const int BV = sh.wide ? 4 : 2;
-    // top: byte offset o into the tree's 8-byte heap records, child = 2o + 8 + 8*right  (step_inc in dte_kernels.cuh)
-    uint32_t o = 0;
-    const uint2* tp = pk.top.data() + (size_t)slot * sh.top_stride;
-    for (uint32_t lvl = 0; lvl < sh.Dtop; ++lvl) {
-        const uint2 nd = tp[o / 8];
-        const uint32_t xv = x[nd.y & 0xFFFFu];
-        uint32_t inc = ((int32_t)xv < (int32_t)nd.x) ? 8u : 16u;
-        if (xv == missing) inc = nd.y >> 16;
-        o = 2 * o + inc;
+    uint32_t j;
+    if (split) {
+        // byte offsets a into the threshold run and b into the meta run, stepped alike: a' = 2a + 4 + 4*right,
+        // b' = 2b + 2 + 2*right (S3 of tile_walk with SPLIT)
+        const unsigned char* ts = reinterpret_cast<const unsigned char*>(pk.top_split.data() + (size_t)slot * sh.top_stride * 3);
+        uint32_t a = 0, b = 0;
+        for (uint32_t lvl = 0; lvl < sh.Dtop; ++lvl) {
+            uint32_t thr;
+            uint16_t meta;
+            memcpy(&thr, ts + a, 4);
+            memcpy(&meta, ts + 4 * sh.top_stride + b, 2);
+            const uint32_t xv = x[meta & 0x7FFFu];
+            const bool right = xv == missing ? (meta >= 0x8000u) : !((int32_t)xv < (int32_t)thr);
+            a = 2 * a + 4 + 4 * right;
+            b = 2 * b + 2 + 2 * right;
+        }
+        j = (a >> 2) - (sh.nb - 1);
+    } else {
+        // top: byte offset o into the tree's 8-byte heap records, child = 2o + 8 + 8*right  (step_inc in dte_kernels.cuh)
+        uint32_t o = 0;
+        const uint2* tp = pk.top.data() + (size_t)slot * sh.top_stride;
+        for (uint32_t lvl = 0; lvl < sh.Dtop; ++lvl) {
+            const uint2 nd = tp[o / 8];
+            const uint32_t xv = x[nd.y & 0xFFFFu];
+            uint32_t inc = ((int32_t)xv < (int32_t)nd.x) ? 8u : 16u;
+            if (xv == missing) inc = nd.y >> 16;
+            o = 2 * o + inc;
+        }
+        j = (o >> 3) - (sh.nb - 1);
     }
-    const uint32_t j = (o >> 3) - (sh.nb - 1);
     const uint4* rec = bottom.data() + ((size_t)slot * sh.nb + j) * BV;
     uint32_t fp, fl_, fr, mp, ml, mr; uint4 leaves;
     if (sh.wide) {
@@ -61,7 +86,8 @@ static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x,
 
 int main(int argc, char** argv) {
     const bool leaf = argc > 1 && !strcmp(argv[1], "leaf");
-    if (leaf) { --argc; ++argv; }
+    const bool split = argc > 1 && !strcmp(argv[1], "split");
+    if (leaf || split) { --argc; ++argv; }
     if (argc < 9) return 2;
     Geom g;
     g.D = (uint32_t)atoi(argv[1]); const uint32_t F = (uint32_t)atoi(argv[2]), T = (uint32_t)atoi(argv[3]);
@@ -90,6 +116,20 @@ int main(int argc, char** argv) {
         fprintf(stderr, "shape: gpc %u (want %u) cls_max %u (want %u) Tpad %u\n", sh.gpc, gpc, sh.cls_max, cmax, sh.Tpad);
         return 4;
     }
+    // top_split record by record against top: the same threshold word, feature index and missing direction
+    if (pk.top_split.size() != (size_t)sh.Tpad * sh.top_stride * 3) return 7;
+    for (uint32_t s = 0; s < sh.Tpad; ++s)
+        for (uint32_t k = 0; k < sh.top_stride; ++k) {
+            const uint2 nd = pk.top[(size_t)s * sh.top_stride + k];
+            const uint16_t* ts = pk.top_split.data() + (size_t)s * sh.top_stride * 3;
+            uint32_t thr;
+            memcpy(&thr, ts + 2 * k, 4);
+            const uint16_t meta = ts[2 * sh.top_stride + k];
+            if (thr != nd.x || (meta & 0x7FFFu) != (nd.y & 0xFFFFu) || (meta >> 15) != ((nd.y >> 16) == 16u ? 1u : 0u)) {
+                fprintf(stderr, "slot %u record %u: split {%08x, %04x} against {%08x, %08x}\n", s, k, thr, meta, nd.x, nd.y);
+                return 7;
+            }
+        }
     std::vector<uint8_t> used(sh.Tpad, 0);
     for (uint32_t t = 0; t < T; ++t) { slot[t] += ((first + t) % C) * gpc * 8; used[slot[t]] = 1; }
     const uint32_t* X = reinterpret_cast<const uint32_t*>(xs.data());
@@ -108,9 +148,9 @@ int main(int argc, char** argv) {
     std::vector<uint32_t> out(n * T);
     for (size_t i = 0; i < n; ++i) {
         const uint32_t* x = X + i * F;
-        for (uint32_t t = 0; t < T; ++t) out[i * T + t] = walk(pk, slot[t], x, g.missing, pk.bottom);
+        for (uint32_t t = 0; t < T; ++t) out[i * T + t] = walk(pk, slot[t], x, g.missing, pk.bottom, split);
         for (uint32_t s = 0; s < sh.Tpad; ++s)
-            if (!used[s] && walk(pk, s, x, g.missing, pk.bottom) != 0u) {
+            if (!used[s] && walk(pk, s, x, g.missing, pk.bottom, split) != 0u) {
                 fprintf(stderr, "padding slot %u gives a non-zero leaf for tuple %zu\n", s, i);
                 return 5;
             }

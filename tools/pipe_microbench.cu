@@ -313,7 +313,8 @@ static void replay_row(const char* name, const uint4* bottom, const uint16_t* id
 }
 
 // --replay FILE: the cfg3 record stream of tools/gather_paths.py against uniformly random records of the same shape,
-// with the cfg3 plan's 5 tuple groups (231,552 B of shared memory) and with 4 (DTE_TUNE=warps=8: 198,784 B)
+// with the cfg3 plan's 5 tuple groups (231,552 B of shared memory), with 4 (DTE_TUNE=warps=8: 198,784 B) and with 4 next
+// to a ring of split tree tops (182,400 B)
 static int run_replay(const char* path) {
     FILE* f = fopen(path, "rb");
     uint32_t hdr[4] = {0, 0, 0, 0};
@@ -341,7 +342,9 @@ static int run_replay(const char* path) {
            "\"trees\": %u, \"records_per_tree\": %u,\n", prop.name, g_sms, T, nb);
     replay_row("uniform_5_groups", bottom, d_uniform, T, N, nb, 10, 231552, sink, cyc, false);
     replay_row("cfg3_stream_5_groups", bottom, d_stream, T, N, nb, 10, 231552, sink, cyc, false);
-    replay_row("cfg3_stream_4_groups", bottom, d_stream, T, N, nb, 8, 198784, sink, cyc, true);
+    replay_row("cfg3_stream_4_groups", bottom, d_stream, T, N, nb, 8, 198784, sink, cyc, false);
+    // 4 groups next to a 48 KiB ring stage of 6-byte split tops instead of 64 KiB of 8-byte ones: 16 KiB more L1
+    replay_row("cfg3_stream_4_groups_split_tops", bottom, d_stream, T, N, nb, 8, 198784 - 16384, sink, cyc, true);
     printf("}\n");
     return cudaGetLastError() == cudaSuccess ? 0 : 1;
 }
