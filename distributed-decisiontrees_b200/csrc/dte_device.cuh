@@ -161,9 +161,6 @@ struct ShapLayout {
     std::vector<unsigned long long> tree_path;   // [Tl + 1] first path of each layout tree
     std::vector<uint32_t> cls_tree;      // [C + 1] first layout tree of each class
     std::vector<unsigned char> paths;    // [paths][stride]
-    size_t bytes() const {
-        return nodes.size() * sizeof(uint2) + tree_path.size() * 8 + cls_tree.size() * 4 + paths.size();
-    }
     size_t num_paths() const { return tree_path.empty() ? 0 : (size_t)tree_path.back(); }
 };
 
@@ -497,61 +494,158 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     return 0;
 }
 
+// ---- owning handles ----------------------------------------------------------------------------
+// A move-only owner of one CUDA object: Release runs on reset() and on destruction, with the device the object was made
+// on current (the caller's device is restored after).  An empty handle makes no CUDA call, so host-only tools can build
+// a Dev without a GPU.  size() is the element count an array handle was asked for.
+template <class H, class Release>
+class Owned {
+  public:
+    Owned() = default;
+    Owned(Owned&& o) noexcept { *this = std::move(o); }
+    Owned& operator=(Owned&& o) noexcept {
+        if (this != &o) {
+            reset();
+            h_ = std::exchange(o.h_, H());
+            n_ = std::exchange(o.n_, 0);
+            dev_ = o.dev_;
+        }
+        return *this;
+    }
+    ~Owned() { reset(); }
+    void reset() {
+        if (!h_) return;
+        int cur = dev_;
+        cudaGetDevice(&cur);
+        if (cur != dev_) cudaSetDevice(dev_);
+        Release()(h_);
+        if (cur != dev_) cudaSetDevice(cur);
+        h_ = H();
+        n_ = 0;
+    }
+    H release() {                     // hands the object to the caller, who then frees it
+        n_ = 0;
+        return std::exchange(h_, H());
+    }
+    H get() const { return h_; }
+    operator H() const { return h_; }
+    size_t size() const { return n_; }
+
+  protected:
+    // Release what the handle holds, then own what make(&h) creates on the current device.
+    template <class Make>
+    cudaError_t own(size_t n, Make make) {
+        reset();
+        H h = H();
+        const cudaError_t rc = make(&h);
+        if (rc != cudaSuccess) return rc;
+        cudaGetDevice(&dev_);
+        h_ = h;
+        n_ = n;
+        return cudaSuccess;
+    }
+
+  private:
+    H h_ = H();
+    size_t n_ = 0;
+    int dev_ = 0;
+};
+struct DeviceFree { void operator()(void* p) const { cudaFree(p); } };
+struct HostFree { void operator()(void* p) const { cudaFreeHost(p); } };
+struct EventDestroy { void operator()(cudaEvent_t ev) const { cudaEventDestroy(ev); } };
+struct StreamDestroy { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+
+// n elements of T in device memory; n = 0 still allocates one, so an empty upload leaves a non-null pointer
+template <class T>
+struct DevArray : Owned<T*, DeviceFree> {
+    cudaError_t alloc(size_t n) {
+        return this->own(n, [&](T** p) { return cudaMalloc(p, std::max<size_t>(n, 1) * sizeof(T)); });
+    }
+    size_t bytes() const { return this->size() * sizeof(T); }
+};
+template <class T>
+struct PinnedArray : Owned<T*, HostFree> {
+    cudaError_t alloc(size_t n, unsigned flags) {
+        return this->own(n, [&](T** p) { return cudaHostAlloc(p, n * sizeof(T), flags); });
+    }
+};
+struct Event : Owned<cudaEvent_t, EventDestroy> {
+    cudaError_t create(unsigned flags = cudaEventDisableTiming) {
+        return own(0, [&](cudaEvent_t* ev) { return cudaEventCreateWithFlags(ev, flags); });
+    }
+};
+struct Stream : Owned<cudaStream_t, StreamDestroy> {
+    cudaError_t create() {
+        return own(0, [](cudaStream_t* s) { return cudaStreamCreateWithFlags(s, cudaStreamNonBlocking); });
+    }
+};
+
+// The resident ensemble of one device, uploaded by upload_ensemble and dropped as one.  The arrays of a layout the load
+// did not build stay empty, so a walk's layout is resident when its first array is.
+struct ResidentLayout {
+    DevArray<uint2> top;
+    DevArray<uint16_t> top_split;     // PackedEnsemble::top_split
+    DevArray<uint4> bottom;
+    // binned layout (dte_load_ensemble_binned only): 4-byte tops, binned bottom records, the edge table (CSR)
+    DevArray<uint32_t> top_b;
+    DevArray<uint4> bottom_b;
+    DevArray<uint32_t> bin_off, bin_edges;
+    // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
+    DevArray<uint4> bottom_id;
+    // contribution layout (dte_load_ensemble_contribs only, DESIGN.md §12): the device copy of a ShapLayout
+    ShapLayout shap;                  // its shape; the host vectors stay empty
+    DevArray<uint2> shap_nodes;
+    DevArray<unsigned char> shap_paths;
+    DevArray<unsigned long long> shap_tree_path;
+    DevArray<uint32_t> shap_cls_tree;
+    // dte_info.ensemble_bytes: every array but the edge table
+    size_t bytes() const {
+        return top.bytes() + top_split.bytes() + bottom.bytes() + top_b.bytes() + bottom_b.bytes() + bottom_id.bytes() +
+               shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes();
+    }
+};
+
 // One landing slot: a device buffer the tuple stream lands in, plus the scores (labels) of its tuples.
 struct Slot {
-    unsigned char* d_tup = nullptr;
-    float* d_sc = nullptr;        // final scores of this slot (single / data-sharded / host node of a group)
-    float* d_part = nullptr;      // group (ensemble-sharded) mode: this device's partial scores
-    uint8_t* d_lb = nullptr;
+    DevArray<unsigned char> d_tup;
+    DevArray<float> d_sc;         // final scores of this slot (single / data-sharded / host node of a group)
+    DevArray<float> d_part;       // group (ensemble-sharded) mode: this device's partial scores
+    DevArray<uint8_t> d_lb;
     // leaf and contribution calls: [cap] result rows of row_bytes each (allocated by the first such call)
-    unsigned char* d_rows = nullptr;
-    // sparse host calls: the chunk's indptr slice and its entries, densified into d_tup (allocated by the first sparse call)
-    long long* d_sp_ptr = nullptr;
-    uint32_t* d_sp_idx = nullptr;
-    uint32_t* d_sp_val = nullptr;
+    DevArray<unsigned char> d_rows;
+    // sparse host calls: the chunk's indptr slice (cap_tuples + 1) and its entries, densified into d_tup (allocated by
+    // the first sparse call)
+    DevArray<long long> d_sp_ptr;
+    DevArray<uint32_t> d_sp_idx;
+    DevArray<uint32_t> d_sp_val;
     size_t fill = 0;              // bytes of tuple stream landed (or enqueued to land) in d_tup
     size_t walked = 0;            // whole tuples already submitted to the walk kernel
-    cudaEvent_t ev_walk = nullptr;   // last walk reading d_tup / writing d_sc, d_part
-    cudaEvent_t ev_d2h = nullptr;    // last D2H reading d_sc / d_lb
-    cudaEvent_t ev_land = nullptr;   // last copy into d_tup issued on THIS device's copy stream
-    cudaEvent_t ev_comb = nullptr;   // group mode, host device: last combine reading every device's d_part
+    Event ev_walk;                // last walk reading d_tup / writing d_sc, d_part
+    Event ev_d2h;                 // last D2H reading d_sc / d_lb
+    Event ev_land;                // last copy into d_tup issued on THIS device's copy stream
+    Event ev_comb;                // group mode, host device: last combine reading every device's d_part
 };
 
 struct Pending {              // one enqueued D2H of results: complete when `ev` fires
-    cudaEvent_t ev;
+    Event ev;
     uint64_t upto;            // device-local count of result tuples complete once ev has fired
 };
 
+// One device of a handle.  Move-only: it owns its streams, events and buffers, and releases them when it goes (the
+// streams last, as they are declared first).
 struct Dev {
+    Stream s_main, s_h2d, s_d2h;
     int ordinal = 0, sm_count = 0, smem_optin = 0;
-    cudaStream_t s_main = nullptr, s_h2d = nullptr, s_d2h = nullptr;
-    cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
+    Event ev_t0, ev_t1;
     bool timing_pending = false;
 
     // ---- resident ensemble ----
     EnsembleShape shape;              // of the resident ensemble; a run's K, S and missing are passed to launch_walk
-    uint2* d_top = nullptr;
-    uint16_t* d_top_split = nullptr;  // PackedEnsemble::top_split
-    uint4* d_bottom = nullptr;
-    uint64_t ensemble_bytes = 0;
-    // binned layout (dte_load_ensemble_binned only): 4-byte tops, binned bottom records, the edge table (CSR)
-    uint32_t* d_top_b = nullptr;
-    uint4* d_bottom_b = nullptr;
-    uint32_t* d_bin_off = nullptr;
-    uint32_t* d_bin_edges = nullptr;
-    // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
-    uint4* d_bottom_id = nullptr;
-    // contribution layout (dte_load_ensemble_contribs only, DESIGN.md §12): the device copy of a ShapLayout
-    ShapLayout shap;                  // its shape; the host vectors are released after the upload
-    uint2* d_shap_nodes = nullptr;
-    unsigned char* d_shap_paths = nullptr;
-    unsigned long long* d_shap_tree_path = nullptr;
-    uint32_t* d_shap_cls_tree = nullptr;
+    ResidentLayout layout;
     // dt_shap_generic's fp64 accumulators, guarded by the event of the last walk using them; a launch of `rows` tuples uses
     // [F + 1][rows] of them.  Sized in words, so a later ensemble with more features regrows it; a placement frees it.
-    double* d_shap_scratch = nullptr;
-    size_t shap_scratch_words = 0;
-    cudaEvent_t ev_shap = nullptr;
+    DevArray<double> d_shap_scratch;
+    Event ev_shap;
     Walk walk = Walk::Fp32;           // the walk the landing slots feed: binned calls land u8 bins (F bytes per tuple)
     size_t run_tuple_bytes() const { return walk == Walk::Binned ? shape.g.F() : shape.g.tuple_bytes(); }
 
@@ -560,31 +654,26 @@ struct Dev {
     size_t cap_tuples = 0;            // tuples per slot
     uint32_t slot_F = 0;
     uint32_t slot_C = 1;              // score words per tuple in d_sc / d_part (the resident ensemble's classes)
-    bool slot_parts = false;          // d_part allocated
     int cur = 0;                      // slot being filled
-    size_t slot_row_bytes = 0;        // bytes allocated per Slot::d_rows
     // result sink of the next submitted tuples: the caller's host rows (fast path), sink_pitch bytes apart (an
     // ensemble-sharded leaf call: this device's columns of the caller's rows), or, when null, the pinned ring (line stream)
     unsigned char* sink = nullptr;
     size_t sink_pitch = 0;
     uint8_t* sink_lb = nullptr;
-    size_t sparse_slot_nnz = 0;       // entries allocated per Slot::d_sp_idx / d_sp_val (d_sp_ptr holds cap_tuples + 1)
     // dte_infer_device_sparse: two [rows][F] buffers the chunks are densified into, each guarded by the event of its
     // last walk, so a call on another stream never overwrites rows a walk still reads
-    uint32_t* d_dense[2] = {nullptr, nullptr};
-    cudaEvent_t ev_dense[2] = {nullptr, nullptr};
-    size_t dense_bytes = 0;           // bytes of each d_dense buffer
-    float* h_ring = nullptr;          // pinned, device-local tuple order
-    size_t ring_cap = 0;              // tuples
+    DevArray<uint32_t> d_dense[2];
+    Event ev_dense[2];
+    PinnedArray<float> h_ring;        // device-local tuple order
     uint64_t res_enq = 0;             // result tuples whose D2H has been enqueued (device-local count)
     uint64_t res_done = 0;            // ... whose D2H has completed
     std::deque<Pending> pend;
-    std::vector<cudaEvent_t> ev_pool;
+    std::vector<Event> ev_pool;
 
     // pageable sources: a small pinned staging ring filled by a few copy threads, DMA'd from there (the driver's own
     // pageable path stages through one thread and reaches ~10 GB/s; PCIe Gen5 takes 55)
-    unsigned char* h_stage[3] = {nullptr, nullptr, nullptr};
-    cudaEvent_t ev_stage[3] = {nullptr, nullptr, nullptr};
+    PinnedArray<unsigned char> h_stage[3];
+    Event ev_stage[3];
     int stage_next = 0;
 
     uint64_t kernel_launches = 0;
@@ -761,7 +850,7 @@ inline constexpr WalkKernel kGenericKernels[8] = {
 // the missing pattern of `run`.  The launchers add what their walk reads and writes.
 inline WalkParams walk_params(const Dev& d, const Geom& run, const Tune& tune, const Plan& pl, const void* d_tuples, size_t n) {
     WalkParams wp = {};
-    wp.top = pl.split ? reinterpret_cast<const uint2*>(d.d_top_split) : d.d_top;
+    wp.top = pl.split ? reinterpret_cast<const uint2*>(d.layout.top_split.get()) : d.layout.top.get();
     wp.tuples = static_cast<const float*>(d_tuples);
     wp.n = n;
     wp.F = d.shape.g.F();
@@ -812,8 +901,8 @@ inline cudaError_t launch_walk(Dev& d, const Geom& run, const Tune& tune, int wa
     const bool u8 = w == Walk::Binned;
     const Plan pl = make_plan(d, tune, want_variant, w);
     WalkParams wp = walk_params(d, run, tune, pl, u8 ? nullptr : d_tuples, n);
-    wp.bottom = u8 ? d.d_bottom_b : d.d_bottom;
-    wp.top4 = u8 ? d.d_top_b : nullptr;
+    wp.bottom = u8 ? d.layout.bottom_b : d.layout.bottom;
+    wp.top4 = u8 ? d.layout.top_b.get() : nullptr;
     wp.bins = u8 ? static_cast<const uint8_t*>(d_tuples) : nullptr;
     wp.scores = d_scores;
     wp.labels = d_labels;
@@ -858,7 +947,7 @@ inline cudaError_t launch_leaf_walk(Dev& d, const Geom& run, const Tune& tune, i
     const Plan pl = make_plan(d, tune, want_variant, Walk::Leaf);
     LeafParams lp = {};
     lp.w = walk_params(d, run, tune, pl, d_tuples, n);
-    lp.w.bottom = d.d_bottom_id;
+    lp.w.bottom = d.layout.bottom_id;
     lp.w.groups = d.shape.Tpad / 8;
     lp.w.K = 1;
     lp.leaves = d_leaves;
@@ -897,7 +986,7 @@ struct ShapPlan {
 };
 inline ShapPlan shap_plan(const Dev& d, int want) {
     ShapPlan p;
-    const uint32_t M = d.shap.M;
+    const uint32_t M = d.layout.shap.M;
     p.bound = M <= 3 ? 3 : M <= 7 ? 7 : 15;
     const int G = shap_tile_groups(d);
     p.tile = want != KERNEL_GENERIC && G >= 1 && (want != KERNEL_AUTO || shap_tile_warps_per_sm(d) >= kShapTileMinWarps);
@@ -915,18 +1004,29 @@ inline ShapKernel shap_kernel(const ShapPlan& p) {
 }
 constexpr size_t kShapScratchBytes = 256ull << 20;   // dt_shap_generic accumulators: rows per launch = this / (8 (F + 1))
 
+// The ShapParams of a contribution or interaction walk on device d: the resident contribution layout and, for a
+// single-class run, the first min(T, 8 S K) trees of `run`, for a multi-class run every tree.  The launchers add the rest.
+inline ShapParams shap_params(const Dev& d, const Geom& run) {
+    const ResidentLayout& lay = d.layout;
+    ShapParams p = {};
+    p.nodes = lay.shap_nodes;
+    p.paths = lay.shap_paths;
+    p.tree_path = lay.shap_tree_path;
+    p.cls_tree = lay.shap_cls_tree;
+    p.F = d.shape.g.F(); p.C = d.shape.C; p.missing = run.missing;
+    p.n_nodes = lay.shap.n_nodes; p.stride = lay.shap.stride; p.zoff = lay.shap.zoff; p.izoff = lay.shap.izoff;
+    p.trees0 = d.shape.C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    return p;
+}
+
 // The device's fp64 scratch of dt_shap_generic and dt_shap_inter, at least `words` long, made ready for a walk on st: it
 // waits for the previous walk using it (on any stream).  Grown after a device synchronise; every placement frees it.
 inline cudaError_t shap_scratch(Dev& d, size_t words, cudaStream_t st) {
     cudaError_t rc;
-    if (!d.ev_shap && (rc = cudaEventCreateWithFlags(&d.ev_shap, cudaEventDisableTiming)) != cudaSuccess) return rc;
-    if (d.shap_scratch_words < words) {               // grow: no walk on any stream may still use the old scratch
+    if (!d.ev_shap && (rc = d.ev_shap.create()) != cudaSuccess) return rc;
+    if (d.d_shap_scratch.size() < words) {            // grow: no walk on any stream may still use the old scratch
         if ((rc = cudaDeviceSynchronize()) != cudaSuccess) return rc;
-        if (d.d_shap_scratch) cudaFree(d.d_shap_scratch);
-        d.d_shap_scratch = nullptr;
-        d.shap_scratch_words = 0;
-        if ((rc = cudaMalloc(&d.d_shap_scratch, words * 8)) != cudaSuccess) return rc;
-        d.shap_scratch_words = words;
+        if ((rc = d.d_shap_scratch.alloc(words)) != cudaSuccess) return rc;
     }
     return cudaStreamWaitEvent(st, d.ev_shap, 0);
 }
@@ -940,14 +1040,7 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     *why = nullptr;
     if (n == 0) return cudaSuccess;
     const uint32_t F = d.shape.g.F(), C = d.shape.C;
-    ShapParams p = {};
-    p.nodes = d.d_shap_nodes;
-    p.paths = d.d_shap_paths;
-    p.tree_path = d.d_shap_tree_path;
-    p.cls_tree = d.d_shap_cls_tree;
-    p.F = F; p.C = C; p.missing = run.missing;
-    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff; p.izoff = d.shap.izoff;
-    p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    ShapParams p = shap_params(d, run);
     const ShapPlan pl = shap_plan(d, want_variant);
     const ShapKernel k = shap_kernel(pl);
     const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
@@ -1009,7 +1102,7 @@ struct InterPlan {
 inline InterPlan inter_plan(const Dev& d, uint32_t forced_block, size_t n) {
     InterPlan p;
     const uint32_t F = d.shape.g.F();
-    p.bound = d.shap.M <= 3 ? 3 : d.shap.M <= 7 ? 7 : 15;
+    p.bound = d.layout.shap.M <= 3 ? 3 : d.layout.shap.M <= 7 ? 7 : 15;
     const size_t row_bytes = (size_t)8 * F;          // one matrix row of one tuple
     const size_t tuples = std::min((size_t)std::max(1, d.sm_count) * kInterRowsPerSM, (std::min<size_t>(n, 1ull << 40) + 31) & ~(size_t)31);
     const size_t B = forced_block ? forced_block : kInterScratchBytes / (row_bytes * std::max<size_t>(tuples, 32));
@@ -1031,13 +1124,7 @@ inline cudaError_t launch_inter(Dev& d, const Geom& run, uint32_t forced_block, 
     const uint32_t F = d.shape.g.F(), C = d.shape.C;
     InterParams ip = {};
     ShapParams& p = ip.s;
-    p.nodes = d.d_shap_nodes;
-    p.paths = d.d_shap_paths;
-    p.tree_path = d.d_shap_tree_path;
-    p.cls_tree = d.d_shap_cls_tree;
-    p.F = F; p.C = C; p.missing = run.missing;
-    p.n_nodes = d.shap.n_nodes; p.stride = d.shap.stride; p.zoff = d.shap.zoff; p.izoff = d.shap.izoff;
-    p.trees0 = C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    p = shap_params(d, run);
     const InterPlan pl = inter_plan(d, forced_block, n);
     const InterKernel k = inter_kernel(pl.bound);
     const size_t rows = std::min(pl.rows, (n + 31) & ~(size_t)31);

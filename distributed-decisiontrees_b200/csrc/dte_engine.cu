@@ -275,11 +275,11 @@ int decide_partition(dte_engine* e, const Geom& g) {
 // Why device d cannot run a walk of kind w: the layout that walk reads is not resident (nullptr: it is).
 const char* missing_layout(const Dev& d, Walk w) {
     switch (w) {
-        case Walk::Binned: return d.d_top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
-        case Walk::Leaf: return d.d_bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
+        case Walk::Binned: return d.layout.top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
+        case Walk::Leaf: return d.layout.bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
         case Walk::Contrib:
-        case Walk::Inter: return d.d_shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
-        default: return d.d_top ? nullptr : "no ensemble loaded";
+        case Walk::Inter: return d.layout.shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
+        default: return d.layout.top ? nullptr : "no ensemble loaded";
     }
 }
 
@@ -316,71 +316,51 @@ int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
 uint32_t classes_of(const dte_engine* e) { return host_dev(e).shape.C; }
 
 // ---- placement of the ensemble on the devices ---------------------------------------------------------
-void free_ensemble(Dev& d) {
-    cudaSetDevice(d.ordinal);
-    for (void* p : {(void*)d.d_top, (void*)d.d_top_split, (void*)d.d_bottom, (void*)d.d_top_b, (void*)d.d_bottom_b, (void*)d.d_bin_off, (void*)d.d_bin_edges,
-                    (void*)d.d_bottom_id, (void*)d.d_shap_nodes, (void*)d.d_shap_paths, (void*)d.d_shap_tree_path,
-                    (void*)d.d_shap_cls_tree, (void*)d.d_shap_scratch})
-        if (p) cudaFree(p);
-    d.d_bottom_id = nullptr;
-    d.d_shap_nodes = nullptr;
-    d.d_shap_paths = nullptr;
-    d.d_shap_tree_path = nullptr;
-    d.d_shap_cls_tree = nullptr;
-    d.d_shap_scratch = nullptr;                       // sized for the F of the ensemble it served
-    d.shap_scratch_words = 0;
-    d.shap = ShapLayout();
-    d.d_top = nullptr;
-    d.d_top_split = nullptr;
-    d.d_bottom = nullptr;
-    d.d_top_b = nullptr;
-    d.d_bottom_b = nullptr;
-    d.d_bin_off = d.d_bin_edges = nullptr;
-    d.shape.T = d.shape.Tpad = 0;    // the geometry stays: the landing slots of a run in progress are cut by it
-    d.ensemble_bytes = 0;
+// Drop device d's resident ensemble once nothing walks it, and the fp64 scratch sized for its F.  The geometry stays:
+// the landing slots of a run in progress are cut by it.
+cudaError_t free_ensemble(Dev& d) {
+    cudaError_t rc = cudaSetDevice(d.ordinal);
+    if (rc == cudaSuccess) rc = cudaDeviceSynchronize();
+    d.layout = ResidentLayout();
+    d.d_shap_scratch.reset();
+    d.shape.T = d.shape.Tpad = 0;
+    return rc;
 }
 
 template <class T>
-int upload(dte_engine* e, T*& dst, const std::vector<T>& src) {
-    CUDA_TRY(e, cudaMalloc(&dst, std::max<size_t>(1, src.size()) * sizeof(T)));
+int upload(dte_engine* e, DevArray<T>& dst, const std::vector<T>& src) {
+    CUDA_TRY(e, dst.alloc(src.size()));
     if (!src.empty()) CUDA_TRY(e, cudaMemcpy(dst, src.data(), src.size() * sizeof(T), cudaMemcpyHostToDevice));
     return DTE_OK;
 }
 
 // `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr.  `shap`: the contribution
-// layout of a dte_load_ensemble_contribs, else nullptr.
+// layout of a dte_load_ensemble_contribs, else nullptr.  The old ensemble is dropped before the new one is allocated.
 int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap) {
-    CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    CUDA_TRY(e, cudaDeviceSynchronize());           // nothing may still be walking the old ensemble
-    free_ensemble(d);
-    TRY(upload(e, d.d_top, pk.top));
-    TRY(upload(e, d.d_top_split, pk.top_split));
-    TRY(upload(e, d.d_bottom, pk.bottom));
+    CUDA_TRY(e, free_ensemble(d));
+    ResidentLayout& lay = d.layout;
+    TRY(upload(e, lay.top, pk.top));
+    TRY(upload(e, lay.top_split, pk.top_split));
+    TRY(upload(e, lay.bottom, pk.bottom));
     d.shape = pk.shape;
-    d.ensemble_bytes = pk.top.size() * sizeof(uint2) + pk.top_split.size() * sizeof(uint16_t) + pk.bottom.size() * sizeof(uint4);
     if (bins) {
-        TRY(upload(e, d.d_top_b, pk.top_b));
-        TRY(upload(e, d.d_bottom_b, pk.bottom_b));
-        TRY(upload(e, d.d_bin_off, bins->offsets));
-        TRY(upload(e, d.d_bin_edges, bins->edges));
-        d.ensemble_bytes += pk.top_b.size() * sizeof(uint32_t) + pk.bottom_b.size() * sizeof(uint4);
+        TRY(upload(e, lay.top_b, pk.top_b));
+        TRY(upload(e, lay.bottom_b, pk.bottom_b));
+        TRY(upload(e, lay.bin_off, bins->offsets));
+        TRY(upload(e, lay.bin_edges, bins->edges));
     }
-    if (!pk.bottom_id.empty()) {
-        TRY(upload(e, d.d_bottom_id, pk.bottom_id));
-        d.ensemble_bytes += pk.bottom_id.size() * sizeof(uint4);
-    }
+    if (!pk.bottom_id.empty()) TRY(upload(e, lay.bottom_id, pk.bottom_id));
     if (shap) {
         double tab[4][kShapTab][kShapTab];
         shap_tables(tab);
         CUDA_TRY(e, cudaMemcpyToSymbol(c_shap_tab, tab, sizeof tab));
-        TRY(upload(e, d.d_shap_nodes, shap->nodes));
-        TRY(upload(e, d.d_shap_paths, shap->paths));
-        TRY(upload(e, d.d_shap_tree_path, shap->tree_path));
-        TRY(upload(e, d.d_shap_cls_tree, shap->cls_tree));
-        d.ensemble_bytes += shap->bytes();
-        d.shap.D = shap->D; d.shap.M = shap->M; d.shap.stride = shap->stride; d.shap.zoff = shap->zoff;
-        d.shap.izoff = shap->izoff;
-        d.shap.n_nodes = shap->n_nodes; d.shap.C = shap->C;
+        TRY(upload(e, lay.shap_nodes, shap->nodes));
+        TRY(upload(e, lay.shap_paths, shap->paths));
+        TRY(upload(e, lay.shap_tree_path, shap->tree_path));
+        TRY(upload(e, lay.shap_cls_tree, shap->cls_tree));
+        lay.shap.D = shap->D; lay.shap.M = shap->M; lay.shap.stride = shap->stride; lay.shap.zoff = shap->zoff;
+        lay.shap.izoff = shap->izoff;
+        lay.shap.n_nodes = shap->n_nodes; lay.shap.C = shap->C;
     }
     return DTE_OK;
 }
@@ -398,28 +378,33 @@ struct TreeShare {
 // start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
 // binned layout is dropped.  With DTE_OPT_LEAF_LAYOUT the leaf-id layout is built and uploaded too; without it any
 // resident leaf-id layout is dropped.  `covers` (fp32 [T_all][2^(D+1)-1] for the trees of the streams): also build and
-// upload the contribution layout of every share, all of them built and checked before anything is uploaded; without it
-// any resident contribution layout is dropped.
+// upload the contribution layout of every share; without it any resident contribution layout is dropped.
+// All or nothing: every share is built and checked before any device changes, so a refused share leaves the previous
+// ensemble resident everywhere; a failed upload leaves no ensemble on any device rather than a mix of two.
 int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr,
                    const float* covers = nullptr) {
     const bool chunked = e->part == Part::Chunked;
-    std::vector<ShapLayout> shap(covers ? (chunked ? e->devs.size() : 1) : 0);
-    for (size_t r = 0; r < shap.size(); ++r) {
+    const size_t n_shares = chunked ? e->devs.size() : 1;
+    std::vector<ShapLayout> shap(covers ? n_shares : 0);
+    std::vector<PackedEnsemble> pk(n_shares);
+    for (size_t r = 0; r < n_shares; ++r) {
         const TreeShare& s = share[r];
         std::string msg;
-        const int rc = build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
-                                         classes, shap[r], msg);
+        int rc = covers ? build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
+                                            classes, shap[r], msg) : 0;
+        if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk[r], msg, bins, e->opt_leaf);
         if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
     }
-    PackedEnsemble pk;
     for (size_t r = 0; r < e->devs.size(); ++r) {
-        if (chunked || r == 0) {
-            const TreeShare& s = share[r];
-            std::string msg;
-            const int rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk, msg, bins, e->opt_leaf);
-            if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
+        const size_t s = chunked ? r : 0;
+        const int rc = upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk[s], bins, covers ? &shap[s] : nullptr);
+        if (rc) {
+            for (Dev& d : e->devs) free_ensemble(d);
+            e->placed.reset();
+            e->bins = BinEdges();
+            e->measured.reset();
+            return rc;
         }
-        TRY(upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk, bins, covers ? &shap[chunked ? r : 0] : nullptr));
     }
     e->bins = bins ? *bins : BinEdges();
     e->measured.reset();              // a plan measured on the previous ensemble says nothing about this one
@@ -445,81 +430,55 @@ int program_devices(dte_engine* e, const Geom& g) {
 }
 
 // ---- landing slots ------------------------------------------------------------------------------
-void free_sparse_slots(Dev& d) {
-    for (Slot& s : d.slot) {
-        for (void* p : {(void*)s.d_sp_ptr, (void*)s.d_sp_idx, (void*)s.d_sp_val})
-            if (p) cudaFree(p);
-        s.d_sp_ptr = nullptr; s.d_sp_idx = nullptr; s.d_sp_val = nullptr;
-    }
-    d.sparse_slot_nnz = 0;
-}
-
-void free_slots(Dev& d) {
-    cudaSetDevice(d.ordinal);
-    free_sparse_slots(d);
-    for (Slot& s : d.slot) {
-        if (s.d_tup) cudaFree(s.d_tup);
-        if (s.d_sc) cudaFree(s.d_sc);
-        if (s.d_part) cudaFree(s.d_part);
-        if (s.d_lb) cudaFree(s.d_lb);
-        if (s.d_rows) cudaFree(s.d_rows);
-        s.d_tup = nullptr; s.d_sc = nullptr; s.d_part = nullptr; s.d_lb = nullptr; s.d_rows = nullptr;
-        s.fill = s.walked = 0;
-    }
-    d.cap_tuples = 0;
-    d.slot_parts = false;
-    d.slot_row_bytes = 0;
-}
-
 // leaf and contribution calls: Slot::d_rows of [cap] rows of walk w on every slot (score runs never allocate them)
 int ensure_row_slots(dte_engine* e, Dev& d, Walk w) {
     const size_t bytes = d.cap_tuples * row_bytes(d, w);
-    if (d.slot_row_bytes >= bytes) return DTE_OK;
+    bool fits = true;
+    for (const Slot& s : d.slot) fits = fits && s.d_rows.size() >= bytes;
+    if (fits) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());
-    for (Slot& s : d.slot) {
-        if (s.d_rows) cudaFree(s.d_rows);
-        s.d_rows = nullptr;
-    }
-    d.slot_row_bytes = 0;
-    for (Slot& s : d.slot) CUDA_TRY(e, cudaMalloc(&s.d_rows, bytes));
-    d.slot_row_bytes = bytes;
+    for (Slot& s : d.slot) s.d_rows.reset();
+    for (Slot& s : d.slot) CUDA_TRY(e, s.d_rows.alloc(bytes));
     return DTE_OK;
 }
 
 // sparse host calls: every slot holds the indptr slice of a whole chunk and `nnz` entries (score-only runs never
-// allocate them); free_slots drops them with the slots they were sized for
+// allocate them); ensure_slots drops them with the slots they were sized for
 int ensure_sparse_slots(dte_engine* e, Dev& d, size_t nnz) {
     nnz = std::max<size_t>(nnz, 1);
-    if (d.slot[0].d_sp_ptr && d.sparse_slot_nnz >= nnz) return DTE_OK;
+    bool fits = true;
+    for (const Slot& s : d.slot) fits = fits && s.d_sp_val.size() >= nnz;      // d_sp_val is allocated last
+    if (fits) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());
-    free_sparse_slots(d);
+    for (Slot& s : d.slot) { s.d_sp_ptr.reset(); s.d_sp_idx.reset(); s.d_sp_val.reset(); }
     for (Slot& s : d.slot) {
-        CUDA_TRY(e, cudaMalloc(&s.d_sp_ptr, (d.cap_tuples + 1) * sizeof(long long)));
-        CUDA_TRY(e, cudaMalloc(&s.d_sp_idx, nnz * 4));
-        CUDA_TRY(e, cudaMalloc(&s.d_sp_val, nnz * 4));
+        CUDA_TRY(e, s.d_sp_ptr.alloc(d.cap_tuples + 1));
+        CUDA_TRY(e, s.d_sp_idx.alloc(nnz));
+        CUDA_TRY(e, s.d_sp_val.alloc(nnz));
     }
-    d.sparse_slot_nnz = nnz;
     return DTE_OK;
 }
 
-// `C` score words per tuple: d_sc / d_part hold [cap][C] fp32 (C >= 2 for a multi-class ensemble)
+// `C` score words per tuple: d_sc / d_part hold [cap][C] fp32 (C >= 2 for a multi-class ensemble).  A new cut replaces
+// every slot, its buffers and events, after the old ones are released.
 int ensure_slots(dte_engine* e, Dev& d, size_t cap, uint32_t F, bool parts, uint32_t C) {
-    if (d.cap_tuples == cap && d.slot_F == F && d.slot_C == C && (d.slot_parts || !parts)) return DTE_OK;
+    if (d.cap_tuples == cap && d.slot_F == F && d.slot_C == C && (d.slot[0].d_part || !parts)) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());
-    free_slots(d);
+    d.cap_tuples = 0;
+    for (Slot& s : d.slot) s = Slot();
     for (Slot& s : d.slot) {
-        CUDA_TRY(e, cudaMalloc(&s.d_tup, cap * F * 4));
-        CUDA_TRY(e, cudaMalloc(&s.d_sc, cap * C * 4));
-        CUDA_TRY(e, cudaMalloc(&s.d_lb, cap));
-        if (parts) CUDA_TRY(e, cudaMalloc(&s.d_part, cap * C * 4));
+        CUDA_TRY(e, s.d_tup.alloc(cap * F * 4));
+        CUDA_TRY(e, s.d_sc.alloc(cap * C));
+        CUDA_TRY(e, s.d_lb.alloc(cap));
+        if (parts) CUDA_TRY(e, s.d_part.alloc(cap * C));
+        for (Event* ev : {&s.ev_walk, &s.ev_d2h, &s.ev_land, &s.ev_comb}) CUDA_TRY(e, ev->create());
     }
     d.cap_tuples = cap;
     d.slot_F = F;
     d.slot_C = C;
-    d.slot_parts = parts;
     d.cur = 0;
     return DTE_OK;
 }
@@ -533,22 +492,20 @@ size_t default_chunk(const dte_engine* e, uint32_t F) {
 }
 
 int ensure_ring(dte_engine* e, Dev& d, size_t cap_tuples) {
-    if (d.ring_cap >= cap_tuples) return DTE_OK;
+    if (d.h_ring.size() >= cap_tuples) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    if (d.h_ring) { cudaFreeHost(d.h_ring); d.h_ring = nullptr; d.ring_cap = 0; }
-    CUDA_TRY(e, cudaHostAlloc(reinterpret_cast<void**>(&d.h_ring), cap_tuples * 4, cudaHostAllocPortable));
-    d.ring_cap = cap_tuples;
+    CUDA_TRY(e, d.h_ring.alloc(cap_tuples, cudaHostAllocPortable));
     return DTE_OK;
 }
 
-cudaEvent_t get_event(Dev& d) {
-    if (!d.ev_pool.empty()) {
-        cudaEvent_t ev = d.ev_pool.back();
+Event get_event(Dev& d) {
+    Event ev;
+    if (d.ev_pool.empty()) {
+        ev.create();
+    } else {
+        ev = std::move(d.ev_pool.back());
         d.ev_pool.pop_back();
-        return ev;
     }
-    cudaEvent_t ev = nullptr;
-    cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
     return ev;
 }
 
@@ -561,7 +518,7 @@ int poll_dev(dte_engine* e, Dev& d, uint64_t need) {
         if (st == cudaErrorNotReady) break;
         if (st != cudaSuccess) return fail(e, DTE_ERR_CUDA, "result copy failed: %s", cudaGetErrorString(st));
         d.res_done = p.upto;
-        d.ev_pool.push_back(p.ev);
+        d.ev_pool.push_back(std::move(p.ev));
         d.pend.pop_front();
     }
     return DTE_OK;
@@ -569,7 +526,7 @@ int poll_dev(dte_engine* e, Dev& d, uint64_t need) {
 
 // The result rows of slot s for the device's walk: d_rows, or the final scores d_sc
 unsigned char* slot_rows(const Dev& d, const Slot& s) {
-    return row_walk(d.walk) ? s.d_rows : reinterpret_cast<unsigned char*>(s.d_sc);
+    return row_walk(d.walk) ? s.d_rows.get() : reinterpret_cast<unsigned char*>(s.d_sc.get());
 }
 
 // D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink: rows of row_bytes,
@@ -590,18 +547,18 @@ int enqueue_results(dte_engine* e, Dev& d, Slot& s, size_t from, size_t cnt, boo
             d.sink_lb += cnt;
         }
     } else {
-        size_t pos = (size_t)(d.res_enq % d.ring_cap), left = cnt, off = from;
+        size_t pos = (size_t)(d.res_enq % d.h_ring.size()), left = cnt, off = from;
         while (left) {                               // the ring may wrap
-            const size_t run = std::min(left, d.ring_cap - pos);
+            const size_t run = std::min(left, d.h_ring.size() - pos);
             CUDA_TRY(e, cudaMemcpyAsync(d.h_ring + pos, s.d_sc + off, run * 4, cudaMemcpyDeviceToHost, d.s_d2h));
             left -= run; off += run; pos = 0;
         }
     }
     CUDA_TRY(e, cudaEventRecord(s.ev_d2h, d.s_d2h));
-    cudaEvent_t ev = get_event(d);
+    Event ev = get_event(d);
     CUDA_TRY(e, cudaEventRecord(ev, d.s_d2h));
     d.res_enq += cnt;
-    d.pend.push_back({ev, d.res_enq});
+    d.pend.push_back({std::move(ev), d.res_enq});
     return DTE_OK;
 }
 
@@ -685,8 +642,8 @@ int h2d_piece(dte_engine* e, Dev& d, unsigned char* dst, const unsigned char* sr
     }
     if (!d.h_stage[0]) {
         for (int b = 0; b < 3; ++b) {
-            CUDA_TRY(e, cudaHostAlloc(reinterpret_cast<void**>(&d.h_stage[b]), kStageBytes, cudaHostAllocDefault));
-            CUDA_TRY(e, cudaEventCreateWithFlags(&d.ev_stage[b], cudaEventDisableTiming));
+            CUDA_TRY(e, d.h_stage[b].alloc(kStageBytes, cudaHostAllocDefault));
+            CUDA_TRY(e, d.ev_stage[b].create());
         }
     }
     for (size_t off = 0; off < bytes; off += kStageBytes) {
@@ -755,12 +712,12 @@ cudaError_t launch_sparse_rows(const Dev& d, const long long* indptr, const uint
 int upload_sparse(dte_engine* e, Dev& d, Slot& s, const SparseRows& sp, size_t row0, size_t cnt) {
     const long long k0 = sp.indptr[row0];
     const size_t nnz = (size_t)(sp.indptr[row0 + cnt] - k0);
-    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_ptr), reinterpret_cast<const unsigned char*>(sp.indptr + row0),
+    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_ptr.get()), reinterpret_cast<const unsigned char*>(sp.indptr + row0),
                   (cnt + 1) * sizeof(long long), sp.pageable[0]));
     if (!nnz) return DTE_OK;
-    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_idx), reinterpret_cast<const unsigned char*>(sp.indices + k0),
+    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_idx.get()), reinterpret_cast<const unsigned char*>(sp.indices + k0),
                   nnz * 4, sp.pageable[1]));
-    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_val), reinterpret_cast<const unsigned char*>(sp.values + k0),
+    TRY(h2d_piece(e, d, reinterpret_cast<unsigned char*>(s.d_sp_val.get()), reinterpret_cast<const unsigned char*>(sp.values + k0),
                   nnz * 4, sp.pageable[2]));
     return DTE_OK;
 }
@@ -1229,46 +1186,9 @@ int init_dev(Dev& d, int ordinal) {
     bool ok = cudaSetDevice(ordinal) == cudaSuccess &&
               cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, ordinal) == cudaSuccess &&
               cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ordinal) == cudaSuccess &&
-              cudaStreamCreateWithFlags(&d.s_main, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaStreamCreateWithFlags(&d.s_h2d, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaStreamCreateWithFlags(&d.s_d2h, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaEventCreate(&d.ev_t0) == cudaSuccess && cudaEventCreate(&d.ev_t1) == cudaSuccess;
-    for (Slot& s : d.slot)
-        ok = ok && cudaEventCreateWithFlags(&s.ev_walk, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&s.ev_d2h, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&s.ev_land, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&s.ev_comb, cudaEventDisableTiming) == cudaSuccess;
+              d.s_main.create() == cudaSuccess && d.s_h2d.create() == cudaSuccess && d.s_d2h.create() == cudaSuccess &&
+              d.ev_t0.create(cudaEventDefault) == cudaSuccess && d.ev_t1.create(cudaEventDefault) == cudaSuccess;
     return ok ? DTE_OK : DTE_ERR_CUDA;
-}
-
-void destroy_dev(Dev& d) {
-    if (cudaSetDevice(d.ordinal) != cudaSuccess) return;
-    cudaDeviceSynchronize();
-    free_ensemble(d);
-    free_slots(d);
-    if (d.ev_shap) cudaEventDestroy(d.ev_shap);
-    for (int j = 0; j < 2; ++j) {
-        if (d.d_dense[j]) cudaFree(d.d_dense[j]);
-        if (d.ev_dense[j]) cudaEventDestroy(d.ev_dense[j]);
-    }
-    if (d.h_ring) cudaFreeHost(d.h_ring);
-    for (int b = 0; b < 3; ++b) {
-        if (d.h_stage[b]) cudaFreeHost(d.h_stage[b]);
-        if (d.ev_stage[b]) cudaEventDestroy(d.ev_stage[b]);
-    }
-    for (Slot& s : d.slot) {
-        if (s.ev_walk) cudaEventDestroy(s.ev_walk);
-        if (s.ev_d2h) cudaEventDestroy(s.ev_d2h);
-        if (s.ev_land) cudaEventDestroy(s.ev_land);
-        if (s.ev_comb) cudaEventDestroy(s.ev_comb);
-    }
-    for (Pending& p : d.pend) cudaEventDestroy(p.ev);
-    for (cudaEvent_t ev : d.ev_pool) cudaEventDestroy(ev);
-    if (d.ev_t0) cudaEventDestroy(d.ev_t0);
-    if (d.ev_t1) cudaEventDestroy(d.ev_t1);
-    if (d.s_main) cudaStreamDestroy(d.s_main);
-    if (d.s_h2d) cudaStreamDestroy(d.s_h2d);
-    if (d.s_d2h) cudaStreamDestroy(d.s_d2h);
 }
 
 uint64_t cycles_of(const dte_engine* e, double ns) {
@@ -1462,7 +1382,6 @@ int dte_create_multi(dte_t** engine, const int* gpu_ordinals, int n_gpus) {
             }
     }
     if (rc) {
-        for (Dev& d : e->devs) destroy_dev(d);
         delete e;
         return rc;
     }
@@ -1481,8 +1400,7 @@ int dte_destroy(dte_t* e) {
     if (!e->nccl_comms.empty() && e->nccl.CommDestroy)
         for (void* c : e->nccl_comms)
             if (c) e->nccl.CommDestroy(c);
-    for (Dev& d : e->devs) destroy_dev(d);
-    delete e;
+    delete e;                                             // every device releases its buffers, events and streams
     return DTE_OK;
 }
 
@@ -1648,8 +1566,8 @@ int dte_stream_read_packets(dte_t* e, void* cl128, uint8_t* last_flags, size_t m
             const uint64_t bt = dealing(e).bt;
             run = std::min(run, bt - i % bt);
         }
-        const size_t pos = (size_t)(loc % d.ring_cap);
-        run = std::min<uint64_t>(run, d.ring_cap - pos);
+        const size_t pos = (size_t)(loc % d.h_ring.size());
+        run = std::min<uint64_t>(run, d.h_ring.size() - pos);
         memcpy(out + (i - e->res_read), d.h_ring + pos, (size_t)run * 4);
         if (&d != &host_dev(e)) e->sl3_res_lines += (run + 3) / 4;
         i += run;
@@ -1735,20 +1653,20 @@ static int time_plans(dte_t* e, Dev& d, const Tune& base, size_t n, std::vector<
     n = std::max(n, 2 * wave_max);
     const uint32_t F = d.shape.g.F();
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
-    void* d_x = nullptr;
-    float* d_s = nullptr;
-    cudaEvent_t ev[2] = {nullptr, nullptr};
+    DevArray<uint32_t> d_x;
+    DevArray<float> d_s;
+    Event ev[2];
     std::vector<float> ms(out.size() * kPlanReps);
     int rc = DTE_OK;
-    if (cudaMalloc(&d_x, n * F * 4) != cudaSuccess || cudaMalloc(&d_s, n * d.shape.C * 4) != cudaSuccess) {
+    if (d_x.alloc(n * F) != cudaSuccess || d_s.alloc(n * d.shape.C) != cudaSuccess) {
         cudaGetLastError();                              // not sticky: the next launch's check must not see it
         rc = fail(e, DTE_ERR_NOMEM, "timing the launch plans: out of device memory for %zu tuples", n);
     }
-    else if (cudaEventCreate(&ev[0]) != cudaSuccess || cudaEventCreate(&ev[1]) != cudaSuccess)
+    else if (ev[0].create(cudaEventDefault) != cudaSuccess || ev[1].create(cudaEventDefault) != cudaSuccess)
         rc = fail(e, DTE_ERR_CUDA, "timing the launch plans: cudaEventCreate failed");
     if (!rc)
-        synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(static_cast<uint32_t*>(d_x), 0, (unsigned long long)n * F,
-                                                                             0x7091E5ull, 10000u, e->g.missing);
+        synth_tuples_kernel<<<(unsigned)d.sm_count * 8, 256, 0, d.s_main>>>(d_x, 0, (unsigned long long)n * F, 0x7091E5ull, 10000u,
+                                                                             e->g.missing);
     for (int round = -1; round < kPlanReps && !rc; ++round)
         for (size_t i = 0; i < out.size() && !rc; ++i) {
             const char* why = nullptr;
@@ -1767,10 +1685,6 @@ static int time_plans(dte_t* e, Dev& d, const Tune& base, size_t n, std::vector<
         std::sort(m, m + kPlanReps);
         out[i].tuples_per_ms = (double)(n / waves[i] * waves[i]) / m[kPlanReps / 2];
     }
-    for (cudaEvent_t x : ev)
-        if (x) cudaEventDestroy(x);
-    cudaFree(d_x);
-    cudaFree(d_s);
     return rc;
 }
 
@@ -1927,15 +1841,13 @@ int dte_ipc_alloc(dte_t* e, size_t bytes, void** d_ptr, unsigned char handle_out
     if (!e || !d_ptr || !handle_out || !bytes) return DTE_ERR_ARG;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "handle size");
     CUDA_TRY(e, cudaSetDevice(e->devs[0].ordinal));
-    CUDA_TRY(e, cudaMalloc(d_ptr, bytes));
+    DevArray<unsigned char> buf;
+    CUDA_TRY(e, buf.alloc(bytes));
     cudaIpcMemHandle_t h;
-    cudaError_t st = cudaIpcGetMemHandle(&h, *d_ptr);
-    if (st != cudaSuccess) {
-        cudaFree(*d_ptr);
-        *d_ptr = nullptr;
-        return fail(e, DTE_ERR_CUDA, "cudaIpcGetMemHandle failed: %s", cudaGetErrorString(st));
-    }
+    cudaError_t st = cudaIpcGetMemHandle(&h, buf);
+    if (st != cudaSuccess) return fail(e, DTE_ERR_CUDA, "cudaIpcGetMemHandle failed: %s", cudaGetErrorString(st));
     memcpy(handle_out, &h, 64);
+    *d_ptr = buf.release();                         // the caller frees it with dte_ipc_close(owner = 1)
     return DTE_OK;
 }
 
@@ -1988,7 +1900,7 @@ int dte_bin_tuples_device(dte_t* e, const void* d_tuples, size_t n, uint8_t* d_b
     const unsigned long long nq = (unsigned long long)n * g.F() / 4;
     const unsigned blocks = (unsigned)std::min<unsigned long long>((nq + 255) / 256, (unsigned long long)d.sm_count * 16);
     bin_tuples_kernel<<<blocks, 256, 0, st>>>(static_cast<const uint4*>(d_tuples), reinterpret_cast<uint32_t*>(d_bins), nq,
-                                              g.F(), d.d_bin_off, d.d_bin_edges, g.missing);
+                                              g.F(), d.layout.bin_off.get(), d.layout.bin_edges.get(), g.missing);
     CUDA_TRY(e, cudaGetLastError());
     if (!cuda_stream) CUDA_TRY(e, cudaStreamSynchronize(st));
     return DTE_OK;
@@ -2089,19 +2001,16 @@ int dte_sparse_to_dense_device(dte_t* e, const int64_t* d_indptr, const uint32_t
     return DTE_OK;
 }
 
-// Two engine-owned buffers of `bytes` for dte_infer_device_sparse; growing them waits for every walk that may read them.
-static int ensure_dense_scratch(dte_t* e, Dev& d, size_t bytes) {
-    if (d.dense_bytes >= bytes) return DTE_OK;
+// Two engine-owned buffers of `words` for dte_infer_device_sparse; growing them waits for every walk that may read them.
+static int ensure_dense_scratch(dte_t* e, Dev& d, size_t words) {
+    if (d.d_dense[0].size() >= words && d.d_dense[1].size() >= words) return DTE_OK;
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     CUDA_TRY(e, cudaDeviceSynchronize());
-    d.dense_bytes = 0;
     for (int j = 0; j < 2; ++j) {
-        if (d.d_dense[j]) cudaFree(d.d_dense[j]);
-        d.d_dense[j] = nullptr;
-        if (!d.ev_dense[j]) CUDA_TRY(e, cudaEventCreateWithFlags(&d.ev_dense[j], cudaEventDisableTiming));
+        d.d_dense[j].reset();
+        if (!d.ev_dense[j]) CUDA_TRY(e, d.ev_dense[j].create());
     }
-    for (int j = 0; j < 2; ++j) CUDA_TRY(e, cudaMalloc(&d.d_dense[j], bytes));
-    d.dense_bytes = bytes;
+    for (int j = 0; j < 2; ++j) CUDA_TRY(e, d.d_dense[j].alloc(words));
     return DTE_OK;
 }
 
@@ -2127,7 +2036,7 @@ int dte_infer_device_sparse(dte_t* e, const int64_t* d_indptr, const uint32_t* d
     size_t rows = default_chunk(e, F);
     if (rows > wave) rows -= rows % wave;
     rows = std::min(n, rows);
-    TRY(ensure_dense_scratch(e, d, rows * F * 4));
+    TRY(ensure_dense_scratch(e, d, rows * F));
     CUDA_TRY(e, cudaSetDevice(d.ordinal));
     cudaStream_t st = pick_stream(d, cuda_stream);
     const long long* indptr = reinterpret_cast<const long long*>(d_indptr);
@@ -2275,13 +2184,14 @@ int dte_get_info(dte_t* e, dte_info* info) {
         d0.timing_pending = false;
     }
     memset(info, 0, sizeof *info);
-    info->num_levels = d0.d_top ? d0.shape.g.D : e->g.D;
-    info->num_features = d0.d_top ? d0.shape.g.F() : e->g.F();
+    const bool loaded = d0.layout.top;
+    info->num_levels = loaded ? d0.shape.g.D : e->g.D;
+    info->num_features = loaded ? d0.shape.g.F() : e->g.F();
     info->clusters = e->g.K;
     info->trees_per_pu = e->g.S;
     info->sm_count = (uint32_t)d0.sm_count;
     for (Dev& d : e->devs) {
-        info->ensemble_bytes += d.ensemble_bytes;
+        info->ensemble_bytes += d.layout.bytes();
         info->kernel_launches += d.kernel_launches;
         if (e->part == Part::Chunked) info->num_trees += d.shape.T;
     }
@@ -2291,8 +2201,8 @@ int dte_get_info(dte_t* e, dte_info* info) {
     info->partition = info_partition(e->part);
     info->tuples_in = e->tuples_in;
     info->tuples_out = e->tuples_out;
-    info->num_classes = d0.d_top ? d0.shape.C : 0;
-    if (d0.d_top) {
+    info->num_classes = loaded ? d0.shape.C : 0;
+    if (loaded) {
         const Plan pl = make_plan(d0, walk_tune(e, Walk::Fp32), e->forced_variant);
         info->kernel_variant = (uint32_t)pl.variant();
         info->tuples_per_cta = pl.tuples_per_cta();
@@ -2306,7 +2216,7 @@ int dte_kernel_name(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, 
 int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     if (!e) return DTE_ERR_ARG;
     Dev& d = e->devs[0];
-    if (!d.d_top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
+    if (!d.layout.top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
     Geom g;
     TRY(decode_geom(e, g));
     TRY(check_resident(e, g));

@@ -153,6 +153,41 @@ def test_multi_fast_paths_load_and_infer_host(devs):
             assert ei.value.code == -4
 
 
+def test_refused_ensemble_leaves_every_chunk_resident():
+    """A new ensemble whose last tree chunk reads a feature index >= F is refused before any device changes, through
+    dte_load_ensemble and through the line stream: every ring position keeps the previous ensemble's chunk, and the
+    ring combine still returns that ensemble's words, never a mix of the two."""
+    devs = [0, 0, 0]
+    G = len(devs)
+    T, D, F, K, n = 24 * G, 5, 32, 2, 1811
+    W, FI, x, wl, fl, _ = _case(T, D, F, n, 91)
+    want, _ = _ensemble_reference(W, FI, x, D, K, G)
+    W_b, FI_b, _, _, _, _ = _case(T, D, F, n, 93)        # B: the same geometry, other trees...
+    FI_b[T - 1, 0] = (int(FI_b[T - 1, 0]) & ~0x7FF) | F   # ...and the root of its last tree reads feature F
+    wl_b, fl_b = L.pack_streams(W_b, FI_b, D)
+    trees_b = np.concatenate([wl_b.view(np.uint8).reshape(-1, 16), fl_b.view(np.uint8).reshape(-1, 16)])
+    with ddt.Engine(devs) as e:
+        _write_regs(e, multi_node_regs(T, D, F, K, n, G, "ensemble"))
+        e.load_ensemble(wl, fl)
+        resident = e.info()["ensemble_bytes"]
+
+        def check_a():
+            sc, lb = e.infer_host(x)
+            assert (sc.view(np.uint32) == want).all() and (lb == O.labels(want)).all()
+            assert e.info()["ensemble_bytes"] == resident
+
+        check_a()
+        with pytest.raises(E.DteError) as ei:
+            e.load_ensemble(wl_b, fl_b)
+        assert ei.value.code == -4
+        check_a()
+        e.start()
+        with pytest.raises(E.DteError) as ei:
+            e.stream_write(trees_b)
+        assert ei.value.code == -4
+        check_a()
+
+
 def _dealt_tuples(n, bt, G, pos):
     """Tuples ring position `pos` keeps when n tuples are dealt in batches of bt tuples over G positions, round-robin
     from position 0 (PCIeReceiver.sv:298-307): full batches first, then the short last batch (if any)."""

@@ -6,6 +6,7 @@
 #                                                        with split tree tops, DTE_TUNE tops=6), a 3-class
 #                                                        ensemble, seven kernel-matrix instantiations, the binned and
 #                                                        the leaf walks, memcheck over the sparse densify kernel,
+#                                                        leak checks of the C++ host on a three-position ring,
 #                                                        racecheck
 #                                                        once (AUTO)
 # racecheck does not model the mbarrier / cp.async.bulk (async-proxy) hand-off: tools/racecheck_canonical.cu is the
@@ -75,6 +76,15 @@ for T in tests/test_gpu_interactions.py::test_row_blocks_give_the_same_bytes tes
          "tests/test_gpu_interactions.py::test_tuple_counts[33]" "tests/test_gpu_interactions.py::test_deep_leafwise[free-15-15-15]"; do
   itag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_inter_${itag}.log"
+done
+# leaks: the C++ host (no torch caching allocator in the process) over a handle's whole life, create to destroy, on three
+# ring positions sharing one GPU, data- and ensemble-sharded, fed by the line stream and by the host fast path
+for mode in stream host; do
+  for part in data ensemble; do
+    log=$OUT/sanitizer_memcheck_leaks_${mode}_${part}.log
+    timeout 900 compute-sanitizer --tool memcheck --leak-check full --error-exitcode 7 tools/dte_host 48 6 256 6000 4 $mode 0,0,0 $part > "$log" 2>&1
+    echo "memcheck leaks [$mode $part] rc=$? $(grep -E 'ERROR SUMMARY|LEAK SUMMARY|leaked' "$log" | tr '\n' ' ' | cut -c1-300)"
+  done
 done
 T=tests/test_gpu_parity.py::test_shipped_plan_headline_geometry_multi_tile
 timeout 300 compute-sanitizer --tool racecheck --racecheck-report all --print-limit 8 --show-backtrace no tools/racecheck_canonical > $OUT/sanitizer_racecheck_canonical.log 2>&1
