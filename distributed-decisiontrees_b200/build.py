@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "dte_engine.cu")
 DEPS = [SRC, os.path.join(HERE, "csrc", "dte_kernels.cuh"), os.path.join(HERE, "csrc", "dte_device.cuh"),
         os.path.join(HERE, "..", "include", "dte.h"), os.path.join(HERE, "csrc", "dte_partition.hpp"),
-        os.path.join(HERE, "csrc", "dte_shap.cuh")]
+        os.path.join(HERE, "csrc", "dte_shap.cuh"), os.path.join(HERE, "csrc", "dte_approx.cuh")]
 OUT = os.path.join(HERE, "libdte.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
@@ -93,7 +93,7 @@ def build_host_check(name, force=False):
     """Compile tools/<name>.cu, a host-only checker over the engine headers (runs without a GPU); CPU test tier."""
     src = os.path.join(HERE, "..", "tools", name + ".cu")
     out = os.path.join(HERE, "..", "tools", name)
-    deps = [src] + DEPS[1:3]
+    deps = [src] + DEPS[1:3] + DEPS[5:]
     if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(d) for d in deps):
         return out
     nvcc = nvcc_path()

@@ -5,6 +5,7 @@
 #pragma once
 #include "dte_kernels.cuh"
 #include "dte_shap.cuh"
+#include "dte_approx.cuh"
 
 #include <algorithm>
 #include <array>
@@ -14,6 +15,7 @@
 #include <cmath>
 #include <cstring>
 #include <deque>
+#include <numeric>
 #include <string>
 #include <utility>
 #include <vector>
@@ -25,8 +27,9 @@ constexpr int kNumSlots = 3;          // landing slots per device: H2D of i+1, w
 enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED = 3 };
 
 // What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), the leaf cell every
-// tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12) or interaction values (DESIGN.md §13)
-enum class Walk { Fp32, Binned, Leaf, Contrib, Inter };
+// tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12), interaction values (DESIGN.md §13)
+// or the approximate feature contributions (DESIGN.md §14)
+enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx };
 
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536,tops=6"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
@@ -164,6 +167,18 @@ struct ShapLayout {
     size_t num_paths() const { return tree_path.empty() ? 0 : (size_t)tree_path.back(); }
 };
 
+// Whether stream tree `tree`'s cover of `cell` is refused (not finite or not > 0); msg then names the tree and cell.
+// Every live internal node and reachable end cell of a contribution or approximate-contribution load is checked.
+inline bool cover_refused(const float* cov, uint32_t tree, uint32_t cell, std::string& msg) {
+    const float c = cov[cell];
+    if (std::isfinite(c) && c > 0.0f) return false;
+    char buf[256];
+    snprintf(buf, sizeof buf, "covers: tree %u cell %u has cover %g: a live node or reachable leaf needs a finite cover > 0",
+             tree, cell, (double)c);
+    msg = buf;
+    return true;
+}
+
 // Builds the contribution layout of trees [first, first + count) of the streams (count = 0 with first = 0: all), class
 // of tree s = s % classes.  covers: fp32 [T_all][2^(D+1) - 1], indexed like the weight heap.  Only live internal nodes
 // and reachable end cells are read; each must be finite and > 0.  Returns 0, -1 (bad covers or streams; msg names the
@@ -208,14 +223,7 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
         const uint16_t* FI = Fall + (size_t)s * fstride;
         const float* cov = covers + (size_t)s * n_all;
         live_nodes(FI, D, live);
-        auto bad_cover = [&](uint32_t cell) {
-            const float c = cov[cell];
-            if (std::isfinite(c) && c > 0.0f) return false;
-            snprintf(buf, sizeof buf, "covers: tree %u cell %u has cover %g: a live node or reachable leaf needs a finite cover > 0",
-                     s, cell, (double)c);
-            msg = buf;
-            return true;
-        };
+        auto bad_cover = [&](uint32_t cell) { return cover_refused(cov, s, cell, msg); };
         cells.clear();
         for (uint32_t i = 0; i < n_int; ++i) {
             out.nodes[(size_t)k * n_int + i] = make_uint2(W[i], (FI[i] & 0x7FFu) | (uint32_t)((FI[i] >> 13) & 1u) << 16);
@@ -268,6 +276,82 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
             out.M = std::max(out.M, m);
         }
         out.tree_path.push_back(out.paths.size() / out.stride);
+    }
+    return 0;
+}
+
+// The approximate-contribution table (DESIGN.md §14), per local tree t in stream order (the leaf walk's columns):
+//   delta[t][2^(D+1)]  fp64: [0] = E[root], [c] = E[c] - E[parent(c)] for every non-root cell on a live path, 0 elsewhere
+//   feat[t][2^D]       u16: the feature index of internal node n (0 below an early leaf), so step n -> ch reads
+//                      delta[ch] and feat[(ch - 1) / 2]
+// E[c] = (double)W[t][c] for a reachable end cell, E[n] = (zl * E[l]) + (zr * E[r]) for a live internal node with
+// zl = (double)cov[l] / (double)cov[n] and zr the same for r, every operation rounded on its own.
+struct ApproxLayout {
+    uint32_t D = 0;
+    std::vector<double> delta;
+    std::vector<uint16_t> feat;
+    uint32_t cell_stride() const { return 2u << D; }
+    uint32_t node_stride() const { return 1u << D; }
+};
+
+// Builds the approximate-contribution table of trees [first, first + count) of the streams (count = 0 with first = 0:
+// all).  covers as for build_shap_layout, checked by the same rule.  Returns 0 or -1 (bad covers or streams; msg names
+// the tree and cell).
+inline int build_approx_layout(uint32_t D, uint32_t w_cls, uint32_t f_cls, const unsigned char* wl, size_t n_wl,
+                               const unsigned char* fl, size_t n_fl, const float* covers, uint32_t first, uint32_t count,
+                               ApproxLayout& out, std::string& msg) {
+    char buf[256];
+    if (n_wl % w_cls || n_fl != (n_wl / w_cls) * f_cls) { msg = "tree streams: line counts do not match the geometry"; return -1; }
+    const size_t T_all = n_wl / w_cls;
+    if (count == 0 && first == 0) count = (uint32_t)T_all;
+    if ((size_t)first + count > T_all || count == 0) {
+        snprintf(buf, sizeof buf, "tree chunk [%u, %u) outside the %zu trees of the stream", first, first + count, T_all);
+        msg = buf; return -1;
+    }
+    const uint32_t n_int = (1u << D) - 1, n_all = (2u << D) - 1;
+    const size_t wstride = (size_t)w_cls * 4, fstride = (size_t)f_cls * 8;
+    const uint32_t* Wall = reinterpret_cast<const uint32_t*>(wl);
+    const uint16_t* Fall = reinterpret_cast<const uint16_t*>(fl);
+    out = ApproxLayout();
+    out.D = D;
+    out.delta.assign((size_t)count * out.cell_stride(), 0.0);
+    out.feat.assign((size_t)count * out.node_stride(), 0);
+    std::vector<uint8_t> live, end(n_all);
+    std::vector<double> E(n_all);
+    for (uint32_t t = 0; t < count; ++t) {
+        const uint32_t s = first + t;
+        const uint32_t* W = Wall + (size_t)s * wstride;
+        const uint16_t* FI = Fall + (size_t)s * fstride;
+        const float* cov = covers + (size_t)s * n_all;
+        live_nodes(FI, D, live);
+        std::fill(end.begin(), end.end(), 0);
+        for (uint32_t i = 0; i < n_int; ++i) {
+            if (!live[i]) continue;
+            if (cover_refused(cov, s, i, msg)) return -1;
+            if ((FI[i] & 0x4000u) || 2 * i + 1 >= n_int) end[2 * i + 1] = end[2 * i + 2] = 1;
+        }
+        for (uint32_t c = 1; c < n_all; ++c) {
+            if (!end[c]) continue;
+            if (cover_refused(cov, s, c, msg)) return -1;
+            float v;
+            memcpy(&v, &W[c], 4);
+            E[c] = (double)v;
+        }
+        for (uint32_t i = n_int; i-- > 0;) {             // children before parents
+            if (!live[i]) continue;
+            const uint32_t l = 2 * i + 1, r = 2 * i + 2;
+            const double zl = (double)cov[l] / (double)cov[i], zr = (double)cov[r] / (double)cov[i];
+            E[i] = zl * E[l] + zr * E[r];
+        }
+        double* dt = out.delta.data() + (size_t)t * out.cell_stride();
+        uint16_t* ft = out.feat.data() + (size_t)t * out.node_stride();
+        dt[0] = E[0];
+        for (uint32_t i = 0; i < n_int; ++i) {
+            if (!live[i]) continue;
+            ft[i] = (uint16_t)(FI[i] & 0x7FFu);
+            dt[2 * i + 1] = E[2 * i + 1] - E[i];
+            dt[2 * i + 2] = E[2 * i + 2] - E[i];
+        }
     }
     return 0;
 }
@@ -598,10 +682,15 @@ struct ResidentLayout {
     DevArray<unsigned char> shap_paths;
     DevArray<unsigned long long> shap_tree_path;
     DevArray<uint32_t> shap_cls_tree;
+    // approximate-contribution table (dte_load_ensemble_approx_contribs only, DESIGN.md §14): an ApproxLayout's arrays
+    DevArray<double> approx_delta;
+    DevArray<uint16_t> approx_feat;
+    uint32_t approx_cell_stride = 0, approx_node_stride = 0;
     // dte_info.ensemble_bytes: every array but the edge table
     size_t bytes() const {
         return top.bytes() + top_split.bytes() + bottom.bytes() + top_b.bytes() + bottom_b.bytes() + bottom_id.bytes() +
-               shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes();
+               shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes() +
+               approx_delta.bytes() + approx_feat.bytes();
     }
 };
 
@@ -681,14 +770,14 @@ struct Dev {
     uint64_t tuples_landed = 0;       // whole tuples landed on this device since `start`
 };
 
-// Leaf, contribution and interaction walks write their rows into Slot::d_rows; score walks into d_sc / d_part, which the
-// combines, the labels and the line stream's ring read.
-inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib || w == Walk::Inter; }
+// Leaf, contribution, interaction and approximate-contribution walks write their rows into Slot::d_rows; score walks
+// into d_sc / d_part, which the combines, the labels and the line stream's ring read.
+inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib || w == Walk::Inter || w == Walk::Approx; }
 // Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes,
-// C (F + 1) contribution words or C (F + 1)^2 interaction words
+// C (F + 1) contribution words (exact or approximate) or C (F + 1)^2 interaction words
 inline size_t row_bytes(const Dev& d, Walk w) {
     if (w == Walk::Leaf) return 2 * (size_t)d.shape.T;
-    if (w == Walk::Contrib) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
+    if (w == Walk::Contrib || w == Walk::Approx) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
     if (w == Walk::Inter) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1) * (d.shape.g.F() + 1);
     return 4 * (size_t)d.slot_C;
 }
@@ -1179,6 +1268,80 @@ inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, siz
         const size_t used = strlen(buf);
         if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
     }
+}
+
+
+// ---- approximate feature contributions (DESIGN.md §14) ----
+// A call runs in chunks of `rows` tuples, each two kernels on the caller's stream: the leaf walk into a cell scratch
+// [rows][T] u16, then dt_approx_generic from those cells into the fp64 accumulators [C (F + 1)][rows].  Both live in the
+// device's fp64 scratch (shap_scratch's rules: guarded by ev_shap, grown after a device synchronise, freed by every
+// placement), at most kApproxScratchBytes of it.
+constexpr size_t kApproxScratchBytes = 1ull << 30;
+
+// Tuples per chunk: as many as kApproxScratchBytes holds, rounded down to whole waves of both passes where that leaves at
+// least one of each (a wave of pass 1 is sm_count tiles of its plan, or sm_count times the resident 128-thread blocks of
+// the generic leaf walk; a wave of pass 2 is sm_count times its resident 128-thread blocks), else to whole waves of pass
+// 2, else to whole warps.
+inline size_t approx_rows(const Dev& d, const Tune& tune, int want) {
+    const uint32_t F = d.shape.g.F(), C = d.shape.C, T = d.shape.T;
+    const size_t per = 2 * (size_t)T + 8 * (size_t)C * (F + 1);
+    const size_t cap = std::max<size_t>(32, (kApproxScratchBytes / per) & ~(size_t)31);
+    const size_t sm = (size_t)std::max(1, d.sm_count);
+    const Plan pl = make_plan(d, tune, want, Walk::Leaf);
+    int occ1 = 1, occ2 = 1;
+    if (pl.row < 0 && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ1, kGenericLeafKernels[pl.wide], 128, 0) != cudaSuccess) occ1 = 1;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ2, dt_approx_generic, 128, 0) != cudaSuccess) occ2 = 1;
+    const size_t w1 = sm * (pl.row < 0 ? 128 * (size_t)std::max(1, occ1) : pl.tuples_per_cta());
+    const size_t w2 = sm * 128 * (size_t)std::max(1, occ2);
+    const size_t both = std::lcm(w1, w2);
+    const size_t unit = both <= cap ? both : w2 <= cap ? w2 : 32;
+    return cap / unit * unit;
+}
+
+// Launch the approximate-contribution walk of n fp32 tuples on device d (cudaSetDevice already done): d_out
+// [n][C][F + 1], the single-class run adding the first min(T, 8 S K) trees of `run`, a multi-class run every tree.  Pass
+// 1 is launch_leaf_walk with the plan of a leaf call (want forces both passes' variant; dt_approx_generic is the only
+// pass 2).  Returns a cudaError_t.
+inline cudaError_t launch_approx(Dev& d, const Geom& run, const Tune& tune, int want, const void* d_tuples, size_t n,
+                                 float* d_out, cudaStream_t st, const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const uint32_t F = d.shape.g.F(), C = d.shape.C, T = d.shape.T;
+    const size_t rows = std::min(approx_rows(d, tune, want), (n + 31) & ~(size_t)31);
+    const size_t acc_words = rows * C * (F + 1);     // a multiple of 32 words: the cells start 16-byte aligned
+    cudaError_t rc;
+    if ((rc = shap_scratch(d, acc_words + (rows * T * 2 + 7) / 8, st)) != cudaSuccess) return rc;
+    ApproxParams p = {};
+    p.acc = d.d_shap_scratch;
+    uint16_t* cells = reinterpret_cast<uint16_t*>(p.acc + acc_words);
+    p.cells = cells;
+    p.delta = d.layout.approx_delta;
+    p.feat = d.layout.approx_feat;
+    p.scratch_rows = rows;
+    p.T = T;
+    p.trees = C == 1 ? (uint32_t)std::min<uint64_t>(T, (uint64_t)8 * run.S * run.K) : T;
+    p.F = F; p.C = C; p.first = d.shape.first % C;
+    p.cell_stride = d.layout.approx_cell_stride;
+    p.node_stride = d.layout.approx_node_stride;
+    const unsigned char* tuples = static_cast<const unsigned char*>(d_tuples);
+    for (size_t off = 0; off < n; off += rows) {
+        const size_t m = std::min(rows, n - off);
+        if ((rc = launch_leaf_walk(d, run, tune, want, tuples + off * d.shape.g.tuple_bytes(), m, cells, st, why)) != cudaSuccess)
+            return rc;
+        p.n = m;
+        p.out = d_out + off * C * (F + 1);
+        dt_approx_generic<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(p);
+        if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
+        d.kernel_launches++;
+    }
+    return cudaEventRecord(d.ev_shap, st);
+}
+
+// "<the leaf walk's name> + dt_approx_generic", as launch_approx would launch it
+inline void approx_kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len) {
+    kernel_name(d, tune, want, buf, len, Walk::Leaf);
+    const size_t used = strlen(buf);
+    if (used < len) snprintf(buf + used, len - used, " + dt_approx_generic");
 }
 
 }  // namespace dte

@@ -279,6 +279,9 @@ const char* missing_layout(const Dev& d, Walk w) {
         case Walk::Leaf: return d.layout.bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
         case Walk::Contrib:
         case Walk::Inter: return d.layout.shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
+        case Walk::Approx:
+            return d.layout.approx_delta ? nullptr
+                                         : "no approximate-contribution table resident: load the ensemble with dte_load_ensemble_approx_contribs";
         default: return d.layout.top ? nullptr : "no ensemble loaded";
     }
 }
@@ -335,8 +338,10 @@ int upload(dte_engine* e, DevArray<T>& dst, const std::vector<T>& src) {
 }
 
 // `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr.  `shap`: the contribution
-// layout of a dte_load_ensemble_contribs, else nullptr.  The old ensemble is dropped before the new one is allocated.
-int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap) {
+// layout of a dte_load_ensemble_contribs, else nullptr.  `approx`: the table of a dte_load_ensemble_approx_contribs, else
+// nullptr.  The old ensemble is dropped before the new one is allocated.
+int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap,
+                    const ApproxLayout* approx) {
     CUDA_TRY(e, free_ensemble(d));
     ResidentLayout& lay = d.layout;
     TRY(upload(e, lay.top, pk.top));
@@ -362,6 +367,12 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
         lay.shap.izoff = shap->izoff;
         lay.shap.n_nodes = shap->n_nodes; lay.shap.C = shap->C;
     }
+    if (approx) {
+        TRY(upload(e, lay.approx_delta, approx->delta));
+        TRY(upload(e, lay.approx_feat, approx->feat));
+        lay.approx_cell_stride = approx->cell_stride();
+        lay.approx_node_stride = approx->node_stride();
+    }
     return DTE_OK;
 }
 
@@ -378,26 +389,33 @@ struct TreeShare {
 // start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
 // binned layout is dropped.  With DTE_OPT_LEAF_LAYOUT the leaf-id layout is built and uploaded too; without it any
 // resident leaf-id layout is dropped.  `covers` (fp32 [T_all][2^(D+1)-1] for the trees of the streams): also build and
-// upload the contribution layout of every share; without it any resident contribution layout is dropped.
+// upload the contribution layout of every share; without it any resident contribution layout is dropped.  `approx`
+// with covers: build the approximate-contribution table and the leaf-id layout instead of the contribution layout.
+// Every placement drops the resident layouts it does not build.
 // All or nothing: every share is built and checked before any device changes, so a refused share leaves the previous
 // ensemble resident everywhere; a failed upload leaves no ensemble on any device rather than a mix of two.
 int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr,
-                   const float* covers = nullptr) {
+                   const float* covers = nullptr, bool approx = false) {
     const bool chunked = e->part == Part::Chunked;
     const size_t n_shares = chunked ? e->devs.size() : 1;
-    std::vector<ShapLayout> shap(covers ? n_shares : 0);
+    const bool with_shap = covers && !approx, with_approx = covers && approx;
+    std::vector<ShapLayout> shap(with_shap ? n_shares : 0);
+    std::vector<ApproxLayout> apx(with_approx ? n_shares : 0);
     std::vector<PackedEnsemble> pk(n_shares);
     for (size_t r = 0; r < n_shares; ++r) {
         const TreeShare& s = share[r];
         std::string msg;
-        int rc = covers ? build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
-                                            classes, shap[r], msg) : 0;
-        if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk[r], msg, bins, e->opt_leaf);
+        int rc = with_shap ? build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
+                                               classes, shap[r], msg)
+               : with_approx ? build_approx_layout(g.D, g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count, apx[r], msg)
+                             : 0;
+        if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk[r], msg, bins, e->opt_leaf || with_approx);
         if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
     }
     for (size_t r = 0; r < e->devs.size(); ++r) {
         const size_t s = chunked ? r : 0;
-        const int rc = upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk[s], bins, covers ? &shap[s] : nullptr);
+        const int rc = upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk[s], bins, with_shap ? &shap[s] : nullptr,
+                                       with_approx ? &apx[s] : nullptr);
         if (rc) {
             for (Dev& d : e->devs) free_ensemble(d);
             e->placed.reset();
@@ -578,10 +596,12 @@ int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, vo
         w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
         : w == Walk::Contrib ? launch_contrib(d, e->g, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
         : w == Walk::Inter   ? launch_inter(d, e->g, e->opt_inter_block, tuples, n, static_cast<float*>(out), st, &why)
+        : w == Walk::Approx  ? launch_approx(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
                              : launch_walk(d, e->g, walk_tune(e, w), e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
     if (rc != cudaSuccess)
         return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s",
-                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : w == Walk::Inter ? "interaction walk" : "walk kernel",
+                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : w == Walk::Inter ? "interaction walk"
+                    : w == Walk::Approx ? "approximate-contribution walk" : "walk kernel",
                     why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
@@ -1137,7 +1157,7 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
     // the contributions (interactions) of a tree chunk are fp64 partials: combining them in ring order is not offered
-    if ((w == Walk::Contrib || w == Walk::Inter) && e->part == Part::Chunked)
+    if ((w == Walk::Contrib || w == Walk::Inter || w == Walk::Approx) && e->part == Part::Chunked)
         return fail(e, DTE_ERR_CONFIG, "%s: an ensemble-sharded handle cannot return %s; use a single-device or data-sharded handle", what,
                     w == Walk::Inter ? "interaction values" : "contributions");
     TRY(check_resident(e, g, w));
@@ -1717,10 +1737,11 @@ static int choose_measured_plan(dte_t* e) {
 }
 
 // dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
-// is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs.
+// is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs, or with `approx`
+// dte_load_ensemble_approx_contribs.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
                          uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins,
-                         const float* covers = nullptr) {
+                         const float* covers = nullptr, bool approx = false) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1754,7 +1775,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers));
+    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers, approx));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
@@ -1779,6 +1800,14 @@ int dte_load_ensemble_contribs(dte_t* e, const void* weight_cls, size_t n_weight
                          covers);
 }
 
+int dte_load_ensemble_approx_contribs(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                                      size_t n_findex_cls, const float* covers, uint32_t first_tree, uint32_t num_local_trees,
+                                      uint32_t num_classes) {
+    if (!covers) return e ? fail(e, DTE_ERR_ARG, "dte_load_ensemble_approx_contribs: covers is NULL") : DTE_ERR_ARG;
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
+                         covers, true);
+}
+
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                       size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees) {
     return dte_load_ensemble_classes(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, 1);
@@ -1796,7 +1825,7 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
     const int align = w == Walk::Leaf ? 16 : 4;
     if (reinterpret_cast<uintptr_t>(out) & (align - 1))
         return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what,
-                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib ? "d_contribs" : w == Walk::Inter ? "d_inter"
+                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib || w == Walk::Approx ? "d_contribs" : w == Walk::Inter ? "d_inter"
                     : accumulate ? "d_scores_accum" : "d_scores", align);
     TRY(single_only(e, what));
     Geom g;
@@ -1822,6 +1851,7 @@ static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
     if (w == Walk::Contrib) contrib_kernel_name(e->devs[0], e->forced_variant, buf, len);
     else if (w == Walk::Inter) inter_kernel_name(e->devs[0], e->opt_inter_block, buf, len);
+    else if (w == Walk::Approx) approx_kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len);
     else kernel_name(e->devs[0], walk_tune(e, w), e->forced_variant, buf, len, w);
     return DTE_OK;
 }
@@ -1945,6 +1975,20 @@ int dte_infer_host_contribs(dte_t* e, const void* h_tuples, size_t n, float* h_c
 }
 
 int dte_kernel_name_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Contrib, buf, len); }
+
+// ---- approximate feature contributions (DESIGN.md §14) ----
+int dte_infer_device_approx_contribs(dte_t* e, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_contribs))) return DTE_ERR_ARG;
+    return infer_device(e, Walk::Approx, "dte_infer_device_approx_contribs", d_tuples, n, d_contribs, nullptr, cuda_stream);
+}
+
+int dte_infer_host_approx_contribs(dte_t* e, const void* h_tuples, size_t n, float* h_contribs) {
+    if (!e || (n && (!h_tuples || !h_contribs))) return DTE_ERR_ARG;
+    return infer_host(e, Walk::Approx, "infer_host_approx_contribs", static_cast<const unsigned char*>(h_tuples), n, h_contribs,
+                      nullptr);
+}
+
+int dte_kernel_name_approx_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Approx, buf, len); }
 
 // ---- interaction values (DESIGN.md §13) ----
 int dte_infer_device_interactions(dte_t* e, const void* d_tuples, size_t n, float* d_inter, void* cuda_stream) {

@@ -74,6 +74,11 @@ ABI = [
     ("dte_infer_device_interactions", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_interactions", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("dte_kernel_name_interactions", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_load_ensemble_approx_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                    C.c_uint32, C.c_uint32, C.c_uint32]),
+    ("dte_infer_device_approx_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_approx_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_kernel_name_approx_contribs", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
     ("dte_sparse_to_dense_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
                                              C.c_void_p, C.c_void_p]),
     ("dte_infer_device_sparse", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p,
@@ -307,14 +312,16 @@ class Engine:
 
     # -- fast paths -----------------------------------------------------------------------------
     def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False,
-                      leaves=False, covers=None):
+                      leaves=False, covers=None, approx=False):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
         call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
         binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
         feature), which the *_binned calls walk with u8 tuples.
         leaves=True: DTE_OPT_LEAF_LAYOUT = 1 for this load, so the *_leaves calls can walk it.
         covers: fp32 [T_all, 2^(D+1)-1] node covers of every tree of the streams, indexed like the weight heap: also build
-        the contribution layout the *_contribs calls walk (dte_load_ensemble_contribs; not with binned=True)."""
+        the contribution layout the *_contribs calls walk (dte_load_ensemble_contribs; not with binned=True).
+        approx=True (with covers): build the approximate-contribution table and the leaf-id layout instead, which the
+        *_approx_contribs and *_leaves calls walk (dte_load_ensemble_approx_contribs; not with binned=True)."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
@@ -322,15 +329,20 @@ class Engine:
             saved = getattr(self, "_leaf_opt", 0)
             self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
             try:
-                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers)
+                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers, approx=approx)
             finally:
                 self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
+        if approx and binned:
+            raise ValueError("approx and binned=True cannot be combined: the approximate contribution calls take fp32 tuples")
+        if approx and covers is None:
+            raise ValueError("approx=True needs covers: the table is built from the node covers")
         if covers is not None:
             if binned:
                 raise ValueError("covers and binned=True cannot be combined: the contribution calls take fp32 tuples")
             cv = np.ascontiguousarray(covers, dtype=np.float32)
-            self._check(self._lib.dte_load_ensemble_contribs(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16, _ptr(cv),
-                                                             int(first_tree), int(num_local_trees), int(num_classes)))
+            load = self._lib.dte_load_ensemble_approx_contribs if approx else self._lib.dte_load_ensemble_contribs
+            self._check(load(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16, _ptr(cv), int(first_tree),
+                             int(num_local_trees), int(num_classes)))
         elif binned:
             self._check(self._lib.dte_load_ensemble_binned(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
                                                            int(first_tree), int(num_local_trees), int(num_classes)))
@@ -443,6 +455,27 @@ class Engine:
 
     def kernel_name_contribs(self):
         return self._name(self._lib.dte_kernel_name_contribs)
+
+    # -- approximate feature contributions (DESIGN.md §14) ---------------------------------------------
+    def infer_device_approx_contribs(self, d_tuples, n, d_contribs, stream=None):
+        """[n, C, F + 1] fp32 approximate (Saabas) contributions (bias last) of fp32 tuples [n, F], both on the device
+        (d_tuples 16-byte, d_contribs 4-byte aligned)."""
+        self._check(self._lib.dte_infer_device_approx_contribs(self._h, _ptr(d_tuples), int(n), _ptr(d_contribs),
+                                                               _stream(stream)))
+
+    def infer_host_approx_contribs(self, tuples, out=None):
+        """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> approximate contributions [n, F + 1] for
+        a single-class ensemble, [n, C, F + 1] for a C-class one: the change in expected score each feature's splits
+        make along the tuple's path, the bias (the trees' expected score) last."""
+        t, n = _host_rows(tuples)
+        F, nc = int(self.info()["num_features"]), self.num_classes()
+        if out is None:
+            out = np.empty((n, F + 1) if nc == 1 else (n, nc, F + 1), dtype=np.float32)
+        self._check(self._lib.dte_infer_host_approx_contribs(self._h, _ptr(t), n, _ptr(out)))
+        return out
+
+    def kernel_name_approx_contribs(self):
+        return self._name(self._lib.dte_kernel_name_approx_contribs)
 
     # -- interaction values (DESIGN.md §13) ------------------------------------------------------------
     def infer_device_interactions(self, d_tuples, n, d_inter, stream=None):

@@ -297,6 +297,43 @@ int dte_infer_host_interactions(dte_t* engine, const void* h_tuples, size_t n, f
  * contribution layout. */
 int dte_kernel_name_interactions(dte_t* engine, char* buf, size_t len);
 
+/* ---- approximate feature contributions (DESIGN.md §14) -------------------------------------- */
+/* The Saabas path attribution (XGBoost pred_contribs with approx_contribs, shap's "saabas", the treeinterpreter package):
+ * every node on the path a tuple takes credits its split feature with the change in the tree's expected value from that
+ * node to the child taken.  The definition is XGBoost's; the words are this contract's.  Trees, classes, decision rule
+ * (the run's missing pattern, int32 compare, bit 13) and source-tree conventions are those of the contribution calls
+ * (§12): a node with bit 14 ends its paths at its two child cells, D = 1 has one level, no padding trees, the first
+ * min(T, 8*S*K) local trees of a single-class ensemble, every tree of a multi-class one.  Per source tree, on the host
+ * at load time, in fp64 with every operation rounded on its own and no contraction:
+ *   E[cell] = (double)W[cell] for every reachable end cell;
+ *   E[n] = (zl * E[l]) + (zr * E[r]) for a live internal node n with children l, r, zl = (double)cov[l] / (double)cov[n]
+ *   and zr the same for r (so E[root] is §12's v_t({}) in exact arithmetic);
+ *   delta[c] = E[c] - E[parent(c)] for every non-root cell on a live path.
+ * Per tuple and class, fp64 accumulators from +0: for each tree of the class in stream order, phi[F] = phi[F] + E[root],
+ * then for each step of the tuple's path, root first (node n -> child ch), phi[fidx(n)] = phi[fidx(n)] + delta[ch]; one
+ * round-to-nearest to fp32 per word.  XGBoost computes the same quantities in fp32 and as (E_l c_l + E_r c_r) / c_n, so
+ * its words may differ in the last bits.  A row sums to the score up to rounding.  Layout [n][C][F+1] fp32, bias last.
+ * Binned and sparse tuples are not taken: densify first (dte_sparse_to_dense_device). */
+/* dte_load_ensemble_classes (same placement), plus the leaf-id layout whatever DTE_OPT_LEAF_LAYOUT says (so the leaf calls
+ * work too) and the approximate-contribution table (DESIGN.md §14).  covers as dte_load_ensemble_contribs, checked by the
+ * same rule (DTE_ERR_ARG naming the tree and cell, before anything is uploaded: the resident ensemble stays).  It does not
+ * build the contribution layout and drops a resident one; every other placement (dte_load_ensemble*, a tree line stream)
+ * drops the table, after which the calls below return DTE_ERR_STATE. */
+int dte_load_ensemble_approx_contribs(dte_t* engine, const void* weight_cls, size_t n_weight_cls,
+                                      const void* findex_cls, size_t n_findex_cls, const float* covers,
+                                      uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes);
+/* [n][C][F+1] approximate contributions of n fp32 tuples in device memory.  Single-device handles; stream as
+ * dte_infer_device.  d_tuples must be 16-byte aligned and d_contribs 4-byte aligned, else DTE_ERR_ARG before any launch.
+ * Two kernels per chunk of tuples on the stream: the leaf walk (the plan of dte_infer_device_leaves, forced variants
+ * included) into a cell scratch, then dt_approx_generic.  The scratch (at most 1 GiB) is kept by the handle and freed
+ * by every placement. */
+int dte_infer_device_approx_contribs(dte_t* engine, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream);
+/* The same from host memory through the landing pipeline: single-device and data-sharded handles (rows in global tuple
+ * order).  An ensemble-sharded handle returns DTE_ERR_CONFIG. */
+int dte_infer_host_approx_contribs(dte_t* engine, const void* h_tuples, size_t n, float* h_contribs);
+/* "<leaf walk name> + dt_approx_generic"; DTE_ERR_STATE without the approximate-contribution table. */
+int dte_kernel_name_approx_contribs(dte_t* engine, char* buf, size_t len);
+
 /* ---- sparse tuples (DESIGN.md §11) ------------------------------------------------------------- */
 /* n tuples as CSR rows: indptr int64 [n + 1], indices uint32 [nnz] (feature numbers), values [nnz] 32-bit words (fp32 bit
  * patterns).  Row i's entries are k in [indptr[i], indptr[i+1]), indexing indices and values absolutely, so indptr[0]

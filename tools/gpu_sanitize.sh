@@ -77,6 +77,14 @@ for T in tests/test_gpu_interactions.py::test_row_blocks_give_the_same_bytes tes
   itag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_inter_${itag}.log"
 done
+# the approximate contributions: both passes (the leaf walk into the cell scratch, dt_approx_generic from it) at D = 15,
+# at F = 2048, in two scratch chunks, on the ragged tail of a warp, and with three classes on a tree chunk
+for T in "tests/test_gpu_approx_contribs.py::test_depths_and_widths[D15-F4]" "tests/test_gpu_approx_contribs.py::test_depths_and_widths[D3-F2048]" \
+         tests/test_gpu_approx_contribs.py::test_two_scratch_chunks "tests/test_gpu_approx_contribs.py::test_tuple_counts[33]" \
+         tests/test_gpu_approx_contribs.py::test_classes_and_a_chunk; do
+  atag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_approx_${atag}.log"
+done
 # leaks: the C++ host (no torch caching allocator in the process) over a handle's whole life, create to destroy, on three
 # ring positions sharing one GPU, data- and ensemble-sharded, fed by the line stream and by the host fast path
 for mode in stream host; do

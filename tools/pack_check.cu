@@ -14,6 +14,10 @@
 //     ->  the leaf words, with the top levels walked through the split tree tops (top_split) as dt_walk_tile_split
 //         walks them
 // Every run also decodes every record of top_split and checks it against the same record of top (exit 7 otherwise).
+//   pack_check approx <D> <F> <weights.bin> <findex.bin> <covers.bin> [<first> <count>]
+//     ->  the approximate-contribution table of build_approx_layout (DESIGN.md §14) for stream trees [first, first +
+//         count) (default: all), binary on stdout: fp64 delta [count][2^(D+1)] ([t][0] = E[root]), then u16 feat
+//         [count][2^D]; a refused load exits 3 with the message on stderr.  covers.bin: fp32 [T_all][2^(D+1)-1].
 #include "../distributed-decisiontrees_b200/csrc/dte_device.cuh"
 #include <cstdio>
 #include <cstring>
@@ -84,7 +88,25 @@ static uint32_t walk(const PackedEnsemble& pk, uint32_t slot, const uint32_t* x,
     return r1 ? (r2 ? leaves.w : leaves.z) : (r2 ? leaves.y : leaves.x);
 }
 
+static int approx_main(int argc, char** argv) {
+    if (argc < 6) return 2;
+    const uint32_t D = (uint32_t)atoi(argv[1]);
+    const uint32_t w_cls = (uint32_t)(((2ull << D) - 1 + 3) / 4), f_cls = (uint32_t)(((1ull << D) - 1 + 7) / 8);
+    auto wl = slurp(argv[3]), fl = slurp(argv[4]), cv = slurp(argv[5]);
+    const uint32_t first = argc > 7 ? (uint32_t)atoi(argv[6]) : 0u, count = argc > 7 ? (uint32_t)atoi(argv[7]) : 0u;
+    if ((wl.size() / 16 / w_cls) * ((2ull << D) - 1) * 4 != cv.size()) return 4;
+    ApproxLayout ap;
+    std::string msg;
+    const int rc = build_approx_layout(D, w_cls, f_cls, wl.data(), wl.size() / 16, fl.data(), fl.size() / 16,
+                                       reinterpret_cast<const float*>(cv.data()), first, count, ap, msg);
+    if (rc) { fprintf(stderr, "build_approx_layout: %d %s\n", rc, msg.c_str()); return 3; }
+    fwrite(ap.delta.data(), 8, ap.delta.size(), stdout);
+    fwrite(ap.feat.data(), 2, ap.feat.size(), stdout);
+    return 0;
+}
+
 int main(int argc, char** argv) {
+    if (argc > 1 && !strcmp(argv[1], "approx")) return approx_main(argc - 1, argv + 1);
     const bool leaf = argc > 1 && !strcmp(argv[1], "leaf");
     const bool split = argc > 1 && !strcmp(argv[1], "split");
     if (leaf || split) { --argc; ++argv; }
