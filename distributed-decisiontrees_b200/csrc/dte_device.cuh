@@ -31,6 +31,41 @@ enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED 
 // or the approximate feature contributions (DESIGN.md §14)
 enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx };
 
+// How an ensemble-sharded handle returns a walk's results: the ring positions' partials combined in ring order, each
+// position's rows in its own columns of the caller's rows, or refused (fp64 attribution partials are never combined).
+enum class Sharded { Combine, Columns, Refuse };
+
+// What the engine needs to know about each kind of walk.  The rest is ResidentLayout::resident (whether the kind's
+// layout is resident), launch_kind and kind_kernel_name.
+struct WalkKind {
+    uint32_t feature_bytes;   // input bytes per feature of a tuple: u8 bins or fp32 words
+    const char* in_arg;       // the device call's input and output pointers, as its refusals name them
+    const char* out_arg;
+    int out_align;            // bytes the output pointer must be aligned to
+    bool rows;                // results land in Slot::d_rows, else in the scores d_sc / d_part
+    const char* missing;      // why the walk is refused when its layout is not resident
+    bool class_slots;         // a multi-class run needs S K 8 slots for the largest class
+    bool row_cap;             // a row of C (F + 1)^2 words may not exceed kInterMaxRowWords
+    Sharded sharded;
+    const char* sharded_noun; // Sharded::Refuse: what the refusal says the handle cannot return
+    const char* label;        // names the walk in a failed launch
+};
+inline constexpr WalkKind kWalkKinds[] = {
+    {4, "d_tuples", "d_scores", 4, false, "no ensemble loaded", true, false, Sharded::Combine, nullptr, "walk kernel"},
+    {1, "d_bins", "d_scores", 4, false, "no binned layout resident: load the ensemble with dte_load_ensemble_binned", true,
+     false, Sharded::Combine, nullptr, "walk kernel"},
+    {4, "d_tuples", "d_leaves", 16, true, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1", false,
+     false, Sharded::Columns, nullptr, "leaf walk"},
+    {4, "d_tuples", "d_contribs", 4, true, "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs",
+     true, false, Sharded::Refuse, "contributions", "contribution walk"},
+    {4, "d_tuples", "d_inter", 4, true, "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs",
+     true, true, Sharded::Refuse, "interaction values", "interaction walk"},
+    {4, "d_tuples", "d_contribs", 4, true,
+     "no approximate-contribution table resident: load the ensemble with dte_load_ensemble_approx_contribs", true, false,
+     Sharded::Refuse, "contributions", "approximate-contribution walk"},
+};
+inline const WalkKind& kind(Walk w) { return kWalkKinds[static_cast<int>(w)]; }
+
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536,tops=6"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
 //  phased: 0 off / k>=1 on with part A ending k levels earlier, fill=1: one bulk copy per tree,
@@ -692,6 +727,18 @@ struct ResidentLayout {
                shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes() +
                approx_delta.bytes() + approx_feat.bytes();
     }
+    // whether the layout a walk of kind w reads is resident
+    bool resident(Walk w) const {
+        switch (w) {
+            case Walk::Fp32: return top;
+            case Walk::Binned: return top_b;
+            case Walk::Leaf: return bottom_id;
+            case Walk::Contrib:
+            case Walk::Inter: return shap_paths;
+            case Walk::Approx: return approx_delta;
+        }
+        return false;
+    }
 };
 
 // One landing slot: a device buffer the tuple stream lands in, plus the scores (labels) of its tuples.
@@ -736,7 +783,7 @@ struct Dev {
     DevArray<double> d_shap_scratch;
     Event ev_shap;
     Walk walk = Walk::Fp32;           // the walk the landing slots feed: binned calls land u8 bins (F bytes per tuple)
-    size_t run_tuple_bytes() const { return walk == Walk::Binned ? shape.g.F() : shape.g.tuple_bytes(); }
+    size_t run_tuple_bytes() const { return (size_t)shape.g.F() * kind(walk).feature_bytes; }
 
     // ---- landing slots ----
     Slot slot[kNumSlots];
@@ -770,9 +817,6 @@ struct Dev {
     uint64_t tuples_landed = 0;       // whole tuples landed on this device since `start`
 };
 
-// Leaf, contribution, interaction and approximate-contribution walks write their rows into Slot::d_rows; score walks
-// into d_sc / d_part, which the combines, the labels and the line stream's ring read.
-inline bool row_walk(Walk w) { return w == Walk::Leaf || w == Walk::Contrib || w == Walk::Inter || w == Walk::Approx; }
 // Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes,
 // C (F + 1) contribution words (exact or approximate) or C (F + 1)^2 interaction words
 inline size_t row_bytes(const Dev& d, Walk w) {
@@ -958,6 +1002,13 @@ inline WalkParams walk_params(const Dev& d, const Geom& run, const Tune& tune, c
 inline WalkParams& walk_of(WalkParams& p) { return p; }
 inline WalkParams& walk_of(LeafParams& p) { return p.w; }
 
+// The status of the kernel launch just issued on device d, which counts it when it succeeded
+inline cudaError_t launched(Dev& d) {
+    const cudaError_t rc = cudaGetLastError();
+    if (rc == cudaSuccess) d.kernel_launches++;
+    return rc;
+}
+
 // Launch `kernel`, the instantiation plan pl selects, over n tuples: one 128-thread block per 128 tuples for the generic
 // walk, else one persistent CTA per SM (at most one per tile) with the plan's dynamic shared memory.  Sets the tile
 // count of the parameter block and counts the launch.  Returns a cudaError_t.
@@ -974,9 +1025,7 @@ inline cudaError_t launch_plan(Dev& d, const Plan& pl, void (*kernel)(Params), P
         if (rc != cudaSuccess) return rc;
     }
     kernel<<<grid, pl.threads(), pl.row < 0 ? 0 : pl.smem, st>>>(params);
-    const cudaError_t rc = cudaGetLastError();
-    if (rc == cudaSuccess) d.kernel_launches++;
-    return rc;
+    return launched(d);
 }
 
 // Launch the walk of n tuples on device d (cudaSetDevice already done), summed with the K, S and missing pattern of
@@ -1063,10 +1112,15 @@ inline int shap_tile_warps_per_sm(const Dev& d) {
 // D = 8, the tile is 5 % faster at F = 20 (28 warps per SM), the generic kernel 1.2-1.4x faster at F = 48-72 (12 and 8
 // tile warps) and 1.4-3x faster from F = 128 (4 and 2 tile warps), DESIGN.md §12.
 constexpr int kShapTileMinWarps = 16;
+// The path-length bound M of the dt_shap_* instantiation that holds the contribution layout's longest merged path
+inline int shap_bound(const Dev& d) {
+    const uint32_t M = d.layout.shap.M;
+    return M <= 3 ? 3 : M <= 7 ? 7 : 15;
+}
 // How a contribution walk runs, read by both launch_contrib and contrib_kernel_name: dt_shap_tile with `groups` warps
-// and `smem` bytes per CTA, or dt_shap_generic, instantiated with the path-length bound that holds the layout's longest
-// merged path.  The tile runs never when GENERIC is forced; when TILE (or TILE_STAGED) is forced, whenever a tuple group
-// fits; under AUTO, when it also keeps kShapTileMinWarps warps per SM.
+// and `smem` bytes per CTA, or dt_shap_generic, instantiated with shap_bound.  The tile runs never when GENERIC is
+// forced; when TILE (or TILE_STAGED) is forced, whenever a tuple group fits; under AUTO, when it also keeps
+// kShapTileMinWarps warps per SM.
 struct ShapPlan {
     bool tile = false;
     int groups = 0;
@@ -1075,8 +1129,7 @@ struct ShapPlan {
 };
 inline ShapPlan shap_plan(const Dev& d, int want) {
     ShapPlan p;
-    const uint32_t M = d.layout.shap.M;
-    p.bound = M <= 3 ? 3 : M <= 7 ? 7 : 15;
+    p.bound = shap_bound(d);
     const int G = shap_tile_groups(d);
     p.tile = want != KERNEL_GENERIC && G >= 1 && (want != KERNEL_AUTO || shap_tile_warps_per_sm(d) >= kShapTileMinWarps);
     if (p.tile) {
@@ -1093,8 +1146,14 @@ inline ShapKernel shap_kernel(const ShapPlan& p) {
 }
 constexpr size_t kShapScratchBytes = 256ull << 20;   // dt_shap_generic accumulators: rows per launch = this / (8 (F + 1))
 
-// The ShapParams of a contribution or interaction walk on device d: the resident contribution layout and, for a
-// single-class run, the first min(T, 8 S K) trees of `run`, for a multi-class run every tree.  The launchers add the rest.
+// The trees an attribution walk adds: for a single-class run the first min(T, 8 S K) trees of `run`, for a multi-class
+// run every tree
+inline uint32_t run_trees(const Dev& d, const Geom& run) {
+    return d.shape.C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : d.shape.T;
+}
+
+// The ShapParams of a contribution or interaction walk on device d: the resident contribution layout and the trees
+// run_trees picks.  The launchers add the rest.
 inline ShapParams shap_params(const Dev& d, const Geom& run) {
     const ResidentLayout& lay = d.layout;
     ShapParams p = {};
@@ -1104,7 +1163,7 @@ inline ShapParams shap_params(const Dev& d, const Geom& run) {
     p.cls_tree = lay.shap_cls_tree;
     p.F = d.shape.g.F(); p.C = d.shape.C; p.missing = run.missing;
     p.n_nodes = lay.shap.n_nodes; p.stride = lay.shap.stride; p.zoff = lay.shap.zoff; p.izoff = lay.shap.izoff;
-    p.trees0 = d.shape.C == 1 ? (uint32_t)std::min<uint64_t>(d.shape.T, (uint64_t)8 * run.S * run.K) : 0;
+    p.trees0 = run_trees(d, run);
     return p;
 }
 
@@ -1120,10 +1179,22 @@ inline cudaError_t shap_scratch(Dev& d, size_t words, cudaStream_t st) {
     return cudaStreamWaitEvent(st, d.ev_shap, 0);
 }
 
+// Run n tuples through the device's fp64 scratch, at least `words` of it made ready on st by shap_scratch: body(scratch,
+// off, m) enqueues the chunk of m <= rows tuples from tuple off on st, counting its launches, and returns a cudaError_t.
+// The scratch's event is recorded after the last chunk.
+template <class Body>
+inline cudaError_t scratch_chunks(Dev& d, size_t n, size_t rows, size_t words, cudaStream_t st, Body body) {
+    cudaError_t rc;
+    if ((rc = shap_scratch(d, words, st)) != cudaSuccess) return rc;
+    for (size_t off = 0; off < n; off += rows)
+        if ((rc = body(d.d_shap_scratch.get(), off, std::min(rows, n - off))) != cudaSuccess) return rc;
+    return cudaEventRecord(d.ev_shap, st);
+}
+
 // Launch the contribution walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident
-// contribution layout: d_out [n][C][F + 1].  The single-class run adds the first min(T, 8 S K) trees of `run`, a
-// multi-class run every tree.  dt_shap_generic runs in launches of at most kShapScratchBytes / (8 (F + 1)) tuples through
-// the device's fp64 scratch, which waits for the previous walk using it.  Returns a cudaError_t.
+// contribution layout: d_out [n][C][F + 1], adding the trees run_trees picks.  dt_shap_generic runs in launches of at
+// most kShapScratchBytes / (8 (F + 1)) tuples through the device's fp64 scratch, which waits for the previous walk using
+// it.  Returns a cudaError_t.
 inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, const void* d_tuples, size_t n, float* d_out,
                                   cudaStream_t st, const char** why) {
     *why = nullptr;
@@ -1134,32 +1205,34 @@ inline cudaError_t launch_contrib(Dev& d, const Geom& run, int want_variant, con
     const ShapKernel k = shap_kernel(pl);
     const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
     const size_t row_words = (size_t)C * (F + 1);
-    cudaError_t rc;
     if (pl.tile) {
         const int G = pl.groups;
         const unsigned long long blocks = ((n + 31) / 32 + G - 1) / G;
         if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
         p.tuples = tuples; p.out = d_out; p.n = n; p.groups = (uint32_t)G;
-        if ((rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem)) != cudaSuccess) return rc;
+        const cudaError_t rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+        if (rc != cudaSuccess) return rc;
         k<<<(unsigned)blocks, 32 * G, pl.smem, st>>>(p);
-        if ((rc = cudaGetLastError()) == cudaSuccess) d.kernel_launches++;
-        return rc;
+        return launched(d);
     }
     const size_t cap = std::max<size_t>(32, (kShapScratchBytes / ((size_t)(F + 1) * 8)) & ~(size_t)31);
     const size_t rows = std::min(cap, (n + 31) & ~(size_t)31);
-    // what the kernel indexes: phi[f * rows + row], f <= F, row < rows
-    if ((rc = shap_scratch(d, rows * (F + 1), st)) != cudaSuccess) return rc;
-    p.scratch = d.d_shap_scratch;
     p.scratch_rows = rows;
-    for (size_t off = 0; off < n; off += rows) {
-        p.n = std::min(rows, n - off);
+    // what the kernel indexes: phi[f * rows + row], f <= F, row < rows
+    return scratch_chunks(d, n, rows, rows * (F + 1), st, [&](double* scratch, size_t off, size_t m) {
+        p.scratch = scratch;
+        p.n = m;
         p.tuples = tuples + off * F;
         p.out = d_out + off * row_words;
-        k<<<(unsigned)((p.n + 127) / 128), 128, 0, st>>>(p);
-        if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
-        d.kernel_launches++;
-    }
-    return cudaEventRecord(d.ev_shap, st);
+        k<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(p);
+        return launched(d);
+    });
+}
+
+// Append the classes of a multi-class ensemble to the name of its walk's kernel in buf
+inline void name_classes(const Dev& d, char* buf, size_t len) {
+    const size_t used = strlen(buf);
+    if (d.shape.C >= 2 && used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
 }
 
 // "dt_shap_tile<bound> warps=G smem=..." or "dt_shap_generic<bound>", as launch_contrib would launch it
@@ -1167,10 +1240,7 @@ inline void contrib_kernel_name(const Dev& d, int want, char* buf, size_t len) {
     const ShapPlan pl = shap_plan(d, want);
     if (pl.tile) snprintf(buf, len, "dt_shap_tile<%d> warps=%d smem=%zu", pl.bound, pl.groups, pl.smem);
     else snprintf(buf, len, "dt_shap_generic<%d>", pl.bound);
-    if (d.shape.C >= 2) {
-        const size_t used = strlen(buf);
-        if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
-    }
+    name_classes(d, buf, len);
 }
 
 // ---- interaction values (DESIGN.md §13) ----
@@ -1191,7 +1261,7 @@ struct InterPlan {
 inline InterPlan inter_plan(const Dev& d, uint32_t forced_block, size_t n) {
     InterPlan p;
     const uint32_t F = d.shape.g.F();
-    p.bound = d.layout.shap.M <= 3 ? 3 : d.layout.shap.M <= 7 ? 7 : 15;
+    p.bound = shap_bound(d);
     const size_t row_bytes = (size_t)8 * F;          // one matrix row of one tuple
     const size_t tuples = std::min((size_t)std::max(1, d.sm_count) * kInterRowsPerSM, (std::min<size_t>(n, 1ull << 40) + 31) & ~(size_t)31);
     const size_t B = forced_block ? forced_block : kInterScratchBytes / (row_bytes * std::max<size_t>(tuples, 32));
@@ -1217,35 +1287,29 @@ inline cudaError_t launch_inter(Dev& d, const Geom& run, uint32_t forced_block, 
     const InterPlan pl = inter_plan(d, forced_block, n);
     const InterKernel k = inter_kernel(pl.bound);
     const size_t rows = std::min(pl.rows, (n + 31) & ~(size_t)31);
-    cudaError_t rc;
-    if ((rc = shap_scratch(d, rows * std::min(pl.block, F) * F, st)) != cudaSuccess) return rc;
-    p.scratch = d.d_shap_scratch;
     p.scratch_rows = rows;
     const size_t row_words = (size_t)C * (F + 1) * (F + 1);
     const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
-    for (size_t off = 0; off < n; off += rows) {
-        p.n = std::min(rows, n - off);
+    return scratch_chunks(d, n, rows, rows * std::min(pl.block, F) * F, st, [&](double* scratch, size_t off, size_t m) {
+        p.scratch = scratch;
+        p.n = m;
         p.tuples = tuples + off * F;
         p.out = d_out + off * row_words;
         for (uint32_t r0 = 0; r0 <= F; r0 += pl.block) {
             ip.r0 = r0;
             ip.r1 = std::min(F + 1, r0 + pl.block);
-            k<<<(unsigned)((p.n + 127) / 128), 128, 0, st>>>(ip);
-            if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
-            d.kernel_launches++;
+            k<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(ip);
+            if (const cudaError_t rc = launched(d)) return rc;
         }
-    }
-    return cudaEventRecord(d.ev_shap, st);
+        return cudaSuccess;
+    });
 }
 
 // "dt_shap_inter<bound> rows=B", as launch_inter would launch a call of a full machine's tuples (or more)
 inline void inter_kernel_name(const Dev& d, uint32_t forced_block, char* buf, size_t len) {
     const InterPlan pl = inter_plan(d, forced_block, SIZE_MAX);
     snprintf(buf, len, "dt_shap_inter<%d> rows=%u", pl.bound, pl.block);
-    if (d.shape.C >= 2) {
-        const size_t used = strlen(buf);
-        if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
-    }
+    name_classes(d, buf, len);
 }
 
 // The plan of a walk of kind w, named dt_walk_generic / dt_walk_tile with the kind's suffix: _u8 binned, _leaf leaf
@@ -1264,10 +1328,7 @@ inline void kernel_name(const Dev& d, const Tune& tune, int want, char* buf, siz
             if (used < len) snprintf(buf + used, len - used, " tops=6");
         }
     }
-    if (d.shape.C >= 2) {
-        const size_t used = strlen(buf);
-        if (used < len) snprintf(buf + used, len - used, " classes=%u", d.shape.C);
-    }
+    name_classes(d, buf, len);
 }
 
 
@@ -1299,9 +1360,8 @@ inline size_t approx_rows(const Dev& d, const Tune& tune, int want) {
 }
 
 // Launch the approximate-contribution walk of n fp32 tuples on device d (cudaSetDevice already done): d_out
-// [n][C][F + 1], the single-class run adding the first min(T, 8 S K) trees of `run`, a multi-class run every tree.  Pass
-// 1 is launch_leaf_walk with the plan of a leaf call (want forces both passes' variant; dt_approx_generic is the only
-// pass 2).  Returns a cudaError_t.
+// [n][C][F + 1], adding the trees run_trees picks.  Pass 1 is launch_leaf_walk with the plan of a leaf call (want forces
+// both passes' variant; dt_approx_generic is the only pass 2).  Returns a cudaError_t.
 inline cudaError_t launch_approx(Dev& d, const Geom& run, const Tune& tune, int want, const void* d_tuples, size_t n,
                                  float* d_out, cudaStream_t st, const char** why) {
     *why = nullptr;
@@ -1309,39 +1369,58 @@ inline cudaError_t launch_approx(Dev& d, const Geom& run, const Tune& tune, int 
     const uint32_t F = d.shape.g.F(), C = d.shape.C, T = d.shape.T;
     const size_t rows = std::min(approx_rows(d, tune, want), (n + 31) & ~(size_t)31);
     const size_t acc_words = rows * C * (F + 1);     // a multiple of 32 words: the cells start 16-byte aligned
-    cudaError_t rc;
-    if ((rc = shap_scratch(d, acc_words + (rows * T * 2 + 7) / 8, st)) != cudaSuccess) return rc;
     ApproxParams p = {};
-    p.acc = d.d_shap_scratch;
-    uint16_t* cells = reinterpret_cast<uint16_t*>(p.acc + acc_words);
-    p.cells = cells;
     p.delta = d.layout.approx_delta;
     p.feat = d.layout.approx_feat;
     p.scratch_rows = rows;
     p.T = T;
-    p.trees = C == 1 ? (uint32_t)std::min<uint64_t>(T, (uint64_t)8 * run.S * run.K) : T;
+    p.trees = run_trees(d, run);
     p.F = F; p.C = C; p.first = d.shape.first % C;
     p.cell_stride = d.layout.approx_cell_stride;
     p.node_stride = d.layout.approx_node_stride;
     const unsigned char* tuples = static_cast<const unsigned char*>(d_tuples);
-    for (size_t off = 0; off < n; off += rows) {
-        const size_t m = std::min(rows, n - off);
-        if ((rc = launch_leaf_walk(d, run, tune, want, tuples + off * d.shape.g.tuple_bytes(), m, cells, st, why)) != cudaSuccess)
+    return scratch_chunks(d, n, rows, acc_words + (rows * T * 2 + 7) / 8, st, [&](double* scratch, size_t off, size_t m) {
+        uint16_t* cells = reinterpret_cast<uint16_t*>(scratch + acc_words);
+        p.acc = scratch;
+        p.cells = cells;
+        if (const cudaError_t rc = launch_leaf_walk(d, run, tune, want, tuples + off * d.shape.g.tuple_bytes(), m, cells, st, why))
             return rc;
         p.n = m;
         p.out = d_out + off * C * (F + 1);
         dt_approx_generic<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(p);
-        if ((rc = cudaGetLastError()) != cudaSuccess) return rc;
-        d.kernel_launches++;
-    }
-    return cudaEventRecord(d.ev_shap, st);
+        return launched(d);
+    });
 }
 
-// "<the leaf walk's name> + dt_approx_generic", as launch_approx would launch it
-inline void approx_kernel_name(const Dev& d, const Tune& tune, int want, char* buf, size_t len) {
-    kernel_name(d, tune, want, buf, len, Walk::Leaf);
-    const size_t used = strlen(buf);
-    if (used < len) snprintf(buf + used, len - used, " + dt_approx_generic");
+// ---- every kind of walk (kWalkKinds) ----
+// Launch the walk of kind w over n tuples on device d (cudaSetDevice already done) with the engine's knobs: the walk
+// tune, the forced variant `want` and the interaction block.  `out` receives n rows of row_bytes; labels and accumulate
+// are the score walks' (Fp32, Binned: launch_walk).  Returns a cudaError_t; *why says why a launch was refused before it ran.
+inline cudaError_t launch_kind(Dev& d, Walk w, const Geom& run, const Tune& tune, int want, uint32_t inter_block,
+                               const void* tuples, size_t n, void* out, uint8_t* labels, cudaStream_t st, bool accumulate,
+                               const char** why) {
+    switch (w) {
+        case Walk::Leaf: return launch_leaf_walk(d, run, tune, want, tuples, n, static_cast<uint16_t*>(out), st, why);
+        case Walk::Contrib: return launch_contrib(d, run, want, tuples, n, static_cast<float*>(out), st, why);
+        case Walk::Inter: return launch_inter(d, run, inter_block, tuples, n, static_cast<float*>(out), st, why);
+        case Walk::Approx: return launch_approx(d, run, tune, want, tuples, n, static_cast<float*>(out), st, why);
+        default: return launch_walk(d, run, tune, want, tuples, n, static_cast<float*>(out), labels, st, accumulate, why, w);
+    }
+}
+
+// The kernel, and its plan, that launch_kind would launch for a walk of kind w with the same knobs
+inline void kind_kernel_name(const Dev& d, Walk w, const Tune& tune, int want, uint32_t inter_block, char* buf, size_t len) {
+    switch (w) {
+        case Walk::Contrib: return contrib_kernel_name(d, want, buf, len);
+        case Walk::Inter: return inter_kernel_name(d, inter_block, buf, len);
+        case Walk::Approx: {                           // the leaf walk, then dt_approx_generic
+            kernel_name(d, tune, want, buf, len, Walk::Leaf);
+            const size_t used = strlen(buf);
+            if (used < len) snprintf(buf + used, len - used, " + dt_approx_generic");
+            return;
+        }
+        default: return kernel_name(d, tune, want, buf, len, w);
+    }
 }
 
 }  // namespace dte

@@ -272,24 +272,11 @@ int decide_partition(dte_engine* e, const Geom& g) {
     return DTE_OK;
 }
 
-// Why device d cannot run a walk of kind w: the layout that walk reads is not resident (nullptr: it is).
-const char* missing_layout(const Dev& d, Walk w) {
-    switch (w) {
-        case Walk::Binned: return d.layout.top_b ? nullptr : "no binned layout resident: load the ensemble with dte_load_ensemble_binned";
-        case Walk::Leaf: return d.layout.bottom_id ? nullptr : "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1";
-        case Walk::Contrib:
-        case Walk::Inter: return d.layout.shap_paths ? nullptr : "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs";
-        case Walk::Approx:
-            return d.layout.approx_delta ? nullptr
-                                         : "no approximate-contribution table resident: load the ensemble with dte_load_ensemble_approx_contribs";
-        default: return d.layout.top ? nullptr : "no ensemble loaded";
-    }
-}
-
 // A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
 // layout and the validated feature-index range; K, S and the missing pattern are free to change), and needs the layout
 // of its walk.  A leaf walk walks every tree whatever K and S say.
 int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
+    const WalkKind& k = kind(w);
     if (e->multi() && e->placed) {
         if (e->part != *e->placed)
             return fail(e, DTE_ERR_CONFIG, "reg 201 selects the %s partition but the resident ensemble was programmed %s",
@@ -299,16 +286,16 @@ int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
     }
     for (Dev& d : e->devs) {
         for (Walk need : {Walk::Fp32, w})            // the ensemble, then the layout of the walk
-            if (const char* why = missing_layout(d, need)) return fail(e, DTE_ERR_STATE, "%s", why);
+            if (!d.layout.resident(need)) return fail(e, DTE_ERR_STATE, "%s", kind(need).missing);
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
                         g.F(), g.D, d.shape.g.F(), d.shape.g.D);
         const uint64_t F1 = d.shape.g.F() + 1;
-        if (w == Walk::Inter && d.shape.C * F1 * F1 > kInterMaxRowWords)
+        if (k.row_cap && d.shape.C * F1 * F1 > kInterMaxRowWords)
             return fail(e, DTE_ERR_UNSUPPORTED, "an interaction row of %u classes x %llu x %llu words exceeds 64 MiB (2^24 words)",
                         d.shape.C, (unsigned long long)F1, (unsigned long long)F1);
         // a multi-class walk covers every tree: the slots must hold the largest class (no silent truncation per class)
-        if (w != Walk::Leaf && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
+        if (k.class_slots && d.shape.C >= 2 && (uint64_t)g.S * g.K * 8 < d.shape.cls_max)
             return fail(e, DTE_ERR_CONFIG, "reg 205: S=%u x K=%u x 8 slots hold fewer trees than the largest of the %u classes (%u trees): "
                         "a multi-class run needs S >= %u", g.S, g.K, d.shape.C, d.shape.cls_max, (d.shape.cls_max + 8 * g.K - 1) / (8 * g.K));
     }
@@ -544,7 +531,7 @@ int poll_dev(dte_engine* e, Dev& d, uint64_t need) {
 
 // The result rows of slot s for the device's walk: d_rows, or the final scores d_sc
 unsigned char* slot_rows(const Dev& d, const Slot& s) {
-    return row_walk(d.walk) ? s.d_rows.get() : reinterpret_cast<unsigned char*>(s.d_sc.get());
+    return kind(d.walk).rows ? s.d_rows.get() : reinterpret_cast<unsigned char*>(s.d_sc.get());
 }
 
 // D2H of `cnt` results of slot s starting at slot-local tuple `from`, into the device's current sink: rows of row_bytes,
@@ -587,22 +574,14 @@ const Tune& walk_tune(const dte_engine* e, Walk w) {
 }
 
 // Launch the walk of kind w over n tuples on device d with the run's geometry; a refused launch is DTE_ERR_ARG.  `out`
-// receives the scores [n][C] (labels too when given), for a leaf walk the cells [n][T], for a contribution walk the
-// contributions [n][C][F + 1].
+// receives n rows of row_bytes (a score walk's labels too when given).
 int walk_or_fail(dte_engine* e, Dev& d, Walk w, const void* tuples, size_t n, void* out, uint8_t* labels, cudaStream_t st,
                  bool accumulate = false) {
     const char* why = nullptr;
-    const cudaError_t rc =
-        w == Walk::Leaf ? launch_leaf_walk(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<uint16_t*>(out), st, &why)
-        : w == Walk::Contrib ? launch_contrib(d, e->g, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
-        : w == Walk::Inter   ? launch_inter(d, e->g, e->opt_inter_block, tuples, n, static_cast<float*>(out), st, &why)
-        : w == Walk::Approx  ? launch_approx(d, e->g, e->tune, e->forced_variant, tuples, n, static_cast<float*>(out), st, &why)
-                             : launch_walk(d, e->g, walk_tune(e, w), e->forced_variant, tuples, n, static_cast<float*>(out), labels, st, accumulate, &why, w);
+    const cudaError_t rc = launch_kind(d, w, e->g, walk_tune(e, w), e->forced_variant, e->opt_inter_block, tuples, n, out,
+                                       labels, st, accumulate, &why);
     if (rc != cudaSuccess)
-        return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s",
-                    w == Walk::Leaf ? "leaf walk" : w == Walk::Contrib ? "contribution walk" : w == Walk::Inter ? "interaction walk"
-                    : w == Walk::Approx ? "approximate-contribution walk" : "walk kernel",
-                    why ? why : cudaGetErrorString(rc));
+        return fail(e, why ? DTE_ERR_ARG : DTE_ERR_CUDA, "%s launch failed: %s", kind(w).label, why ? why : cudaGetErrorString(rc));
     return DTE_OK;
 }
 
@@ -833,21 +812,21 @@ int submit_group(dte_engine* e, int b) {
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         CUDA_TRY(e, cudaEventRecord(d.slot[b].ev_land, d.s_h2d));
     }
-    // every ring position walks every tuple for its own trees: a leaf walk lands its cells in its own columns, a score
-    // walk leaves partials that are ring-combined on the host device
-    const bool cells = h.walk == Walk::Leaf;
+    // every ring position walks every tuple for its own trees: a Sharded::Columns walk lands its rows in its own columns,
+    // a Sharded::Combine walk leaves partials that are ring-combined on the host device (infer_host refuses the rest)
+    const bool columns = kind(h.walk).sharded == Sharded::Columns;
     for (Dev& d : e->devs) {
         Slot& s = d.slot[b];
         CUDA_TRY(e, cudaSetDevice(d.ordinal));
         for (Dev& src : e->devs) CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, src.slot[b].ev_land, 0));   // every piece has landed here
-        // the cells of this slot have been copied out / the previous combine is done with our partials
-        CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, cells ? s.ev_d2h : h.slot[b].ev_comb, 0));
-        void* out = cells ? (void*)(s.d_rows + walked * row_bytes(d, Walk::Leaf)) : (void*)(s.d_part + walked * C);
+        // the rows of this slot have been copied out / the previous combine is done with our partials
+        CUDA_TRY(e, cudaStreamWaitEvent(d.s_main, columns ? s.ev_d2h : h.slot[b].ev_comb, 0));
+        void* out = columns ? (void*)(s.d_rows + walked * row_bytes(d, h.walk)) : (void*)(s.d_part + walked * C);
         TRY(walk_or_fail(e, d, h.walk, s.d_tup + walked * tb, cnt, out, nullptr, d.s_main));
         CUDA_TRY(e, cudaEventRecord(s.ev_walk, d.s_main));
         s.walked = whole;
     }
-    if (cells) {
+    if (columns) {
         for (Dev& d : e->devs) {
             CUDA_TRY(e, cudaSetDevice(d.ordinal));
             TRY(enqueue_results(e, d, d.slot[b], walked, cnt, false));
@@ -1066,14 +1045,14 @@ int infer_host_run(dte_engine* e, const unsigned char* h_tuples, size_t n, unsig
     if (e->part == Part::Chunked) {
         Dev& h = host_dev(e);
         h.sink_lb = h_labels;
-        if (h.walk == Walk::Leaf) {                      // ring position r owns columns [sum of T before r, + T_r)
+        if (kind(h.walk).sharded == Sharded::Columns) {  // ring position r owns the columns after those of positions < r
             size_t pitch = 0, off = 0;
-            for (const Dev& d : e->devs) pitch += row_bytes(d, Walk::Leaf);
+            for (const Dev& d : e->devs) pitch += row_bytes(d, h.walk);
             for (size_t r = 0; r < e->devs.size(); ++r) {
                 Dev& d = e->devs[(size_t)e->pos2dev[r]];
                 d.sink = h_out + off;
                 d.sink_pitch = pitch;
-                off += row_bytes(d, Walk::Leaf);
+                off += row_bytes(d, h.walk);
             }
         } else {                                         // the scores are combined on the host device
             h.sink = h_out;
@@ -1156,10 +1135,10 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
     if (fragment_pending(e)) return fail(e, DTE_ERR_STATE, "a partial tuple is pending in the line stream");
     TRY(drain_all(e));
     if (e->multi()) TRY(decide_partition(e, g));
-    // the contributions (interactions) of a tree chunk are fp64 partials: combining them in ring order is not offered
-    if ((w == Walk::Contrib || w == Walk::Inter || w == Walk::Approx) && e->part == Part::Chunked)
+    const WalkKind& k = kind(w);
+    if (k.sharded == Sharded::Refuse && e->part == Part::Chunked)
         return fail(e, DTE_ERR_CONFIG, "%s: an ensemble-sharded handle cannot return %s; use a single-device or data-sharded handle", what,
-                    w == Walk::Inter ? "interaction values" : "contributions");
+                    k.sharded_noun);
     TRY(check_resident(e, g, w));
     if (n == 0) return DTE_OK;
     e->g = g;
@@ -1167,7 +1146,7 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
         if (d.cap_tuples && d.slot[d.cur].fill) advance_slot(d);
     const uint32_t F = g.F();
     size_t cap = default_chunk(e, F);
-    if (row_walk(w)) {
+    if (k.rows) {
         // The rows of a slot (2T bytes per tuple for leaf cells, 4 C (F + 1) for contributions: 2 MiB at C = 256,
         // F = 2048, 4 C (F + 1)^2 for interactions: at most 64 MiB) may take at most twice the tuple budget, so a
         // many-tree or many-feature ensemble lands fewer tuples per slot instead of allocating GiBs of rows; every slot
@@ -1178,7 +1157,7 @@ int infer_host(dte_engine* e, Walk w, const char* what, const unsigned char* h_t
         cap = std::min(cap, std::max<size_t>(4, budget / row) & ~(size_t)3);
     }
     for (Dev& d : e->devs) TRY(ensure_slots(e, d, cap, F, e->part == Part::Chunked, d.shape.C));
-    if (row_walk(w))
+    if (k.rows)
         for (Dev& d : e->devs) TRY(ensure_row_slots(e, d, w));
     if (sp) {                                        // every chunk is a slot: the scratch holds the largest one's entries
         size_t nnz = 0;
@@ -1820,13 +1799,10 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
     // the tile kernels read tuple rows as 16-byte vectors, every score walk stores 4-byte words and the leaf walk stores
     // the cells of a row in pieces of up to 16 bytes: a misaligned pointer would fault the walk and leave the caller's
     // CUDA context unusable, so it is refused here
-    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u)
-        return fail(e, DTE_ERR_ARG, "%s: %s not 16-byte aligned", what, w == Walk::Binned ? "d_bins" : "d_tuples");
-    const int align = w == Walk::Leaf ? 16 : 4;
-    if (reinterpret_cast<uintptr_t>(out) & (align - 1))
-        return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what,
-                    w == Walk::Leaf ? "d_leaves" : w == Walk::Contrib || w == Walk::Approx ? "d_contribs" : w == Walk::Inter ? "d_inter"
-                    : accumulate ? "d_scores_accum" : "d_scores", align);
+    const WalkKind& k = kind(w);
+    if (reinterpret_cast<uintptr_t>(d_tuples) & 15u) return fail(e, DTE_ERR_ARG, "%s: %s not 16-byte aligned", what, k.in_arg);
+    if (reinterpret_cast<uintptr_t>(out) & (k.out_align - 1))
+        return fail(e, DTE_ERR_ARG, "%s: %s not %d-byte aligned", what, accumulate ? "d_scores_accum" : k.out_arg, k.out_align);
     TRY(single_only(e, what));
     Geom g;
     TRY(decode_geom(e, g));
@@ -1848,11 +1824,8 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
 // the kernel and plan the next walk of kind w would launch
 static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
-    if (const char* why = missing_layout(e->devs[0], w)) return fail(e, DTE_ERR_STATE, "%s", why);
-    if (w == Walk::Contrib) contrib_kernel_name(e->devs[0], e->forced_variant, buf, len);
-    else if (w == Walk::Inter) inter_kernel_name(e->devs[0], e->opt_inter_block, buf, len);
-    else if (w == Walk::Approx) approx_kernel_name(e->devs[0], e->tune, e->forced_variant, buf, len);
-    else kernel_name(e->devs[0], walk_tune(e, w), e->forced_variant, buf, len, w);
+    if (!e->devs[0].layout.resident(w)) return fail(e, DTE_ERR_STATE, "%s", kind(w).missing);
+    kind_kernel_name(e->devs[0], w, walk_tune(e, w), e->forced_variant, e->opt_inter_block, buf, len);
     return DTE_OK;
 }
 
@@ -1938,7 +1911,7 @@ int dte_bin_tuples_device(dte_t* e, const void* d_tuples, size_t n, uint8_t* d_b
 
 int dte_bin_edges(dte_t* e, uint32_t* offsets, uint32_t* edges, size_t cap, size_t* total) {
     if (!e || !offsets || !total) return DTE_ERR_ARG;
-    if (e->bins.offsets.empty()) return fail(e, DTE_ERR_STATE, "no binned layout resident: load the ensemble with dte_load_ensemble_binned");
+    if (e->bins.offsets.empty()) return fail(e, DTE_ERR_STATE, "%s", kind(Walk::Binned).missing);
     const std::vector<uint32_t>& o = e->bins.offsets;
     *total = e->bins.edges.size();
     std::copy(o.begin(), o.end(), offsets);

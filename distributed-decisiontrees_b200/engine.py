@@ -383,6 +383,19 @@ class Engine:
         self._check(fn(self._h, _ptr(t), n, _ptr(scores), _ptr(labels)))
         return scores, labels
 
+    def _infer_host_rows(self, fn, tuples, out, row_shape, dtype=np.float32):
+        """Run a host-buffer row call of fp32 tuples [n, F] into out, else into a new array [n, *row_shape()] -> out."""
+        t, n = _host_rows(tuples)
+        if out is None:
+            out = np.empty((n,) + row_shape(), dtype=dtype)
+        self._check(fn(self._h, _ptr(t), n, _ptr(out)))
+        return out
+
+    def _attribution_row(self, axes):
+        """The row shape of an attribution call: `axes` axes of F + 1, after a class axis for a multi-class ensemble."""
+        F1, nc = int(self.info()["num_features"]) + 1, self.num_classes()
+        return (F1,) * axes if nc == 1 else (nc,) + (F1,) * axes
+
     def _name(self, fn):
         buf = C.create_string_buffer(256)
         self._check(fn(self._h, buf, 256))
@@ -429,10 +442,8 @@ class Engine:
     def infer_host_leaves(self, tuples, out=None):
         """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> [n, T] uint16: the cell, in tree t's
         own weight heap, of the leaf that local tree t sends each tuple to (T = info()["num_trees"])."""
-        t, n = _host_rows(tuples)
-        leaves = out if out is not None else np.empty((n, int(self.info()["num_trees"])), dtype=np.uint16)
-        self._check(self._lib.dte_infer_host_leaves(self._h, _ptr(t), n, _ptr(leaves)))
-        return leaves
+        return self._infer_host_rows(self._lib.dte_infer_host_leaves, tuples, out, lambda: (int(self.info()["num_trees"]),),
+                                     np.uint16)
 
     def kernel_name_leaves(self):
         return self._name(self._lib.dte_kernel_name_leaves)
@@ -446,12 +457,7 @@ class Engine:
     def infer_host_contribs(self, tuples, out=None):
         """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> contributions [n, F + 1] for a
         single-class ensemble, [n, C, F + 1] for a C-class one: feature f's share of the class score, the bias last."""
-        t, n = _host_rows(tuples)
-        F, nc = int(self.info()["num_features"]), self.num_classes()
-        if out is None:
-            out = np.empty((n, F + 1) if nc == 1 else (n, nc, F + 1), dtype=np.float32)
-        self._check(self._lib.dte_infer_host_contribs(self._h, _ptr(t), n, _ptr(out)))
-        return out
+        return self._infer_host_rows(self._lib.dte_infer_host_contribs, tuples, out, lambda: self._attribution_row(1))
 
     def kernel_name_contribs(self):
         return self._name(self._lib.dte_kernel_name_contribs)
@@ -467,12 +473,7 @@ class Engine:
         """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> approximate contributions [n, F + 1] for
         a single-class ensemble, [n, C, F + 1] for a C-class one: the change in expected score each feature's splits
         make along the tuple's path, the bias (the trees' expected score) last."""
-        t, n = _host_rows(tuples)
-        F, nc = int(self.info()["num_features"]), self.num_classes()
-        if out is None:
-            out = np.empty((n, F + 1) if nc == 1 else (n, nc, F + 1), dtype=np.float32)
-        self._check(self._lib.dte_infer_host_approx_contribs(self._h, _ptr(t), n, _ptr(out)))
-        return out
+        return self._infer_host_rows(self._lib.dte_infer_host_approx_contribs, tuples, out, lambda: self._attribution_row(1))
 
     def kernel_name_approx_contribs(self):
         return self._name(self._lib.dte_kernel_name_approx_contribs)
@@ -487,12 +488,7 @@ class Engine:
         """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> interaction values [n, F + 1, F + 1] for
         a single-class ensemble, [n, C, F + 1, F + 1] for a C-class one: row f sums to feature f's contribution, [F, F] is
         the bias."""
-        t, n = _host_rows(tuples)
-        F, nc = int(self.info()["num_features"]), self.num_classes()
-        if out is None:
-            out = np.empty((n, F + 1, F + 1) if nc == 1 else (n, nc, F + 1, F + 1), dtype=np.float32)
-        self._check(self._lib.dte_infer_host_interactions(self._h, _ptr(t), n, _ptr(out)))
-        return out
+        return self._infer_host_rows(self._lib.dte_infer_host_interactions, tuples, out, lambda: self._attribution_row(2))
 
     def kernel_name_interactions(self):
         return self._name(self._lib.dte_kernel_name_interactions)
