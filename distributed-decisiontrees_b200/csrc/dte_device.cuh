@@ -6,6 +6,7 @@
 #include "dte_kernels.cuh"
 #include "dte_shap.cuh"
 #include "dte_approx.cuh"
+#include "dte_interv.cuh"
 
 #include <algorithm>
 #include <array>
@@ -27,9 +28,9 @@ constexpr int kNumSlots = 3;          // landing slots per device: H2D of i+1, w
 enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED = 3 };
 
 // What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), the leaf cell every
-// tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12), interaction values (DESIGN.md §13)
-// or the approximate feature contributions (DESIGN.md §14)
-enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx };
+// tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12), interaction values (DESIGN.md §13),
+// the approximate feature contributions (DESIGN.md §14) or the interventional contributions (DESIGN.md §15)
+enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx, Interv };
 
 // How an ensemble-sharded handle returns a walk's results: the ring positions' partials combined in ring order, each
 // position's rows in its own columns of the caller's rows, or refused (fp64 attribution partials are never combined).
@@ -63,6 +64,9 @@ inline constexpr WalkKind kWalkKinds[] = {
     {4, "d_tuples", "d_contribs", 4, true,
      "no approximate-contribution table resident: load the ensemble with dte_load_ensemble_approx_contribs", true, false,
      Sharded::Refuse, "contributions", "approximate-contribution walk"},
+    {4, "d_tuples", "d_contribs", 4, true,
+     "no interventional layout resident: load the ensemble with dte_load_ensemble_interventional", true, false,
+     Sharded::Refuse, "contributions", "interventional contribution walk"},
 };
 inline const WalkKind& kind(Walk w) { return kWalkKinds[static_cast<int>(w)]; }
 
@@ -189,6 +193,8 @@ inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& liv
 //   +24  u16    feat[Dmax]   feature of each element
 //   +zoff double z[Dmax]     zero fraction of each element
 //   +izoff double iz[Dmax]   1 / z of each element (read only where z > 1, by the bottom-up unwinding)
+// The path part alone (built without covers, for the interventional walk, DESIGN.md §15) has no fraction words: bz = 0,
+// zoff = izoff = 0 and stride = roundup16(24 + 2 Dmax).
 // Nodes: per layout tree [2^D - 1] {thr word, fidx | missing_right << 16}; only the ancestors of end cells are read.
 struct ShapLayout {
     uint32_t D = 0, M = 0;               // levels; longest merged path of the layout
@@ -216,8 +222,9 @@ inline bool cover_refused(const float* cov, uint32_t tree, uint32_t cell, std::s
 
 // Builds the contribution layout of trees [first, first + count) of the streams (count = 0 with first = 0: all), class
 // of tree s = s % classes.  covers: fp32 [T_all][2^(D+1) - 1], indexed like the weight heap.  Only live internal nodes
-// and reachable end cells are read; each must be finite and > 0.  Returns 0, -1 (bad covers or streams; msg names the
-// tree and cell) or -4 (a feature index >= F).
+// and reachable end cells are read; each must be finite and > 0.  covers == nullptr: the path part only (no fraction
+// words, no cover checks).  Returns 0, -1 (bad covers or streams; msg names the tree and cell) or -4 (a feature index
+// >= F).
 inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_cls, const unsigned char* wl, size_t n_wl,
                              const unsigned char* fl, size_t n_fl, const float* covers, uint32_t first, uint32_t count,
                              uint32_t classes, ShapLayout& out, std::string& msg) {
@@ -235,9 +242,13 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
     const uint16_t* Fall = reinterpret_cast<const uint16_t*>(fl);
     out = ShapLayout();
     out.D = D; out.C = classes; out.n_nodes = n_int;
-    out.zoff = (24u + 2u * D + 7u) & ~7u;
-    out.izoff = out.zoff + 8u * D;
-    out.stride = (out.izoff + 8u * D + 15u) & ~15u;
+    if (covers) {
+        out.zoff = (24u + 2u * D + 7u) & ~7u;
+        out.izoff = out.zoff + 8u * D;
+        out.stride = (out.izoff + 8u * D + 15u) & ~15u;
+    } else {
+        out.stride = (24u + 2u * D + 15u) & ~15u;
+    }
     std::vector<uint32_t> order;                     // layout tree -> local tree, class-major
     out.cls_tree.assign(classes + 1, 0);
     for (uint32_t c = 0; c < classes; ++c) {
@@ -256,9 +267,9 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
         const uint32_t s = first + order[k];
         const uint32_t* W = Wall + (size_t)s * wstride;
         const uint16_t* FI = Fall + (size_t)s * fstride;
-        const float* cov = covers + (size_t)s * n_all;
+        const float* cov = covers ? covers + (size_t)s * n_all : nullptr;
         live_nodes(FI, D, live);
-        auto bad_cover = [&](uint32_t cell) { return cover_refused(cov, s, cell, msg); };
+        auto bad_cover = [&](uint32_t cell) { return cov && cover_refused(cov, s, cell, msg); };
         cells.clear();
         for (uint32_t i = 0; i < n_int; ++i) {
             out.nodes[(size_t)k * n_int + i] = make_uint2(W[i], (FI[i] & 0x7FFu) | (uint32_t)((FI[i] >> 13) & 1u) << 16);
@@ -283,7 +294,7 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
             for (uint32_t st = 0; st < L; ++st) {
                 const uint32_t node = st ? anc[L - st] : 0, child = anc[L - 1 - st];
                 const uint32_t f = FI[node] & 0x7FFu;
-                const double frac = (double)cov[child] / (double)cov[node];
+                const double frac = cov ? (double)cov[child] / (double)cov[node] : 1.0;
                 uint32_t e = 0;
                 while (e < m && efeat[e] != f) ++e;
                 if (e == m) { efeat[m] = f; ez[m] = frac; ++m; }
@@ -294,7 +305,7 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
             memcpy(&v, &W[cell], 4);
             double zp = ez[0];
             for (uint32_t e = 1; e < m; ++e) zp = zp * ez[e];
-            const double bz = (double)v * zp;
+            const double bz = cov ? (double)v * zp : 0.0;
             unsigned char* r = out.paths.data() + (p0 + q) * out.stride;
             const uint32_t meta = cell | m << 16 | L << 24;
             memcpy(r, &bz, 8);
@@ -304,6 +315,7 @@ inline int build_shap_layout(uint32_t D, uint32_t F, uint32_t w_cls, uint32_t f_
             for (uint32_t e = 0; e < m; ++e) {
                 const uint16_t f16 = (uint16_t)efeat[e];
                 memcpy(r + 24 + 2 * e, &f16, 2);
+                if (!cov) continue;
                 const double iz = 1.0 / ez[e];
                 memcpy(r + out.zoff + 8 * e, &ez[e], 8);
                 memcpy(r + out.izoff + 8 * e, &iz, 8);
@@ -717,6 +729,10 @@ struct ResidentLayout {
     DevArray<unsigned char> shap_paths;
     DevArray<unsigned long long> shap_tree_path;
     DevArray<uint32_t> shap_cls_tree;
+    // interventional layout (dte_load_ensemble_interventional only, DESIGN.md §15): the shap_* arrays above built without
+    // covers (the path part of a ShapLayout), and the background rows [N][F]
+    DevArray<uint32_t> background;
+    uint64_t background_rows = 0;
     // approximate-contribution table (dte_load_ensemble_approx_contribs only, DESIGN.md §14): an ApproxLayout's arrays
     DevArray<double> approx_delta;
     DevArray<uint16_t> approx_feat;
@@ -725,7 +741,7 @@ struct ResidentLayout {
     size_t bytes() const {
         return top.bytes() + top_split.bytes() + bottom.bytes() + top_b.bytes() + bottom_b.bytes() + bottom_id.bytes() +
                shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes() +
-               approx_delta.bytes() + approx_feat.bytes();
+               approx_delta.bytes() + approx_feat.bytes() + background.bytes();
     }
     // whether the layout a walk of kind w reads is resident
     bool resident(Walk w) const {
@@ -734,8 +750,9 @@ struct ResidentLayout {
             case Walk::Binned: return top_b;
             case Walk::Leaf: return bottom_id;
             case Walk::Contrib:
-            case Walk::Inter: return shap_paths;
+            case Walk::Inter: return shap_paths && !background;
             case Walk::Approx: return approx_delta;
+            case Walk::Interv: return background;
         }
         return false;
     }
@@ -818,10 +835,10 @@ struct Dev {
 };
 
 // Bytes of one tuple's result row of a walk of kind w on device d: slot_C score words, T leaf cells of 2 bytes,
-// C (F + 1) contribution words (exact or approximate) or C (F + 1)^2 interaction words
+// C (F + 1) contribution words (exact, approximate or interventional) or C (F + 1)^2 interaction words
 inline size_t row_bytes(const Dev& d, Walk w) {
     if (w == Walk::Leaf) return 2 * (size_t)d.shape.T;
-    if (w == Walk::Contrib || w == Walk::Approx) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
+    if (w == Walk::Contrib || w == Walk::Approx || w == Walk::Interv) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1);
     if (w == Walk::Inter) return 4 * (size_t)d.shape.C * (d.shape.g.F() + 1) * (d.shape.g.F() + 1);
     return 4 * (size_t)d.slot_C;
 }
@@ -1392,6 +1409,42 @@ inline cudaError_t launch_approx(Dev& d, const Geom& run, const Tune& tune, int 
     });
 }
 
+// ---- interventional contributions (DESIGN.md §15) ----
+using IntervKernel = void (*)(IntervParams);
+inline IntervKernel interv_kernel(int bound) {
+    return bound == 3 ? dt_shap_interv<3> : bound == 7 ? dt_shap_interv<7> : dt_shap_interv<15>;
+}
+
+// Launch the interventional walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident path
+// layout and background rows: d_out [n][C][F + 1], the trees as launch_contrib's.  dt_shap_interv<shap_bound> runs in
+// launches of at most kShapScratchBytes / (8 (F + 1)) tuples through the device's fp64 scratch, as dt_shap_generic does.
+// Returns a cudaError_t.
+inline cudaError_t launch_interv(Dev& d, const Geom& run, const void* d_tuples, size_t n, float* d_out, cudaStream_t st,
+                                 const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const uint32_t F = d.shape.g.F(), C = d.shape.C;
+    IntervParams ip = {};
+    ShapParams& p = ip.s;
+    p = shap_params(d, run);
+    ip.bg = d.layout.background;
+    ip.N = d.layout.background_rows;
+    const IntervKernel k = interv_kernel(shap_bound(d));
+    const uint32_t* tuples = static_cast<const uint32_t*>(d_tuples);
+    const size_t row_words = (size_t)C * (F + 1);
+    const size_t cap = std::max<size_t>(32, (kShapScratchBytes / ((size_t)(F + 1) * 8)) & ~(size_t)31);
+    const size_t rows = std::min(cap, (n + 31) & ~(size_t)31);
+    p.scratch_rows = rows;
+    return scratch_chunks(d, n, rows, rows * (F + 1), st, [&](double* scratch, size_t off, size_t m) {
+        p.scratch = scratch;
+        p.n = m;
+        p.tuples = tuples + off * F;
+        p.out = d_out + off * row_words;
+        k<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(ip);
+        return launched(d);
+    });
+}
+
 // ---- every kind of walk (kWalkKinds) ----
 // Launch the walk of kind w over n tuples on device d (cudaSetDevice already done) with the engine's knobs: the walk
 // tune, the forced variant `want` and the interaction block.  `out` receives n rows of row_bytes; labels and accumulate
@@ -1404,6 +1457,7 @@ inline cudaError_t launch_kind(Dev& d, Walk w, const Geom& run, const Tune& tune
         case Walk::Contrib: return launch_contrib(d, run, want, tuples, n, static_cast<float*>(out), st, why);
         case Walk::Inter: return launch_inter(d, run, inter_block, tuples, n, static_cast<float*>(out), st, why);
         case Walk::Approx: return launch_approx(d, run, tune, want, tuples, n, static_cast<float*>(out), st, why);
+        case Walk::Interv: return launch_interv(d, run, tuples, n, static_cast<float*>(out), st, why);
         default: return launch_walk(d, run, tune, want, tuples, n, static_cast<float*>(out), labels, st, accumulate, why, w);
     }
 }
@@ -1419,6 +1473,9 @@ inline void kind_kernel_name(const Dev& d, Walk w, const Tune& tune, int want, u
             if (used < len) snprintf(buf + used, len - used, " + dt_approx_generic");
             return;
         }
+        case Walk::Interv:                             // one kernel: a forced variant does not apply
+            snprintf(buf, len, "dt_shap_interv<%d>", shap_bound(d));
+            return name_classes(d, buf, len);
         default: return kernel_name(d, tune, want, buf, len, w);
     }
 }

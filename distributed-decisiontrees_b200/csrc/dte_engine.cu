@@ -325,10 +325,11 @@ int upload(dte_engine* e, DevArray<T>& dst, const std::vector<T>& src) {
 }
 
 // `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr.  `shap`: the contribution
-// layout of a dte_load_ensemble_contribs, else nullptr.  `approx`: the table of a dte_load_ensemble_approx_contribs, else
-// nullptr.  The old ensemble is dropped before the new one is allocated.
+// layout of a dte_load_ensemble_contribs, or the path layout of a dte_load_ensemble_interventional, else nullptr.
+// `approx`: the table of a dte_load_ensemble_approx_contribs, else nullptr.  `bg`: the background rows [bg_rows][F] of a
+// dte_load_ensemble_interventional, else nullptr.  The old ensemble is dropped before the new one is allocated.
 int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap,
-                    const ApproxLayout* approx) {
+                    const ApproxLayout* approx, const std::vector<uint32_t>* bg, uint64_t bg_rows) {
     CUDA_TRY(e, free_ensemble(d));
     ResidentLayout& lay = d.layout;
     TRY(upload(e, lay.top, pk.top));
@@ -360,6 +361,10 @@ int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEd
         lay.approx_cell_stride = approx->cell_stride();
         lay.approx_node_stride = approx->node_stride();
     }
+    if (bg) {
+        TRY(upload(e, lay.background, *bg));
+        lay.background_rows = bg_rows;
+    }
     return DTE_OK;
 }
 
@@ -378,17 +383,25 @@ struct TreeShare {
 // resident leaf-id layout is dropped.  `covers` (fp32 [T_all][2^(D+1)-1] for the trees of the streams): also build and
 // upload the contribution layout of every share; without it any resident contribution layout is dropped.  `approx`
 // with covers: build the approximate-contribution table and the leaf-id layout instead of the contribution layout.
-// Every placement drops the resident layouts it does not build.
+// `background` (fp32 words [n_background][F]), without covers: build the path part of the contribution layout and upload
+// it with the background rows (the interventional layout).  Every placement drops the resident layouts it does not build.
 // All or nothing: every share is built and checked before any device changes, so a refused share leaves the previous
 // ensemble resident everywhere; a failed upload leaves no ensemble on any device rather than a mix of two.
 int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr,
-                   const float* covers = nullptr, bool approx = false) {
+                   const float* covers = nullptr, bool approx = false, const void* background = nullptr,
+                   size_t n_background = 0) {
     const bool chunked = e->part == Part::Chunked;
     const size_t n_shares = chunked ? e->devs.size() : 1;
-    const bool with_shap = covers && !approx, with_approx = covers && approx;
+    const bool with_bg = background && !covers;
+    const bool with_shap = (covers && !approx) || with_bg, with_approx = covers && approx;
     std::vector<ShapLayout> shap(with_shap ? n_shares : 0);
     std::vector<ApproxLayout> apx(with_approx ? n_shares : 0);
     std::vector<PackedEnsemble> pk(n_shares);
+    std::vector<uint32_t> bg;
+    if (with_bg) {
+        const uint32_t* b = static_cast<const uint32_t*>(background);
+        bg.assign(b, b + n_background * g.F());
+    }
     for (size_t r = 0; r < n_shares; ++r) {
         const TreeShare& s = share[r];
         std::string msg;
@@ -402,7 +415,7 @@ int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_
     for (size_t r = 0; r < e->devs.size(); ++r) {
         const size_t s = chunked ? r : 0;
         const int rc = upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk[s], bins, with_shap ? &shap[s] : nullptr,
-                                       with_approx ? &apx[s] : nullptr);
+                                       with_approx ? &apx[s] : nullptr, with_bg ? &bg : nullptr, n_background);
         if (rc) {
             for (Dev& d : e->devs) free_ensemble(d);
             e->placed.reset();
@@ -1717,10 +1730,11 @@ static int choose_measured_plan(dte_t* e) {
 
 // dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
 // is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs, or with `approx`
-// dte_load_ensemble_approx_contribs.
+// dte_load_ensemble_approx_contribs.  `background`: dte_load_ensemble_interventional.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
                          uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins,
-                         const float* covers = nullptr, bool approx = false) {
+                         const float* covers = nullptr, bool approx = false, const void* background = nullptr,
+                         size_t n_background = 0) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1754,7 +1768,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers, approx));
+    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers, approx, background, n_background));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
@@ -1785,6 +1799,18 @@ int dte_load_ensemble_approx_contribs(dte_t* e, const void* weight_cls, size_t n
     if (!covers) return e ? fail(e, DTE_ERR_ARG, "dte_load_ensemble_approx_contribs: covers is NULL") : DTE_ERR_ARG;
     return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
                          covers, true);
+}
+
+int dte_load_ensemble_interventional(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                                     size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes,
+                                     const void* background, size_t n_background) {
+    if (!e) return DTE_ERR_ARG;
+    if (!background || !n_background)
+        return fail(e, DTE_ERR_ARG, "dte_load_ensemble_interventional: %s", background ? "n_background is 0" : "background is NULL");
+    if (n_background > 0xFFFFFFFFull)     // every K of DESIGN.md §15 stays below 2^53
+        return fail(e, DTE_ERR_ARG, "dte_load_ensemble_interventional: %zu background rows, at most 2^32 - 1", n_background);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
+                         nullptr, false, background, n_background);
 }
 
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1962,6 +1988,20 @@ int dte_infer_host_approx_contribs(dte_t* e, const void* h_tuples, size_t n, flo
 }
 
 int dte_kernel_name_approx_contribs(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Approx, buf, len); }
+
+// ---- interventional contributions (DESIGN.md §15) ----
+int dte_infer_device_interventional(dte_t* e, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_contribs))) return DTE_ERR_ARG;
+    return infer_device(e, Walk::Interv, "dte_infer_device_interventional", d_tuples, n, d_contribs, nullptr, cuda_stream);
+}
+
+int dte_infer_host_interventional(dte_t* e, const void* h_tuples, size_t n, float* h_contribs) {
+    if (!e || (n && (!h_tuples || !h_contribs))) return DTE_ERR_ARG;
+    return infer_host(e, Walk::Interv, "infer_host_interventional", static_cast<const unsigned char*>(h_tuples), n, h_contribs,
+                      nullptr);
+}
+
+int dte_kernel_name_interventional(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Interv, buf, len); }
 
 // ---- interaction values (DESIGN.md §13) ----
 int dte_infer_device_interactions(dte_t* e, const void* d_tuples, size_t n, float* d_inter, void* cuda_stream) {

@@ -79,6 +79,11 @@ ABI = [
     ("dte_infer_device_approx_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_approx_contribs", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("dte_kernel_name_approx_contribs", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_load_ensemble_interventional", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                   C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t]),
+    ("dte_infer_device_interventional", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_interventional", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_kernel_name_interventional", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
     ("dte_sparse_to_dense_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
                                              C.c_void_p, C.c_void_p]),
     ("dte_infer_device_sparse", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p,
@@ -240,6 +245,8 @@ class Engine:
         if int(addr) == 200 and int(data) & 1:
             self._classes = None                         # `start`: a tree stream may place a new ensemble
         self._check(self._lib.dte_softreg_write(self._h, int(addr), int(data) & 0xFFFFFFFFFFFFFFFF))
+        self._written = getattr(self, "_written", {})
+        self._written[int(addr)] = int(data) & 0xFFFFFFFFFFFFFFFF    # reads return status counters, not these words
 
     def softreg_read(self, addr):
         v = C.c_uint64()
@@ -312,7 +319,7 @@ class Engine:
 
     # -- fast paths -----------------------------------------------------------------------------
     def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False,
-                      leaves=False, covers=None, approx=False):
+                      leaves=False, covers=None, approx=False, background=None):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
         call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
         binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
@@ -321,7 +328,9 @@ class Engine:
         covers: fp32 [T_all, 2^(D+1)-1] node covers of every tree of the streams, indexed like the weight heap: also build
         the contribution layout the *_contribs calls walk (dte_load_ensemble_contribs; not with binned=True).
         approx=True (with covers): build the approximate-contribution table and the leaf-id layout instead, which the
-        *_approx_contribs and *_leaves calls walk (dte_load_ensemble_approx_contribs; not with binned=True)."""
+        *_approx_contribs and *_leaves calls walk (dte_load_ensemble_approx_contribs; not with binned=True).
+        background: [N, F] float32 (or uint32 words) background rows: build the interventional layout the *_interventional
+        calls walk (dte_load_ensemble_interventional; not with covers, approx=True or binned=True)."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
@@ -329,14 +338,29 @@ class Engine:
             saved = getattr(self, "_leaf_opt", 0)
             self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
             try:
-                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers, approx=approx)
+                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers, approx=approx,
+                                          background=background)
             finally:
                 self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
+        if background is not None and (covers is not None or approx or binned):
+            raise ValueError("background cannot be combined with covers, approx=True or binned=True: one attribution layout "
+                             "is resident at a time, and the interventional calls take fp32 tuples")
         if approx and binned:
             raise ValueError("approx and binned=True cannot be combined: the approximate contribution calls take fp32 tuples")
         if approx and covers is None:
             raise ValueError("approx=True needs covers: the table is built from the node covers")
-        if covers is not None:
+        if background is not None:
+            bg = np.asarray(background)
+            r204 = getattr(self, "_written", {}).get(204)
+            F = ((r204 >> 48) & 0xFFFF) * 4 if r204 is not None else None   # tuple lines of register 204, four words each
+            if bg.dtype not in (np.float32, np.uint32) or bg.ndim != 2 or F is None or bg.shape[1] != F:
+                raise ValueError("background must be a [N, F] float32 or uint32 array with F from register 204 (%s), "
+                                 "not %s %s" % (F if F is not None else "not written", bg.dtype, bg.shape))
+            bg = np.ascontiguousarray(bg).view(np.uint32)
+            self._check(self._lib.dte_load_ensemble_interventional(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
+                                                                   int(first_tree), int(num_local_trees), int(num_classes),
+                                                                   _ptr(bg), int(bg.shape[0])))
+        elif covers is not None:
             if binned:
                 raise ValueError("covers and binned=True cannot be combined: the contribution calls take fp32 tuples")
             cv = np.ascontiguousarray(covers, dtype=np.float32)
@@ -477,6 +501,22 @@ class Engine:
 
     def kernel_name_approx_contribs(self):
         return self._name(self._lib.dte_kernel_name_approx_contribs)
+
+    # -- interventional contributions (DESIGN.md §15) ------------------------------------------------
+    def infer_device_interventional(self, d_tuples, n, d_contribs, stream=None):
+        """[n, C, F + 1] fp32 interventional SHAP values (bias last) of fp32 tuples [n, F] against the background rows of the
+        load, both on the device (d_tuples 16-byte, d_contribs 4-byte aligned)."""
+        self._check(self._lib.dte_infer_device_interventional(self._h, _ptr(d_tuples), int(n), _ptr(d_contribs),
+                                                              _stream(stream)))
+
+    def infer_host_interventional(self, tuples, out=None):
+        """tuples: host array [n, F] fp32 (numpy, or a pinned torch CPU tensor) -> interventional contributions [n, F + 1]
+        for a single-class ensemble, [n, C, F + 1] for a C-class one: feature f's share of the score's distance from the
+        background mean, the bias (the mean score over the background rows) last."""
+        return self._infer_host_rows(self._lib.dte_infer_host_interventional, tuples, out, lambda: self._attribution_row(1))
+
+    def kernel_name_interventional(self):
+        return self._name(self._lib.dte_kernel_name_interventional)
 
     # -- interaction values (DESIGN.md §13) ------------------------------------------------------------
     def infer_device_interactions(self, d_tuples, n, d_inter, stream=None):

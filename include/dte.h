@@ -334,6 +334,47 @@ int dte_infer_host_approx_contribs(dte_t* engine, const void* h_tuples, size_t n
 /* "<leaf walk name> + dt_approx_generic"; DTE_ERR_STATE without the approximate-contribution table. */
 int dte_kernel_name_approx_contribs(dte_t* engine, char* buf, size_t len);
 
+/* ---- interventional contributions (DESIGN.md §15) --------------------------------------------- */
+/* Interventional TreeSHAP (shap's TreeExplainer(model, data=background), feature_perturbation="interventional"): each
+ * feature's share of a tuple's score against N background rows r_1..r_N.  No covers.  For tuple x and tree t the game is
+ * v_t(S) = mean_r f_t(z_S), z_S = x's features in S and r's elsewhere; f_t walks with the run's missing pattern (reg 205
+ * at the call, for tuples and background rows alike), int32 compare and bit 13.  phi[c][f] (f < F) sums the Shapley values
+ * of f over the class-c trees; phi[c][F] = mean_r sum_t f_t(r) (the bias).  Trees, classes, source-tree conventions,
+ * paths (one per reachable end cell, increasing cell) and elements (the path's features merged by first occurrence) are
+ * those of the contribution calls (§12).  Per path of m elements and leaf word v:
+ *   X = the tuple's mask (bit e: x takes the path's direction at every step of element e), R_r the same for row r;
+ *   r reaches the path when X | R_r covers the m bits; A = X & ~R_r, B = R_r & ~X, a = |A|, b = |B|;
+ *   G(a, b) = 360360 / (a * C(a + b, a)), an exact integer (360360 = lcm(1..15));
+ *   K_e = sum over reaching r of (e in A ? +G(a, b) : e in B ? -G(b, a) : 0), Kb = #{r : R_r = all m bits}.
+ * Per tuple and class, fp64 accumulators from +0: trees in stream order, a tree's paths in increasing end cell, for each
+ * element e in element order phi[f_e] = phi[f_e] + v * (double)K_e, then phi[F] = phi[F] + v * (double)Kb, every
+ * operation rounded on its own, no contraction (a term with K_e = 0 may be skipped: it changes no word).  Words:
+ * __double2float_rn(phi[f] / (double)(360360 N)) and __double2float_rn(phi[F] / (double)N).  Every K is an exact integer,
+ * so the words do not depend on the order the background rows are visited in.  Layout [n][C][F+1] fp32, bias last.
+ * Binned and sparse tuples are not taken: densify first (dte_sparse_to_dense_device). */
+/* dte_load_ensemble_classes (same placement: Dealt handles replicate, Chunked handles keep their ranges) plus the
+ * interventional layout: the path part of the contribution layout (no fractions) and the background rows, fp32 words
+ * [n_background][F] with F from register 204.  A NULL background, n_background = 0 or n_background > 2^32 - 1 returns
+ * DTE_ERR_ARG and a feature index >= F DTE_ERR_UNSUPPORTED, each before anything is uploaded (the resident ensemble
+ * stays).  It drops a resident contribution layout and approximate-contribution table; every other placement
+ * (dte_load_ensemble*, a tree line stream) drops the interventional layout, after which the calls below return
+ * DTE_ERR_STATE. */
+int dte_load_ensemble_interventional(dte_t* engine, const void* weight_cls, size_t n_weight_cls,
+                                     const void* findex_cls, size_t n_findex_cls, uint32_t first_tree,
+                                     uint32_t num_local_trees, uint32_t num_classes, const void* background,
+                                     size_t n_background);
+/* [n][C][F+1] interventional contributions of n fp32 tuples in device memory.  Single-device handles; stream as
+ * dte_infer_device.  d_tuples must be 16-byte aligned and d_contribs 4-byte aligned, else DTE_ERR_ARG before any launch.
+ * dt_shap_interv<M> runs in launches through the handle's fp64 scratch, as dt_shap_generic does; a forced kernel variant
+ * does not apply. */
+int dte_infer_device_interventional(dte_t* engine, const void* d_tuples, size_t n, float* d_contribs, void* cuda_stream);
+/* The same from host memory through the landing pipeline: single-device and data-sharded handles (rows in global tuple
+ * order).  An ensemble-sharded handle returns DTE_ERR_CONFIG. */
+int dte_infer_host_interventional(dte_t* engine, const void* h_tuples, size_t n, float* h_contribs);
+/* "dt_shap_interv<M>" (M = 3, 7 or 15, the smallest bound that holds the longest path; " classes=C" appended for C >= 2);
+ * DTE_ERR_STATE without the interventional layout. */
+int dte_kernel_name_interventional(dte_t* engine, char* buf, size_t len);
+
 /* ---- sparse tuples (DESIGN.md §11) ------------------------------------------------------------- */
 /* n tuples as CSR rows: indptr int64 [n + 1], indices uint32 [nnz] (feature numbers), values [nnz] 32-bit words (fp32 bit
  * patterns).  Row i's entries are k in [indptr[i], indptr[i+1]), indexing indices and values absolutely, so indptr[0]

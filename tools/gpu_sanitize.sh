@@ -85,6 +85,20 @@ for T in "tests/test_gpu_approx_contribs.py::test_depths_and_widths[D15-F4]" "te
   atag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
   run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_approx_${atag}.log"
 done
+# the interventional kernel: the <3>, <7> and <15> instantiations on leaf-wise deep trees, a ragged block of 32 background
+# rows and 1000 rows, two launches through the fp64 scratch at F = 2048, the ragged tail of a warp and three classes on a
+# tree chunk; synccheck and racecheck over the shared-memory G table its blocks fill before the __syncthreads
+for T in "tests/test_gpu_interventional.py::test_leafwise_bounds[D13-M3]" "tests/test_gpu_interventional.py::test_leafwise_bounds[D14-M7]" \
+         "tests/test_gpu_interventional.py::test_leafwise_bounds[D15-M15]" \
+         "tests/test_gpu_interventional.py::test_background_sizes[33]" "tests/test_gpu_interventional.py::test_background_sizes[1000]" \
+         tests/test_gpu_interventional.py::test_several_scratch_launches "tests/test_gpu_interventional.py::test_tuple_counts[33]" \
+         tests/test_gpu_interventional.py::test_classes_and_a_chunk; do
+  vtag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_interv_${vtag}.log"
+done
+T="tests/test_gpu_interventional.py::test_background_sizes[33]"
+run synccheck "" ""; mv "$OUT/sanitizer_synccheck_auto.log" "$OUT/sanitizer_synccheck_interv.log"
+run racecheck "" "--racecheck-report all"; mv "$OUT/sanitizer_racecheck_auto.log" "$OUT/sanitizer_racecheck_interv.log"
 # leaks: the C++ host (no torch caching allocator in the process) over a handle's whole life, create to destroy, on three
 # ring positions sharing one GPU, data- and ensemble-sharded, fed by the line stream and by the host fast path
 for mode in stream host; do
