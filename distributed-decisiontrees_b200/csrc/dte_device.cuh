@@ -36,8 +36,19 @@ enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx, Interv };
 // position's rows in its own columns of the caller's rows, or refused (fp64 attribution partials are never combined).
 enum class Sharded { Combine, Columns, Refuse };
 
-// What the engine needs to know about each kind of walk.  The rest is ResidentLayout::resident (whether the kind's
-// layout is resident), launch_kind and kind_kernel_name.
+// The layouts a placement can leave resident on a device (ResidentLayout::layouts): the base pack, which every placement
+// builds, and the optional layouts a load asks for (kLoadKinds).
+enum : uint32_t {
+    kBasePack = 1,          // top, top_split, bottom
+    kBinnedLayout = 2,      // top_b, bottom_b and the edge table (DESIGN.md §9)
+    kLeafIds = 4,           // bottom_id (DESIGN.md §10)
+    kPaths = 8,             // the path records and nodes of a ShapLayout (DESIGN.md §12, §15)
+    kPathFractions = 16,    // the paths' zero fractions, built from covers (DESIGN.md §12)
+    kApproxTable = 32,      // an ApproxLayout (DESIGN.md §14)
+    kBackground = 64,       // the background rows (DESIGN.md §15)
+};
+
+// What the engine needs to know about each kind of walk.  The rest is launch_kind and kind_kernel_name.
 struct WalkKind {
     uint32_t feature_bytes;   // input bytes per feature of a tuple: u8 bins or fp32 words
     const char* in_arg;       // the device call's input and output pointers, as its refusals name them
@@ -50,25 +61,36 @@ struct WalkKind {
     Sharded sharded;
     const char* sharded_noun; // Sharded::Refuse: what the refusal says the handle cannot return
     const char* label;        // names the walk in a failed launch
+    uint32_t needs;           // the layouts the walk reads
 };
 inline constexpr WalkKind kWalkKinds[] = {
-    {4, "d_tuples", "d_scores", 4, false, "no ensemble loaded", true, false, Sharded::Combine, nullptr, "walk kernel"},
+    {4, "d_tuples", "d_scores", 4, false, "no ensemble loaded", true, false, Sharded::Combine, nullptr, "walk kernel", kBasePack},
     {1, "d_bins", "d_scores", 4, false, "no binned layout resident: load the ensemble with dte_load_ensemble_binned", true,
-     false, Sharded::Combine, nullptr, "walk kernel"},
+     false, Sharded::Combine, nullptr, "walk kernel", kBinnedLayout},
     {4, "d_tuples", "d_leaves", 16, true, "no leaf-id layout resident: place the ensemble with DTE_OPT_LEAF_LAYOUT = 1", false,
-     false, Sharded::Columns, nullptr, "leaf walk"},
+     false, Sharded::Columns, nullptr, "leaf walk", kLeafIds},
     {4, "d_tuples", "d_contribs", 4, true, "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs",
-     true, false, Sharded::Refuse, "contributions", "contribution walk"},
+     true, false, Sharded::Refuse, "contributions", "contribution walk", kPaths | kPathFractions},
     {4, "d_tuples", "d_inter", 4, true, "no contribution layout resident: load the ensemble with dte_load_ensemble_contribs",
-     true, true, Sharded::Refuse, "interaction values", "interaction walk"},
+     true, true, Sharded::Refuse, "interaction values", "interaction walk", kPaths | kPathFractions},
     {4, "d_tuples", "d_contribs", 4, true,
      "no approximate-contribution table resident: load the ensemble with dte_load_ensemble_approx_contribs", true, false,
-     Sharded::Refuse, "contributions", "approximate-contribution walk"},
+     Sharded::Refuse, "contributions", "approximate-contribution walk", kApproxTable},
     {4, "d_tuples", "d_contribs", 4, true,
      "no interventional layout resident: load the ensemble with dte_load_ensemble_interventional", true, false,
-     Sharded::Refuse, "contributions", "interventional contribution walk"},
+     Sharded::Refuse, "contributions", "interventional contribution walk", kPaths | kBackground},
 };
 inline const WalkKind& kind(Walk w) { return kWalkKinds[static_cast<int>(w)]; }
+
+// What each kind of load builds besides the base pack.  The approximate contributions' first pass is the leaf walk, so
+// that load always builds the leaf ids; any load builds them when DTE_OPT_LEAF_LAYOUT = 1 at placement.
+enum Load : uint32_t {
+    kScoresLoad = 0,                            // dte_load_ensemble, dte_load_ensemble_classes, the tree line stream
+    kBinnedLoad = kBinnedLayout,                // dte_load_ensemble_binned
+    kContribLoad = kPaths | kPathFractions,     // dte_load_ensemble_contribs
+    kApproxLoad = kApproxTable | kLeafIds,      // dte_load_ensemble_approx_contribs
+    kIntervLoad = kPaths | kBackground,         // dte_load_ensemble_interventional
+};
 
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536,tops=6"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
@@ -176,6 +198,15 @@ struct BinEdges {
     }
 };
 
+// One load: the layouts it builds and the inputs they are built from.
+struct LoadRequest {
+    uint32_t layouts;                   // its Load, and kLeafIds once placement has read DTE_OPT_LEAF_LAYOUT
+    const float* covers = nullptr;      // kPathFractions, kApproxTable: fp32 [T_all][2^(D+1)-1]
+    const uint32_t* background = nullptr;   // kBackground: [n_background][F] words
+    uint64_t n_background = 0;
+    BinEdges bins = {};                 // kBinnedLayout: the edge table over every tree of the streams (bin_edges)
+};
+
 // Live nodes of one stream tree: not below an early leaf (those are unreachable; the node with bit 14 itself is live).
 // live[i] for the 2^D - 1 internal nodes of fi.
 inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& live) {
@@ -196,11 +227,13 @@ inline void live_nodes(const uint16_t* fi, uint32_t D, std::vector<uint8_t>& liv
 // The path part alone (built without covers, for the interventional walk, DESIGN.md §15) has no fraction words: bz = 0,
 // zoff = izoff = 0 and stride = roundup16(24 + 2 Dmax).
 // Nodes: per layout tree [2^D - 1] {thr word, fidx | missing_right << 16}; only the ancestors of end cells are read.
-struct ShapLayout {
+struct PathShape {
     uint32_t D = 0, M = 0;               // levels; longest merged path of the layout
     uint32_t stride = 0, zoff = 0, izoff = 0;   // bytes per path record, offsets of z and 1 / z in it
     uint32_t n_nodes = 0;                // 2^D - 1
     uint32_t C = 1;
+};
+struct ShapLayout : PathShape {
     std::vector<uint2> nodes;            // [Tl][n_nodes], layout trees class-major, stream order inside a class
     std::vector<unsigned long long> tree_path;   // [Tl + 1] first path of each layout tree
     std::vector<uint32_t> cls_tree;      // [C + 1] first layout tree of each class
@@ -711,51 +744,41 @@ struct Stream : Owned<cudaStream_t, StreamDestroy> {
     }
 };
 
-// The resident ensemble of one device, uploaded by upload_ensemble and dropped as one.  The arrays of a layout the load
-// did not build stay empty, so a walk's layout is resident when its first array is.
+// The resident ensemble of one device, uploaded by upload_share and dropped as one.  `layouts` records which layouts the
+// placement built; the arrays of every other layout stay empty.
 struct ResidentLayout {
+    uint32_t layouts = 0;
+    // base pack
     DevArray<uint2> top;
     DevArray<uint16_t> top_split;     // PackedEnsemble::top_split
     DevArray<uint4> bottom;
-    // binned layout (dte_load_ensemble_binned only): 4-byte tops, binned bottom records, the edge table (CSR)
+    // binned layout: 4-byte tops, binned bottom records, the edge table (CSR)
     DevArray<uint32_t> top_b;
     DevArray<uint4> bottom_b;
     DevArray<uint32_t> bin_off, bin_edges;
-    // leaf-id layout (DTE_OPT_LEAF_LAYOUT = 1 at placement): bottom records with stream cell indices as leaf words
+    // leaf ids: bottom records with stream cell indices as leaf words
     DevArray<uint4> bottom_id;
-    // contribution layout (dte_load_ensemble_contribs only, DESIGN.md §12): the device copy of a ShapLayout
-    ShapLayout shap;                  // its shape; the host vectors stay empty
+    // paths: a ShapLayout's shape and arrays, with or without the fraction words
+    PathShape shap;
     DevArray<uint2> shap_nodes;
     DevArray<unsigned char> shap_paths;
     DevArray<unsigned long long> shap_tree_path;
     DevArray<uint32_t> shap_cls_tree;
-    // interventional layout (dte_load_ensemble_interventional only, DESIGN.md §15): the shap_* arrays above built without
-    // covers (the path part of a ShapLayout), and the background rows [N][F]
-    DevArray<uint32_t> background;
-    uint64_t background_rows = 0;
-    // approximate-contribution table (dte_load_ensemble_approx_contribs only, DESIGN.md §14): an ApproxLayout's arrays
+    // approximate-contribution table: an ApproxLayout's arrays
     DevArray<double> approx_delta;
     DevArray<uint16_t> approx_feat;
     uint32_t approx_cell_stride = 0, approx_node_stride = 0;
+    // background rows [background_rows][F]
+    DevArray<uint32_t> background;
+    uint64_t background_rows = 0;
     // dte_info.ensemble_bytes: every array but the edge table
     size_t bytes() const {
         return top.bytes() + top_split.bytes() + bottom.bytes() + top_b.bytes() + bottom_b.bytes() + bottom_id.bytes() +
                shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes() +
                approx_delta.bytes() + approx_feat.bytes() + background.bytes();
     }
-    // whether the layout a walk of kind w reads is resident
-    bool resident(Walk w) const {
-        switch (w) {
-            case Walk::Fp32: return top;
-            case Walk::Binned: return top_b;
-            case Walk::Leaf: return bottom_id;
-            case Walk::Contrib:
-            case Walk::Inter: return shap_paths && !background;
-            case Walk::Approx: return approx_delta;
-            case Walk::Interv: return background;
-        }
-        return false;
-    }
+    // whether every layout a walk of kind w reads is resident
+    bool resident(Walk w) const { return (layouts & kind(w).needs) == kind(w).needs; }
 };
 
 // One landing slot: a device buffer the tuple stream lands in, plus the scores (labels) of its tuples.

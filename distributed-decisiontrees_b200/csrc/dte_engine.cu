@@ -324,47 +324,53 @@ int upload(dte_engine* e, DevArray<T>& dst, const std::vector<T>& src) {
     return DTE_OK;
 }
 
-// `bins`: the edge table of a binned load (pk then holds the binned layout too), else nullptr.  `shap`: the contribution
-// layout of a dte_load_ensemble_contribs, or the path layout of a dte_load_ensemble_interventional, else nullptr.
-// `approx`: the table of a dte_load_ensemble_approx_contribs, else nullptr.  `bg`: the background rows [bg_rows][F] of a
-// dte_load_ensemble_interventional, else nullptr.  The old ensemble is dropped before the new one is allocated.
-int upload_ensemble(dte_engine* e, Dev& d, const PackedEnsemble& pk, const BinEdges* bins, const ShapLayout* shap,
-                    const ApproxLayout* approx, const std::vector<uint32_t>* bg, uint64_t bg_rows) {
+// The layouts of one share, built on the host: the packed ensemble and, when the request asks for them, the paths or
+// the approximate-contribution table.
+struct ShareBuild {
+    PackedEnsemble pk;
+    ShapLayout paths;
+    ApproxLayout approx;
+};
+
+// Replace device d's ensemble with a share's build, the request's edge table and the background rows `bg` (one host
+// copy for every device): the device then holds exactly the layouts the request names.
+int upload_share(dte_engine* e, Dev& d, const LoadRequest& req, const ShareBuild& b, const std::vector<uint32_t>& bg) {
     CUDA_TRY(e, free_ensemble(d));
     ResidentLayout& lay = d.layout;
-    TRY(upload(e, lay.top, pk.top));
-    TRY(upload(e, lay.top_split, pk.top_split));
-    TRY(upload(e, lay.bottom, pk.bottom));
-    d.shape = pk.shape;
-    if (bins) {
-        TRY(upload(e, lay.top_b, pk.top_b));
-        TRY(upload(e, lay.bottom_b, pk.bottom_b));
-        TRY(upload(e, lay.bin_off, bins->offsets));
-        TRY(upload(e, lay.bin_edges, bins->edges));
+    TRY(upload(e, lay.top, b.pk.top));
+    TRY(upload(e, lay.top_split, b.pk.top_split));
+    TRY(upload(e, lay.bottom, b.pk.bottom));
+    d.shape = b.pk.shape;
+    if (req.layouts & kBinnedLayout) {
+        TRY(upload(e, lay.top_b, b.pk.top_b));
+        TRY(upload(e, lay.bottom_b, b.pk.bottom_b));
+        TRY(upload(e, lay.bin_off, req.bins.offsets));
+        TRY(upload(e, lay.bin_edges, req.bins.edges));
     }
-    if (!pk.bottom_id.empty()) TRY(upload(e, lay.bottom_id, pk.bottom_id));
-    if (shap) {
+    if (req.layouts & kLeafIds) TRY(upload(e, lay.bottom_id, b.pk.bottom_id));
+    if (req.layouts & kPathFractions) {
         double tab[4][kShapTab][kShapTab];
         shap_tables(tab);
         CUDA_TRY(e, cudaMemcpyToSymbol(c_shap_tab, tab, sizeof tab));
-        TRY(upload(e, lay.shap_nodes, shap->nodes));
-        TRY(upload(e, lay.shap_paths, shap->paths));
-        TRY(upload(e, lay.shap_tree_path, shap->tree_path));
-        TRY(upload(e, lay.shap_cls_tree, shap->cls_tree));
-        lay.shap.D = shap->D; lay.shap.M = shap->M; lay.shap.stride = shap->stride; lay.shap.zoff = shap->zoff;
-        lay.shap.izoff = shap->izoff;
-        lay.shap.n_nodes = shap->n_nodes; lay.shap.C = shap->C;
     }
-    if (approx) {
-        TRY(upload(e, lay.approx_delta, approx->delta));
-        TRY(upload(e, lay.approx_feat, approx->feat));
-        lay.approx_cell_stride = approx->cell_stride();
-        lay.approx_node_stride = approx->node_stride();
+    if (req.layouts & kPaths) {
+        TRY(upload(e, lay.shap_nodes, b.paths.nodes));
+        TRY(upload(e, lay.shap_paths, b.paths.paths));
+        TRY(upload(e, lay.shap_tree_path, b.paths.tree_path));
+        TRY(upload(e, lay.shap_cls_tree, b.paths.cls_tree));
+        lay.shap = b.paths;
     }
-    if (bg) {
-        TRY(upload(e, lay.background, *bg));
-        lay.background_rows = bg_rows;
+    if (req.layouts & kApproxTable) {
+        TRY(upload(e, lay.approx_delta, b.approx.delta));
+        TRY(upload(e, lay.approx_feat, b.approx.feat));
+        lay.approx_cell_stride = b.approx.cell_stride();
+        lay.approx_node_stride = b.approx.node_stride();
     }
+    if (req.layouts & kBackground) {
+        TRY(upload(e, lay.background, bg));
+        lay.background_rows = req.n_background;
+    }
+    lay.layouts = kBasePack | req.layouts;
     return DTE_OK;
 }
 
@@ -375,65 +381,53 @@ struct TreeShare {
     uint32_t first, count;
 };
 
+// Build share s for the request: the path or approximate-contribution builder first, then pack_ensemble, so the first
+// refusal is the one reported.
+int build_share(dte_engine* e, const Geom& g, const TreeShare& s, uint32_t classes, const LoadRequest& req, ShareBuild& out) {
+    const uint32_t has = req.layouts;
+    std::string msg;
+    int rc = has & kPaths ? build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl,
+                                              has & kPathFractions ? req.covers : nullptr, s.first, s.count, classes, out.paths, msg)
+           : has & kApproxTable ? build_approx_layout(g.D, g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, req.covers, s.first, s.count,
+                                                      out.approx, msg)
+                                : 0;
+    if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, out.pk, msg,
+                                has & kBinnedLayout ? &req.bins : nullptr, has & kLeafIds);
+    return rc ? fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str()) : DTE_OK;
+}
+
 // Place the ensemble for the run's partition: Chunked puts share[r] on the device of ring position r; every other
-// partition packs share[0] once and replicates it.  Records the placement for check_resident.  `classes` >= 2: every
+// partition builds share[0] once and replicates it.  Records the placement for check_resident.  `classes` >= 2: every
 // share is packed class-major, the class of a tree taken from its global stream index (share.first counts from the
-// start of the stream).  `bins`: also build and upload the binned layout with this edge table; without it any resident
-// binned layout is dropped.  With DTE_OPT_LEAF_LAYOUT the leaf-id layout is built and uploaded too; without it any
-// resident leaf-id layout is dropped.  `covers` (fp32 [T_all][2^(D+1)-1] for the trees of the streams): also build and
-// upload the contribution layout of every share; without it any resident contribution layout is dropped.  `approx`
-// with covers: build the approximate-contribution table and the leaf-id layout instead of the contribution layout.
-// `background` (fp32 words [n_background][F]), without covers: build the path part of the contribution layout and upload
-// it with the background rows (the interventional layout).  Every placement drops the resident layouts it does not build.
-// All or nothing: every share is built and checked before any device changes, so a refused share leaves the previous
-// ensemble resident everywhere; a failed upload leaves no ensemble on any device rather than a mix of two.
-int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, const BinEdges* bins = nullptr,
-                   const float* covers = nullptr, bool approx = false, const void* background = nullptr,
-                   size_t n_background = 0) {
+// start of the stream).  The request names the layouts to build besides the base pack; DTE_OPT_LEAF_LAYOUT adds the leaf
+// ids.  Every placement drops the resident layouts it does not build.  All or nothing: every share is built and checked
+// before any device changes, so a refused share leaves the previous ensemble resident everywhere; a failed upload leaves
+// no ensemble on any device rather than a mix of two.
+int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, LoadRequest& req) {
+    if (e->opt_leaf) req.layouts |= kLeafIds;
     const bool chunked = e->part == Part::Chunked;
-    const size_t n_shares = chunked ? e->devs.size() : 1;
-    const bool with_bg = background && !covers;
-    const bool with_shap = (covers && !approx) || with_bg, with_approx = covers && approx;
-    std::vector<ShapLayout> shap(with_shap ? n_shares : 0);
-    std::vector<ApproxLayout> apx(with_approx ? n_shares : 0);
-    std::vector<PackedEnsemble> pk(n_shares);
+    std::vector<ShareBuild> built(chunked ? e->devs.size() : 1);
+    for (size_t r = 0; r < built.size(); ++r) TRY(build_share(e, g, share[r], classes, req, built[r]));
     std::vector<uint32_t> bg;
-    if (with_bg) {
-        const uint32_t* b = static_cast<const uint32_t*>(background);
-        bg.assign(b, b + n_background * g.F());
+    if (req.layouts & kBackground) bg.assign(req.background, req.background + req.n_background * g.F());
+    int rc = DTE_OK;
+    for (size_t r = 0; r < e->devs.size() && !rc; ++r)
+        rc = upload_share(e, e->devs[(size_t)e->pos2dev[r]], req, built[chunked ? r : 0], bg);
+    if (rc) {
+        for (Dev& d : e->devs) free_ensemble(d);
+        e->placed.reset();
+    } else {
+        e->placed = e->part;
+        memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
     }
-    for (size_t r = 0; r < n_shares; ++r) {
-        const TreeShare& s = share[r];
-        std::string msg;
-        int rc = with_shap ? build_shap_layout(g.D, g.F(), g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count,
-                                               classes, shap[r], msg)
-               : with_approx ? build_approx_layout(g.D, g.w_cls, g.f_cls, s.wl, s.n_wl, s.fl, s.n_fl, covers, s.first, s.count, apx[r], msg)
-                             : 0;
-        if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, pk[r], msg, bins, e->opt_leaf || with_approx);
-        if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
-    }
-    for (size_t r = 0; r < e->devs.size(); ++r) {
-        const size_t s = chunked ? r : 0;
-        const int rc = upload_ensemble(e, e->devs[(size_t)e->pos2dev[r]], pk[s], bins, with_shap ? &shap[s] : nullptr,
-                                       with_approx ? &apx[s] : nullptr, with_bg ? &bg : nullptr, n_background);
-        if (rc) {
-            for (Dev& d : e->devs) free_ensemble(d);
-            e->placed.reset();
-            e->bins = BinEdges();
-            e->measured.reset();
-            return rc;
-        }
-    }
-    e->bins = bins ? *bins : BinEdges();
+    e->bins = rc ? BinEdges() : std::move(req.bins);       // the host mirror of the resident edge table
     e->measured.reset();              // a plan measured on the previous ensemble says nothing about this one
-    e->placed = e->part;
-    memcpy(e->prog_pos2dev, e->pos2dev, sizeof e->prog_pos2dev);
-    return DTE_OK;
+    return rc;
 }
 
 // Program the devices from the tree lines the receiver kept: all of them in entry 0 unless the stream was cut, then
 // entry r for ring position r (a single-device handle: the entry of its own node).
-int program_devices(dte_engine* e, const Geom& g) {
+int program_devices(dte_engine* e, const Geom& g, LoadRequest req) {
     const bool cut = decode_flags(e).cut_trees();
     TreeShare share[kMaxRing];
     const size_t n = e->part == Part::Chunked ? e->devs.size() : 1;
@@ -444,7 +438,7 @@ int program_devices(dte_engine* e, const Geom& g) {
                                           : fail(e, DTE_ERR_CONFIG, "node %u received no trees", e->node_index);
         share[r] = {e->tree_w[src].data(), e->tree_f[src].data(), lw, lf, 0, 0};
     }
-    return place_ensemble(e, g, share, 1);      // the reference's result stream carries one score per tuple
+    return place_ensemble(e, g, share, 1, req);      // the reference's result stream carries one score per tuple
 }
 
 // ---- landing slots ------------------------------------------------------------------------------
@@ -1293,7 +1287,7 @@ int receive_tree_lines(dte_engine* e, const unsigned char*& p, size_t& n_lines) 
     n_lines -= take;
     if (e->lines_received == total) {
         // prog_mode = (numcls_received < total_num_weights_cls), PCIeReceiver.sv:136-139
-        int rc = program_devices(e, e->g);
+        int rc = program_devices(e, e->g, {kScoresLoad});
         for (auto& v : e->tree_w) { v.clear(); v.shrink_to_fit(); }
         for (auto& v : e->tree_f) { v.clear(); v.shrink_to_fit(); }
         if (!rc) rc = prepare_data_phase(e);
@@ -1728,13 +1722,10 @@ static int choose_measured_plan(dte_t* e) {
     return DTE_OK;
 }
 
-// dte_load_ensemble_classes, and with `with_bins` dte_load_ensemble_binned: the edge table over every tree of the streams
-// is built, and refused, before anything is packed or uploaded.  `covers`: dte_load_ensemble_contribs, or with `approx`
-// dte_load_ensemble_approx_contribs.  `background`: dte_load_ensemble_interventional.
+// Every dte_load_ensemble* after its own argument checks.  A binned load's edge table over every tree of the streams is
+// built, and refused, before anything is packed or uploaded.
 static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls, size_t n_findex_cls,
-                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, bool with_bins,
-                         const float* covers = nullptr, bool approx = false, const void* background = nullptr,
-                         size_t n_background = 0) {
+                         uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes, LoadRequest req) {
     if (!e || !weight_cls || !findex_cls || !n_weight_cls || !n_findex_cls) return DTE_ERR_ARG;
     if (num_classes < 1 || num_classes > 256)            // the label is one byte
         return fail(e, DTE_ERR_ARG, "num_classes = %u, need 1..256", num_classes);
@@ -1744,10 +1735,9 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
     if (e->multi()) TRY(decide_partition(e, g));
     const unsigned char* wl = static_cast<const unsigned char*>(weight_cls);
     const unsigned char* fl = static_cast<const unsigned char*>(findex_cls);
-    BinEdges bins;
-    if (with_bins) {
+    if (req.layouts & kBinnedLayout) {
         std::string msg;
-        const int rc = bin_edges(g, wl, n_weight_cls, fl, n_findex_cls, bins, msg);
+        const int rc = bin_edges(g, wl, n_weight_cls, fl, n_findex_cls, req.bins, msg);
         if (rc) return fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str());
     }
     TreeShare share[kMaxRing];
@@ -1768,7 +1758,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
             share[r] = {wl, fl, n_weight_cls, n_findex_cls, first_tree + lo, hi - lo};
         }
     }
-    TRY(place_ensemble(e, g, share, num_classes, with_bins ? &bins : nullptr, covers, approx, background, n_background));
+    TRY(place_ensemble(e, g, share, num_classes, req));
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
@@ -1777,28 +1767,26 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
 
 int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                               size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
-    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, {kScoresLoad});
 }
 
 int dte_load_ensemble_binned(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                              size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes) {
-    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, true);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, {kBinnedLoad});
 }
 
 int dte_load_ensemble_contribs(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                                size_t n_findex_cls, const float* covers, uint32_t first_tree, uint32_t num_local_trees,
                                uint32_t num_classes) {
     if (!covers) return e ? fail(e, DTE_ERR_ARG, "dte_load_ensemble_contribs: covers is NULL") : DTE_ERR_ARG;
-    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
-                         covers);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, {kContribLoad, covers});
 }
 
 int dte_load_ensemble_approx_contribs(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
                                       size_t n_findex_cls, const float* covers, uint32_t first_tree, uint32_t num_local_trees,
                                       uint32_t num_classes) {
     if (!covers) return e ? fail(e, DTE_ERR_ARG, "dte_load_ensemble_approx_contribs: covers is NULL") : DTE_ERR_ARG;
-    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
-                         covers, true);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, {kApproxLoad, covers});
 }
 
 int dte_load_ensemble_interventional(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1809,8 +1797,8 @@ int dte_load_ensemble_interventional(dte_t* e, const void* weight_cls, size_t n_
         return fail(e, DTE_ERR_ARG, "dte_load_ensemble_interventional: %s", background ? "n_background is 0" : "background is NULL");
     if (n_background > 0xFFFFFFFFull)     // every K of DESIGN.md §15 stays below 2^53
         return fail(e, DTE_ERR_ARG, "dte_load_ensemble_interventional: %zu background rows, at most 2^32 - 1", n_background);
-    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, false,
-                         nullptr, false, background, n_background);
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes,
+                         {kIntervLoad, nullptr, static_cast<const uint32_t*>(background), n_background});
 }
 
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,

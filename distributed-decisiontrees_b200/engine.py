@@ -334,14 +334,6 @@ class Engine:
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
-        if leaves:
-            saved = getattr(self, "_leaf_opt", 0)
-            self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
-            try:
-                return self.load_ensemble(w, f, first_tree, num_local_trees, num_classes, binned, covers=covers, approx=approx,
-                                          background=background)
-            finally:
-                self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
         if background is not None and (covers is not None or approx or binned):
             raise ValueError("background cannot be combined with covers, approx=True or binned=True: one attribution layout "
                              "is resident at a time, and the interventional calls take fp32 tuples")
@@ -349,6 +341,8 @@ class Engine:
             raise ValueError("approx and binned=True cannot be combined: the approximate contribution calls take fp32 tuples")
         if approx and covers is None:
             raise ValueError("approx=True needs covers: the table is built from the node covers")
+        args = (_ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16)
+        tail = (int(first_tree), int(num_local_trees), int(num_classes))
         if background is not None:
             bg = np.asarray(background)
             r204 = getattr(self, "_written", {}).get(204)
@@ -357,25 +351,22 @@ class Engine:
                 raise ValueError("background must be a [N, F] float32 or uint32 array with F from register 204 (%s), "
                                  "not %s %s" % (F if F is not None else "not written", bg.dtype, bg.shape))
             bg = np.ascontiguousarray(bg).view(np.uint32)
-            self._check(self._lib.dte_load_ensemble_interventional(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
-                                                                   int(first_tree), int(num_local_trees), int(num_classes),
-                                                                   _ptr(bg), int(bg.shape[0])))
+            kind, args = "interventional", args + tail + (_ptr(bg), int(bg.shape[0]))
         elif covers is not None:
             if binned:
                 raise ValueError("covers and binned=True cannot be combined: the contribution calls take fp32 tuples")
             cv = np.ascontiguousarray(covers, dtype=np.float32)
-            load = self._lib.dte_load_ensemble_approx_contribs if approx else self._lib.dte_load_ensemble_contribs
-            self._check(load(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16, _ptr(cv), int(first_tree),
-                             int(num_local_trees), int(num_classes)))
-        elif binned:
-            self._check(self._lib.dte_load_ensemble_binned(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
-                                                           int(first_tree), int(num_local_trees), int(num_classes)))
-        elif num_classes == 1:
-            self._check(self._lib.dte_load_ensemble(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
-                                                    int(first_tree), int(num_local_trees)))
+            kind, args = "approx_contribs" if approx else "contribs", args + (_ptr(cv),) + tail
         else:
-            self._check(self._lib.dte_load_ensemble_classes(self._h, _ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16,
-                                                            int(first_tree), int(num_local_trees), int(num_classes)))
+            kind, args = "binned" if binned else "classes", args + tail
+        saved = getattr(self, "_leaf_opt", 0)
+        if leaves:
+            self.set_option(DTE_OPT_LEAF_LAYOUT, 1)
+        try:
+            self._check(getattr(self._lib, "dte_load_ensemble_" + kind)(self._h, *args))
+        finally:
+            if leaves:
+                self.set_option(DTE_OPT_LEAF_LAYOUT, saved)
         self._classes = int(num_classes)
 
     def num_classes(self):
