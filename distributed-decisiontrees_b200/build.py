@@ -8,7 +8,7 @@ SRC = os.path.join(HERE, "csrc", "dte_engine.cu")
 DEPS = [SRC, os.path.join(HERE, "csrc", "dte_kernels.cuh"), os.path.join(HERE, "csrc", "dte_device.cuh"),
         os.path.join(HERE, "..", "include", "dte.h"), os.path.join(HERE, "csrc", "dte_partition.hpp"),
         os.path.join(HERE, "csrc", "dte_shap.cuh"), os.path.join(HERE, "csrc", "dte_approx.cuh"),
-        os.path.join(HERE, "csrc", "dte_interv.cuh")]
+        os.path.join(HERE, "csrc", "dte_interv.cuh"), os.path.join(HERE, "csrc", "dte_cat.cuh")]
 OUT = os.path.join(HERE, "libdte.so")
 
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]

@@ -7,6 +7,7 @@
 #include "dte_shap.cuh"
 #include "dte_approx.cuh"
 #include "dte_interv.cuh"
+#include "dte_cat.cuh"
 
 #include <algorithm>
 #include <array>
@@ -29,8 +30,9 @@ enum { KERNEL_AUTO = 0, KERNEL_GENERIC = 1, KERNEL_TILE = 2, KERNEL_TILE_STAGED 
 
 // What a walk computes: fp32 scores, scores of u8 bins against the binned layout (DESIGN.md §9), the leaf cell every
 // tree reaches (DESIGN.md §10), the TreeSHAP feature contributions (DESIGN.md §12), interaction values (DESIGN.md §13),
-// the approximate feature contributions (DESIGN.md §14) or the interventional contributions (DESIGN.md §15)
-enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx, Interv };
+// the approximate feature contributions (DESIGN.md §14), the interventional contributions (DESIGN.md §15) or fp32 scores
+// of trees with categorical nodes (DESIGN.md §16)
+enum class Walk { Fp32, Binned, Leaf, Contrib, Inter, Approx, Interv, Cat };
 
 // How an ensemble-sharded handle returns a walk's results: the ring positions' partials combined in ring order, each
 // position's rows in its own columns of the caller's rows, or refused (fp64 attribution partials are never combined).
@@ -46,6 +48,7 @@ enum : uint32_t {
     kPathFractions = 16,    // the paths' zero fractions, built from covers (DESIGN.md §12)
     kApproxTable = 32,      // an ApproxLayout (DESIGN.md §14)
     kBackground = 64,       // the background rows (DESIGN.md §15)
+    kCatPack = 128,         // cat_top, cat_bottom and the set words (DESIGN.md §16); placed alone, without the base pack
 };
 
 // What the engine needs to know about each kind of walk.  The rest is launch_kind and kind_kernel_name.
@@ -79,6 +82,8 @@ inline constexpr WalkKind kWalkKinds[] = {
     {4, "d_tuples", "d_contribs", 4, true,
      "no interventional layout resident: load the ensemble with dte_load_ensemble_interventional", true, false,
      Sharded::Refuse, "contributions", "interventional contribution walk", kPaths | kBackground},
+    {4, "d_tuples", "d_scores", 4, false, "no categorical layout resident: load the ensemble with dte_load_ensemble_categorical",
+     true, false, Sharded::Combine, nullptr, "categorical walk", kCatPack},
 };
 inline const WalkKind& kind(Walk w) { return kWalkKinds[static_cast<int>(w)]; }
 
@@ -90,7 +95,12 @@ enum Load : uint32_t {
     kContribLoad = kPaths | kPathFractions,     // dte_load_ensemble_contribs
     kApproxLoad = kApproxTable | kLeafIds,      // dte_load_ensemble_approx_contribs
     kIntervLoad = kPaths | kBackground,         // dte_load_ensemble_interventional
+    kCatLoad = kCatPack,                        // dte_load_ensemble_categorical
 };
+
+// Why every other walk is refused while a categorical layout is resident (it is the only layout then)
+constexpr const char* kCatResident =
+    "a categorical ensemble is resident: walk it with dte_infer_device_categorical / dte_infer_host_categorical";
 
 // experiment knobs, env DTE_TUNE="ilp=4,pair=2,stages=1,warps=10,phased=1,fill=0,chunk=65536,tops=6"
 // (ilp: trees per warp, pair: warps per tuple group, stages: ring depth, warps: consumer-warp cap,
@@ -171,6 +181,10 @@ struct EnsembleShape {
 //   binned layout (DESIGN.md §9), built only when pack_ensemble is given the edge table:
 //   top_b[t][2^(D-2)]     4-byte heap records rank | fidx << 8 | missing_right << 20
 //   bottom_b              the bottom records with the rank of each node in its threshold word
+//   categorical layout (DESIGN.md §16), built only when pack_ensemble is given the sets:
+//   cat_top[t][top_stride]  8-byte heap records {word, meta} in the node format of dte_cat.cuh
+//   cat_bottom[t][nb][4]    wide bottom records {w_p, w_l, w_r, meta_p} {meta_l, meta_r, 0, 0} {leaves} {0}
+//   cat_words               0, then the set words set_words[set_offsets[0] .. set_offsets[n_sets])
 //   leaf-id layout (DESIGN.md §10), built only when pack_ensemble is asked for it:
 //   bottom_id             the bottom records with, in each leaf word, the stream cell index (in the tree's own heap
 //                         W[0 .. 2^(D+1)-2]) whose word the score walk adds: an expanded early leaf's cell in every slot
@@ -183,6 +197,17 @@ struct PackedEnsemble {
     std::vector<uint32_t> top_b;
     std::vector<uint4> bottom_b;
     std::vector<uint4> bottom_id;
+    std::vector<uint2> cat_top;
+    std::vector<uint4> cat_bottom;
+    std::vector<uint32_t> cat_words;
+};
+
+// The sets of a categorical load (CSR): set s is words[offsets[s] .. offsets[s + 1]), indexed absolutely; n = 0 with
+// null arrays: no set (and then no live node may be categorical).
+struct CatSets {
+    const uint32_t* offsets = nullptr;        // [n + 1], non-decreasing
+    const uint32_t* words = nullptr;
+    uint64_t n = 0;
 };
 
 // Per-feature edge table of the binned layout: feature f's distinct live threshold words, sorted as int32, are
@@ -205,6 +230,7 @@ struct LoadRequest {
     const uint32_t* background = nullptr;   // kBackground: [n_background][F] words
     uint64_t n_background = 0;
     BinEdges bins = {};                 // kBinnedLayout: the edge table over every tree of the streams (bin_edges)
+    CatSets cats = {};                  // kCatPack: the sets, checked by dte_load_ensemble_categorical
 };
 
 // Live nodes of one stream tree: not below an early leaf (those are unreachable; the node with bit 14 itself is live).
@@ -484,10 +510,12 @@ inline int bin_edges(const Geom& g, const unsigned char* wl, size_t n_wl, const 
 // with `classes` = C >= 2 tree first + t belongs to class (first + t) % C.  The trees are then stored class-major:
 // class c occupies tree slots [c * gpc * 8, (c + 1) * gpc * 8) in stream order, gpc = ceil(largest class / 8).
 // With `bins` (the edge table of these streams, bin_edges) the binned layout is built as well, and with `id_layout` the
-// leaf-id layout.  Returns 0 or a negative dte_status; *msg receives the reason.
+// leaf-id layout.  With `cats` only the categorical layout is built: a live node with bit 15 of its feature-index word is
+// categorical and its weight word a set number (< cats->n, else the load is refused).  Returns 0 or a negative
+// dte_status; *msg receives the reason.
 inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, const unsigned char* fl, size_t n_fl,
                          uint32_t first, uint32_t count, uint32_t classes, PackedEnsemble& out, std::string& msg,
-                         const BinEdges* bins = nullptr, bool id_layout = false) {
+                         const BinEdges* bins = nullptr, bool id_layout = false, const CatSets* cats = nullptr) {
     char buf[256];
     if (classes < 1) { msg = "class count 0"; return -1; }
     if (n_wl % g.w_cls) {
@@ -548,6 +576,14 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                 msg = buf; return -4;
             }
             max_f = std::max(max_f, f);
+            if (cats && (fi[i] & 0x8000u)) {
+                const uint32_t s = Wall[(size_t)(first + t) * wstride + i];
+                if (s >= cats->n) {
+                    snprintf(buf, sizeof buf, "tree %u node %u: categorical node with set number %u, but %llu sets were given",
+                             first + t, i, s, (unsigned long long)cats->n);
+                    msg = buf; return -1;
+                }
+            }
         }
     }
     const bool wide = max_f >= 512;
@@ -559,6 +595,24 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
     out.top_b.assign(bins ? (size_t)Tpad * top_stride : 0, 0u);
     out.bottom_b.assign(bins ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
     out.bottom_id.assign(id_layout ? out.bottom.size() : 0, make_uint4(0, 0, 0, 0));
+    out.cat_top.assign(cats ? out.top.size() : 0, make_uint2(0u, 0u));
+    out.cat_bottom.assign(cats ? (size_t)Tpad * nb * 4 : 0, make_uint4(0, 0, 0, 0));
+    const uint32_t set_base = cats && cats->n ? cats->offsets[0] : 0;
+    if (cats) {
+        out.cat_words.assign(1, 0u);
+        if (cats->n) out.cat_words.insert(out.cat_words.end(), cats->words + set_base, cats->words + cats->offsets[cats->n]);
+    }
+    // {word, meta} of node n of the packed heap in the categorical node format (dte_cat.cuh).  Only live nodes keep bit 15:
+    // the dummy level of D = 1 and the constant nodes of an expanded early leaf have index word 0.
+    auto cat_node = [&](const std::vector<uint32_t>& Wk, const std::vector<uint16_t>& Fk, uint32_t n) {
+        uint32_t word = Wk[n], meta = (Fk[n] & 0x7FFu) | ((Fk[n] >> 13) & 1u) * kCatMissingRight;
+        if (Fk[n] & 0x8000u) {
+            const uint32_t lo = cats->offsets[Wk[n]], len = cats->offsets[Wk[n] + 1] - lo;
+            word = len ? 1u + (lo - set_base) : 0u;
+            meta |= kCatFlag | (std::max(len, 1u) - 1u) << 13;
+        }
+        return make_uint2(word, meta);
+    };
     std::vector<uint32_t> Wk((2u << Dk) - 1);
     std::vector<uint16_t> Fk((1u << Dk) - 1);
     std::vector<uint32_t> cell((2u << Dk) - 1);        // stream cell each cell of the packed heap stands for
@@ -616,6 +670,18 @@ inline int pack_ensemble(const Geom& g, const unsigned char* wl, size_t n_wl, co
                 const uint32_t pack = (fp | (mp << 9)) | ((fl_ | (ml << 9)) << 10) | ((fr | (mr << 9)) << 20);
                 bp[j * 2 + 0] = make_uint4(Wk[n], Wk[l], Wk[r], pack);
                 bp[j * 2 + 1] = leaves;
+            }
+        }
+        if (cats) {
+            uint2* tc = out.cat_top.data() + (size_t)slot_of[t] * top_stride;
+            for (uint32_t n = 0; n + 1 < (1u << Dtop); ++n) tc[n] = cat_node(Wk, Fk, n);
+            uint4* bc = out.cat_bottom.data() + (size_t)slot_of[t] * nb * 4;
+            for (uint32_t j = 0; j < nb; ++j) {
+                const uint32_t n = nb - 1 + j, l = 2 * n + 1, r = 2 * n + 2;
+                const uint2 cp = cat_node(Wk, Fk, n), cl = cat_node(Wk, Fk, l), cr = cat_node(Wk, Fk, r);
+                bc[j * 4 + 0] = make_uint4(cp.x, cl.x, cr.x, cp.y);
+                bc[j * 4 + 1] = make_uint4(cl.y, cr.y, 0, 0);
+                bc[j * 4 + 2] = make_uint4(Wk[2 * l + 1], Wk[2 * l + 2], Wk[2 * r + 1], Wk[2 * r + 2]);
             }
         }
         if (id_layout) {
@@ -771,11 +837,16 @@ struct ResidentLayout {
     // background rows [background_rows][F]
     DevArray<uint32_t> background;
     uint64_t background_rows = 0;
+    // categorical layout: tree tops, wide bottom records and set words (PackedEnsemble::cat_*)
+    DevArray<uint2> cat_top;
+    DevArray<uint4> cat_bottom;
+    DevArray<uint32_t> cat_words;
     // dte_info.ensemble_bytes: every array but the edge table
     size_t bytes() const {
         return top.bytes() + top_split.bytes() + bottom.bytes() + top_b.bytes() + bottom_b.bytes() + bottom_id.bytes() +
                shap_nodes.bytes() + shap_paths.bytes() + shap_tree_path.bytes() + shap_cls_tree.bytes() +
-               approx_delta.bytes() + approx_feat.bytes() + background.bytes();
+               approx_delta.bytes() + approx_feat.bytes() + background.bytes() + cat_top.bytes() + cat_bottom.bytes() +
+               cat_words.bytes();
     }
     // whether every layout a walk of kind w reads is resident
     bool resident(Walk w) const { return (layouts & kind(w).needs) == kind(w).needs; }
@@ -1468,6 +1539,78 @@ inline cudaError_t launch_interv(Dev& d, const Geom& run, const void* d_tuples, 
     });
 }
 
+// ---- categorical walk (DESIGN.md §16) ----
+// How a categorical walk runs, read by launch_cat and cat_kernel_name: dt_walk_tile_cat with `warps` tuple groups of one
+// warp and smem bytes per CTA, or dt_walk_generic_cat when warps = 0.  The plan is static: GENERIC forces the generic
+// walk; every other variant takes the tile whenever one tuple group (F x 128 bytes) fits the opt-in shared memory, with as
+// many groups as fit, at most kCatTileNT / 32.
+struct CatPlan {
+    int warps = 0;
+    size_t smem = 0;
+};
+inline CatPlan cat_plan(const Dev& d, int want) {
+    CatPlan p;
+    if (want == KERNEL_GENERIC) return p;
+    const size_t group = (size_t)d.shape.g.F() * 128;
+    p.warps = (int)std::min<size_t>(kCatTileNT / 32, (size_t)d.smem_optin / group);
+    p.smem = (size_t)p.warps * group;
+    return p;
+}
+constexpr int kCatILP = 4;              // trees per warp and step of dt_walk_tile_cat
+using CatKernel = void (*)(CatParams);
+
+// Launch the categorical walk of n fp32 tuples on device d (cudaSetDevice already done) against the resident categorical
+// layout: scores [n][C] and labels as launch_walk's, summed with the K, S and missing pattern of `run`.  Returns a
+// cudaError_t.
+inline cudaError_t launch_cat(Dev& d, const Geom& run, int want, const void* d_tuples, size_t n, float* d_scores,
+                              uint8_t* d_labels, cudaStream_t st, const char** why) {
+    *why = nullptr;
+    if (n == 0) return cudaSuccess;
+    const CatPlan pl = cat_plan(d, want);
+    const bool mc = d.shape.C >= 2;
+    CatParams cp = {};
+    WalkParams& wp = cp.w;
+    wp.top = d.layout.cat_top;
+    wp.bottom = d.layout.cat_bottom;
+    wp.tuples = static_cast<const float*>(d_tuples);
+    wp.scores = d_scores;
+    wp.labels = d_labels;
+    wp.n = n;
+    wp.F = d.shape.g.F();
+    wp.Dtop = d.shape.Dtop;
+    wp.top_stride = d.shape.top_stride;
+    wp.nb = d.shape.nb;
+    wp.classes = d.shape.C;
+    wp.groups_per_class = d.shape.gpc;
+    wp.missing = run.missing;
+    wp.K = run.K;
+    wp.groups = mc ? d.shape.C * d.shape.gpc : (uint32_t)std::min<uint64_t>((uint64_t)run.S * run.K, d.shape.Tpad / 8);
+    cp.words = d.layout.cat_words;
+    if (pl.warps == 0) {
+        const unsigned long long blocks = (n + 127) / 128;
+        if (blocks > 0x7FFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+        (mc ? dt_walk_generic_cat<true> : dt_walk_generic_cat<false>)<<<(unsigned)blocks, 128, 0, st>>>(cp);
+        return launched(d);
+    }
+    const unsigned long long per = 32ull * pl.warps, tiles = (n + per - 1) / per;
+    if (tiles > 0xFFFFFFFFull) { *why = "batch too large for one launch"; return cudaErrorInvalidValue; }
+    wp.tiles = (uint32_t)tiles;
+    wp.nwarps = (uint32_t)pl.warps;
+    const CatKernel k = mc ? dt_walk_tile_cat<kCatILP, kCatTileNT, true> : dt_walk_tile_cat<kCatILP, kCatTileNT, false>;
+    const cudaError_t rc = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.smem);
+    if (rc != cudaSuccess) return rc;
+    k<<<(unsigned)std::min<unsigned long long>(tiles, (unsigned long long)d.sm_count), 32 * pl.warps, pl.smem, st>>>(cp);
+    return launched(d);
+}
+
+// "dt_walk_tile_cat<ILP> warps=G smem=..." or "dt_walk_generic_cat", as launch_cat would launch it
+inline void cat_kernel_name(const Dev& d, int want, char* buf, size_t len) {
+    const CatPlan pl = cat_plan(d, want);
+    if (pl.warps) snprintf(buf, len, "dt_walk_tile_cat<%d> warps=%d smem=%zu", kCatILP, pl.warps, pl.smem);
+    else snprintf(buf, len, "dt_walk_generic_cat");
+    name_classes(d, buf, len);
+}
+
 // ---- every kind of walk (kWalkKinds) ----
 // Launch the walk of kind w over n tuples on device d (cudaSetDevice already done) with the engine's knobs: the walk
 // tune, the forced variant `want` and the interaction block.  `out` receives n rows of row_bytes; labels and accumulate
@@ -1481,6 +1624,7 @@ inline cudaError_t launch_kind(Dev& d, Walk w, const Geom& run, const Tune& tune
         case Walk::Inter: return launch_inter(d, run, inter_block, tuples, n, static_cast<float*>(out), st, why);
         case Walk::Approx: return launch_approx(d, run, tune, want, tuples, n, static_cast<float*>(out), st, why);
         case Walk::Interv: return launch_interv(d, run, tuples, n, static_cast<float*>(out), st, why);
+        case Walk::Cat: return launch_cat(d, run, want, tuples, n, static_cast<float*>(out), labels, st, why);
         default: return launch_walk(d, run, tune, want, tuples, n, static_cast<float*>(out), labels, st, accumulate, why, w);
     }
 }
@@ -1499,6 +1643,7 @@ inline void kind_kernel_name(const Dev& d, Walk w, const Tune& tune, int want, u
         case Walk::Interv:                             // one kernel: a forced variant does not apply
             snprintf(buf, len, "dt_shap_interv<%d>", shap_bound(d));
             return name_classes(d, buf, len);
+        case Walk::Cat: return cat_kernel_name(d, want, buf, len);
         default: return kernel_name(d, tune, want, buf, len, w);
     }
 }

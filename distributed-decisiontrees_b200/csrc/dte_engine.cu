@@ -274,7 +274,8 @@ int decide_partition(dte_engine* e, const Geom& g) {
 
 // A run may reuse the resident ensemble only with the geometry it was loaded with (F and D fix the device
 // layout and the validated feature-index range; K, S and the missing pattern are free to change), and needs the layout
-// of its walk.  A leaf walk walks every tree whatever K and S say.
+// of its walk.  A leaf walk walks every tree whatever K and S say.  A categorical layout is resident alone: only the
+// categorical walk reads it, and it needs no base pack.
 int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
     const WalkKind& k = kind(w);
     if (e->multi() && e->placed) {
@@ -285,7 +286,8 @@ int check_resident(dte_engine* e, const Geom& g, Walk w = Walk::Fp32) {
             return fail(e, DTE_ERR_CONFIG, "devices_list (registers 208-210) changed since the tree chunks were programmed: the ring order of the partial sums would change");
     }
     for (Dev& d : e->devs) {
-        for (Walk need : {Walk::Fp32, w})            // the ensemble, then the layout of the walk
+        if (w != Walk::Cat && d.layout.resident(Walk::Cat)) return fail(e, DTE_ERR_STATE, "%s", kCatResident);
+        for (Walk need : {w == Walk::Cat ? w : Walk::Fp32, w})   // the ensemble, then the layout of the walk
             if (!d.layout.resident(need)) return fail(e, DTE_ERR_STATE, "%s", kind(need).missing);
         if (d.shape.g.tuple_cls != g.tuple_cls || d.shape.g.D != g.D)
             return fail(e, DTE_ERR_CONFIG, "registers describe %u features / %u levels but the resident ensemble was loaded with %u / %u",
@@ -333,10 +335,19 @@ struct ShareBuild {
 };
 
 // Replace device d's ensemble with a share's build, the request's edge table and the background rows `bg` (one host
-// copy for every device): the device then holds exactly the layouts the request names.
+// copy for every device): the device then holds exactly the layouts the request names.  A categorical request holds its
+// layout alone.
 int upload_share(dte_engine* e, Dev& d, const LoadRequest& req, const ShareBuild& b, const std::vector<uint32_t>& bg) {
     CUDA_TRY(e, free_ensemble(d));
     ResidentLayout& lay = d.layout;
+    if (req.layouts & kCatPack) {
+        TRY(upload(e, lay.cat_top, b.pk.cat_top));
+        TRY(upload(e, lay.cat_bottom, b.pk.cat_bottom));
+        TRY(upload(e, lay.cat_words, b.pk.cat_words));
+        d.shape = b.pk.shape;
+        lay.layouts = kCatPack;
+        return DTE_OK;
+    }
     TRY(upload(e, lay.top, b.pk.top));
     TRY(upload(e, lay.top_split, b.pk.top_split));
     TRY(upload(e, lay.bottom, b.pk.bottom));
@@ -392,7 +403,7 @@ int build_share(dte_engine* e, const Geom& g, const TreeShare& s, uint32_t class
                                                       out.approx, msg)
                                 : 0;
     if (!rc) rc = pack_ensemble(g, s.wl, s.n_wl, s.fl, s.n_fl, s.first, s.count, classes, out.pk, msg,
-                                has & kBinnedLayout ? &req.bins : nullptr, has & kLeafIds);
+                                has & kBinnedLayout ? &req.bins : nullptr, has & kLeafIds, has & kCatPack ? &req.cats : nullptr);
     return rc ? fail(e, rc == -4 ? DTE_ERR_UNSUPPORTED : DTE_ERR_ARG, "%s", msg.c_str()) : DTE_OK;
 }
 
@@ -404,7 +415,7 @@ int build_share(dte_engine* e, const Geom& g, const TreeShare& s, uint32_t class
 // before any device changes, so a refused share leaves the previous ensemble resident everywhere; a failed upload leaves
 // no ensemble on any device rather than a mix of two.
 int place_ensemble(dte_engine* e, const Geom& g, const TreeShare* share, uint32_t classes, LoadRequest& req) {
-    if (e->opt_leaf) req.layouts |= kLeafIds;
+    if (e->opt_leaf && !(req.layouts & kCatPack)) req.layouts |= kLeafIds;    // a categorical layout is placed alone
     const bool chunked = e->part == Part::Chunked;
     std::vector<ShareBuild> built(chunked ? e->devs.size() : 1);
     for (size_t r = 0; r < built.size(); ++r) TRY(build_share(e, g, share[r], classes, req, built[r]));
@@ -1472,7 +1483,11 @@ int dte_softreg_write(dte_t* e, uint32_t addr, uint64_t data) {
     int rc = decode_geom(e, g);
     if (!rc) rc = decide_partition(e, g);
     if (!rc && e->state == dte_engine::ST_DATA) {
-        rc = check_resident(e, g);
+        // the line stream walks the fp32 layout: a resident categorical ensemble is a configuration it cannot run
+        if (host_dev(e).layout.resident(Walk::Cat))
+            rc = fail(e, DTE_ERR_CONFIG, "a categorical ensemble is resident: the line stream walks numeric trees only "
+                      "(use dte_infer_host_categorical / dte_infer_device_categorical)");
+        if (!rc) rc = check_resident(e, g);
         // the result stream carries one score per tuple (ResultsCombiner.sv:132-162): no data-only run over C >= 2
         if (!rc && classes_of(e) >= 2)
             rc = fail(e, DTE_ERR_CONFIG, "the resident ensemble has %u classes: the line stream carries one score per tuple "
@@ -1762,7 +1777,7 @@ static int load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, 
     e->g = g;
     e->prog_seen = true; e->prog_open = false;
     e->t_prog0 = t0; e->t_prog1 = Clock::now();
-    return choose_measured_plan(e);
+    return req.layouts & kCatPack ? DTE_OK : choose_measured_plan(e);     // the categorical walk runs its static plan
 }
 
 int dte_load_ensemble_classes(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1799,6 +1814,29 @@ int dte_load_ensemble_interventional(dte_t* e, const void* weight_cls, size_t n_
         return fail(e, DTE_ERR_ARG, "dte_load_ensemble_interventional: %zu background rows, at most 2^32 - 1", n_background);
     return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes,
                          {kIntervLoad, nullptr, static_cast<const uint32_t*>(background), n_background});
+}
+
+// The sets are checked whole before anything is built: CSR offsets that never decrease, no set longer than
+// kCatMaxSetWords (every category below 2^24 fits), and at most 2^32 - 2 words in all (a node's 32-bit word offset).
+int dte_load_ensemble_categorical(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                                  size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes,
+                                  const uint32_t* set_offsets, size_t n_sets, const uint32_t* set_words) {
+    const char* what = "dte_load_ensemble_categorical";
+    if (!e) return DTE_ERR_ARG;
+    if (n_sets && (!set_offsets || !set_words))
+        return fail(e, DTE_ERR_ARG, "%s: %zu sets but %s is NULL", what, n_sets, set_offsets ? "set_words" : "set_offsets");
+    for (size_t s = 0; s < n_sets; ++s) {
+        if (set_offsets[s + 1] < set_offsets[s])
+            return fail(e, DTE_ERR_ARG, "%s: set_offsets decreases at set %zu (%u -> %u)", what, s, set_offsets[s], set_offsets[s + 1]);
+        if (set_offsets[s + 1] - set_offsets[s] > kCatMaxSetWords)
+            return fail(e, DTE_ERR_UNSUPPORTED, "%s: set %zu has %u words: a set holds at most 2^19 words (categories below 2^24)",
+                        what, s, set_offsets[s + 1] - set_offsets[s]);
+    }
+    if (n_sets && set_offsets[n_sets] - set_offsets[0] > 0xFFFFFFFEu)
+        return fail(e, DTE_ERR_UNSUPPORTED, "%s: the sets hold %u words, at most 2^32 - 2", what, set_offsets[n_sets] - set_offsets[0]);
+    LoadRequest req{kCatLoad};
+    req.cats = {set_offsets, set_words, (uint64_t)n_sets};
+    return load_ensemble(e, weight_cls, n_weight_cls, findex_cls, n_findex_cls, first_tree, num_local_trees, num_classes, req);
 }
 
 int dte_load_ensemble(dte_t* e, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
@@ -1838,6 +1876,7 @@ static int infer_device(dte_t* e, Walk w, const char* what, const void* d_tuples
 // the kernel and plan the next walk of kind w would launch
 static int kernel_name_of(dte_t* e, Walk w, char* buf, size_t len) {
     if (!e || !buf || !len) return DTE_ERR_ARG;
+    if (w != Walk::Cat && e->devs[0].layout.resident(Walk::Cat)) return fail(e, DTE_ERR_STATE, "%s", kCatResident);
     if (!e->devs[0].layout.resident(w)) return fail(e, DTE_ERR_STATE, "%s", kind(w).missing);
     kind_kernel_name(e->devs[0], w, walk_tune(e, w), e->forced_variant, e->opt_inter_block, buf, len);
     return DTE_OK;
@@ -1990,6 +2029,19 @@ int dte_infer_host_interventional(dte_t* e, const void* h_tuples, size_t n, floa
 }
 
 int dte_kernel_name_interventional(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Interv, buf, len); }
+
+// ---- categorical splits (DESIGN.md §16) ----
+int dte_infer_device_categorical(dte_t* e, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels, void* cuda_stream) {
+    if (!e || (n && (!d_tuples || !d_scores))) return DTE_ERR_ARG;
+    return infer_device(e, Walk::Cat, "dte_infer_device_categorical", d_tuples, n, d_scores, d_labels, cuda_stream);
+}
+
+int dte_infer_host_categorical(dte_t* e, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels) {
+    if (!e || (n && (!h_tuples || !h_scores))) return DTE_ERR_ARG;
+    return infer_host(e, Walk::Cat, "infer_host_categorical", static_cast<const unsigned char*>(h_tuples), n, h_scores, h_labels);
+}
+
+int dte_kernel_name_categorical(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, Walk::Cat, buf, len); }
 
 // ---- interaction values (DESIGN.md §13) ----
 int dte_infer_device_interactions(dte_t* e, const void* d_tuples, size_t n, float* d_inter, void* cuda_stream) {
@@ -2229,7 +2281,7 @@ int dte_get_info(dte_t* e, dte_info* info) {
         d0.timing_pending = false;
     }
     memset(info, 0, sizeof *info);
-    const bool loaded = d0.layout.top;
+    const bool loaded = d0.layout.layouts != 0;
     info->num_levels = loaded ? d0.shape.g.D : e->g.D;
     info->num_features = loaded ? d0.shape.g.F() : e->g.F();
     info->clusters = e->g.K;
@@ -2247,7 +2299,11 @@ int dte_get_info(dte_t* e, dte_info* info) {
     info->tuples_in = e->tuples_in;
     info->tuples_out = e->tuples_out;
     info->num_classes = loaded ? d0.shape.C : 0;
-    if (loaded) {
+    if (loaded && d0.layout.resident(Walk::Cat)) {
+        const CatPlan pl = cat_plan(d0, e->forced_variant);
+        info->kernel_variant = pl.warps ? KERNEL_TILE : KERNEL_GENERIC;
+        info->tuples_per_cta = pl.warps ? 32u * pl.warps : 128u;
+    } else if (loaded) {
         const Plan pl = make_plan(d0, walk_tune(e, Walk::Fp32), e->forced_variant);
         info->kernel_variant = (uint32_t)pl.variant();
         info->tuples_per_cta = pl.tuples_per_cta();
@@ -2261,6 +2317,8 @@ int dte_kernel_name(dte_t* e, char* buf, size_t len) { return kernel_name_of(e, 
 int dte_autotune(dte_t* e, size_t n_tuples, char* report, size_t report_len) {
     if (!e) return DTE_ERR_ARG;
     Dev& d = e->devs[0];
+    if (d.layout.resident(Walk::Cat))
+        return fail(e, DTE_ERR_STATE, "dte_autotune times the fp32 walk's plans; the resident categorical ensemble's walk runs its static plan");
     if (!d.layout.top) return fail(e, DTE_ERR_STATE, "no ensemble loaded");
     Geom g;
     TRY(decode_geom(e, g));

@@ -84,6 +84,11 @@ ABI = [
     ("dte_infer_device_interventional", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     ("dte_infer_host_interventional", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     ("dte_kernel_name_interventional", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    ("dte_load_ensemble_categorical", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_uint32,
+                                                C.c_uint32, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p]),
+    ("dte_infer_device_categorical", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("dte_infer_host_categorical", C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    ("dte_kernel_name_categorical", C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
     ("dte_sparse_to_dense_device", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64,
                                              C.c_void_p, C.c_void_p]),
     ("dte_infer_device_sparse", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint64, C.c_void_p,
@@ -319,7 +324,7 @@ class Engine:
 
     # -- fast paths -----------------------------------------------------------------------------
     def load_ensemble(self, weight_cls, findex_cls, first_tree=0, num_local_trees=0, num_classes=1, binned=False,
-                      leaves=False, covers=None, approx=False, background=None):
+                      leaves=False, covers=None, approx=False, background=None, categories=None):
         """num_classes >= 2: a multi-class ensemble, tree t of the stream belongs to class t % num_classes; every infer
         call then returns [n, num_classes] scores and argmax labels (dte_load_ensemble_classes).
         binned=True: also build the binned layout (dte_load_ensemble_binned; at most 254 distinct live thresholds per
@@ -330,20 +335,34 @@ class Engine:
         approx=True (with covers): build the approximate-contribution table and the leaf-id layout instead, which the
         *_approx_contribs and *_leaves calls walk (dte_load_ensemble_approx_contribs; not with binned=True).
         background: [N, F] float32 (or uint32 words) background rows: build the interventional layout the *_interventional
-        calls walk (dte_load_ensemble_interventional; not with covers, approx=True or binned=True)."""
+        calls walk (dte_load_ensemble_interventional; not with covers, approx=True or binned=True).
+        categories: (set_offsets uint32 [n_sets + 1], set_words uint32) CSR category sets: a live node with bit 15 of its
+        feature-index word tests x[f]'s category against set W[n] (dte_load_ensemble_categorical); the *_categorical calls
+        walk it and every other call is refused until the next load.  Not with binned=True, covers, approx=True or
+        background; (None, None) or empty arrays: no sets."""
         w = np.ascontiguousarray(weight_cls)
         f = np.ascontiguousarray(findex_cls)
         self._classes = None
         if background is not None and (covers is not None or approx or binned):
             raise ValueError("background cannot be combined with covers, approx=True or binned=True: one attribution layout "
                              "is resident at a time, and the interventional calls take fp32 tuples")
+        if categories is not None and (binned or covers is not None or approx or background is not None):
+            raise ValueError("categories cannot be combined with binned=True, covers, approx=True or background: a "
+                             "categorical layout is resident alone and only the categorical calls walk it")
         if approx and binned:
             raise ValueError("approx and binned=True cannot be combined: the approximate contribution calls take fp32 tuples")
         if approx and covers is None:
             raise ValueError("approx=True needs covers: the table is built from the node covers")
         args = (_ptr(w), w.nbytes // 16, _ptr(f), f.nbytes // 16)
         tail = (int(first_tree), int(num_local_trees), int(num_classes))
-        if background is not None:
+        if categories is not None:
+            offs, words = categories
+            offs = np.ascontiguousarray(offs if offs is not None else np.zeros(0), dtype=np.uint32)
+            words = np.ascontiguousarray(words if words is not None and np.size(words) else np.zeros(1), dtype=np.uint32)
+            n_sets = max(0, offs.size - 1)
+            self._cat_sets = (offs, words)           # kept alive for the call
+            kind, args = "categorical", args + tail + ((_ptr(offs), n_sets, _ptr(words)) if n_sets else (None, 0, None))
+        elif background is not None:
             bg = np.asarray(background)
             r204 = getattr(self, "_written", {}).get(204)
             F = ((r204 >> 48) & 0xFFFF) * 4 if r204 is not None else None   # tuple lines of register 204, four words each
@@ -508,6 +527,19 @@ class Engine:
 
     def kernel_name_interventional(self):
         return self._name(self._lib.dte_kernel_name_interventional)
+
+    # -- categorical splits (DESIGN.md §16) ----------------------------------------------------------
+    def infer_device_categorical(self, d_tuples, n, d_scores, d_labels=None, stream=None):
+        """infer_device against a categorical load: fp32 tuples [n, F] -> scores [n] ([n, C]) and labels, on the device."""
+        self._check(self._lib.dte_infer_device_categorical(self._h, _ptr(d_tuples), int(n), _ptr(d_scores), _ptr(d_labels),
+                                                           _stream(stream)))
+
+    def infer_host_categorical(self, tuples, want_labels=True, out_scores=None, out_labels=None):
+        """infer_host against a categorical load: host fp32 tuples [n, F] (category codes as fp32 values) -> (scores, labels)."""
+        return self._infer_host(self._lib.dte_infer_host_categorical, tuples, None, want_labels, out_scores, out_labels)
+
+    def kernel_name_categorical(self):
+        return self._name(self._lib.dte_kernel_name_categorical)
 
     # -- interaction values (DESIGN.md §13) ------------------------------------------------------------
     def infer_device_interactions(self, d_tuples, n, d_inter, stream=None):

@@ -186,3 +186,59 @@ def result_lines(scores):
     (rtl/DTEngine/ResultsCombiner.sv:132-162)."""
     s = np.asarray(scores, dtype=np.float32)
     return s[: (s.size // 4) * 4].reshape(-1, 4)
+
+
+def live_nodes(FI, depth_levels):
+    """bool [T, 2^D-1]: the internal nodes of each tree that are not below an early leaf (bit 14); a node with bit 14 is
+    itself live."""
+    FI = np.asarray(FI, dtype=np.uint16)
+    n_int = (1 << int(depth_levels)) - 1
+    live = np.ones(FI.shape, dtype=bool)
+    for i in range(n_int):
+        if 2 * i + 2 >= n_int:
+            break
+        keep = live[:, i] & ((FI[:, i] & np.uint16(0x4000)) == 0)
+        live[:, 2 * i + 1] = keep
+        live[:, 2 * i + 2] = keep
+    return live
+
+
+def synth_categorical(W, FI, depth_levels, cat_features, n_categories, share=0.25, seed=0xCA7):
+    """Categorical splits on an ensemble (dte_load_ensemble_categorical, DESIGN.md §16): a `share` of the live internal
+    nodes of W uint32 [T, 2^(D+1)-1] / FI uint16 [T, 2^D-1], drawn with a generator seeded by `seed`, become categorical:
+    feature index a random entry f of cat_features, bit 15 set, bits 13 and 14 kept, and weight word a set number of its
+    own.  The set draws each of the feature's C_f = n_categories categories (an int, or one count per entry of
+    cat_features) with probability 1/2, over ceil(C_f / 32) words.
+    -> (W, FI, set_offsets uint32 [n_sets + 1], set_words uint32): new arrays, the inputs stay as they are."""
+    rng = np.random.default_rng(seed)
+    W = np.array(W, dtype=np.uint32)
+    FI = np.array(FI, dtype=np.uint16)
+    feats = np.asarray(cat_features, dtype=np.int64)
+    cf = np.broadcast_to(np.asarray(n_categories, dtype=np.int64), feats.shape)
+    pick = live_nodes(FI, depth_levels) & (rng.random(FI.shape) < float(share))
+    t_idx, n_idx = np.nonzero(pick)
+    k = rng.integers(0, feats.size, size=t_idx.size)
+    FI[t_idx, n_idx] = (FI[t_idx, n_idx] & np.uint16(0x6000)) | feats[k].astype(np.uint16) | np.uint16(0x8000)
+    W[t_idx, n_idx] = np.arange(t_idx.size, dtype=np.uint32)
+    lens = (cf[k] + 31) // 32
+    offsets = np.zeros(t_idx.size + 1, dtype=np.uint32)
+    offsets[1:] = np.cumsum(lens)
+    words = rng.integers(0, 1 << 32, size=int(offsets[-1]), dtype=np.uint64).astype(np.uint32)
+    top = cf[k] % 32                                 # clear the bits past C_f in each set's last word
+    last = offsets[1:][top > 0] - 1
+    words[last] &= ((np.uint64(1) << top[top > 0].astype(np.uint64)) - np.uint64(1)).astype(np.uint32)
+    return W, FI, offsets, words
+
+
+def categorical_tuples(x_words, cat_features, n_categories, seed=0xC0DE, missing=MISSING_DEFAULT):
+    """Tuples for a categorical ensemble: x_words uint32 [n, F] with column cat_features[i] replaced by fp32 category
+    codes 0 .. C_i - 1 (n_categories: an int or one count per entry), drawn uniformly with a generator seeded by `seed`;
+    words equal to the missing pattern stay missing.  -> a new uint32 array."""
+    rng = np.random.default_rng(seed)
+    x = np.array(x_words, dtype=np.uint32)
+    feats = np.asarray(cat_features, dtype=np.int64)
+    cf = np.broadcast_to(np.asarray(n_categories, dtype=np.int64), feats.shape)
+    for f, c in zip(feats, cf):
+        codes = rng.integers(0, int(c), size=x.shape[0]).astype(np.float32).view(np.uint32)
+        x[:, f] = np.where(x[:, f] == np.uint32(missing), x[:, f], codes)
+    return x

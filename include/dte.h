@@ -375,6 +375,46 @@ int dte_infer_host_interventional(dte_t* engine, const void* h_tuples, size_t n,
  * DTE_ERR_STATE without the interventional layout. */
 int dte_kernel_name_interventional(dte_t* engine, char* buf, size_t len);
 
+/* ---- categorical splits (DESIGN.md §16) ------------------------------------------------------------ */
+/* Trees whose nodes may test a category set instead of a threshold (XGBoost split_type = 1, LightGBM cat_threshold,
+ * scikit-learn categorical_features).  Under dte_load_ensemble_categorical a LIVE internal node (not below an early leaf)
+ * whose feature-index word has bit 15 set is categorical: bits 10:0 give the feature f, bit 13 the missing direction,
+ * bit 14 an early leaf, bits 11-12 are ignored, and its weight word W[n] is a set number s instead of a threshold.
+ * Everywhere else bit 15 stays ignored.  Sets are CSR: set s is set_words[set_offsets[s] .. set_offsets[s+1]) (indexed
+ * absolutely, L_s words, possibly 0); category c is in set s when c < 32 L_s and bit c % 32 of word c / 32 is 1 (LSB
+ * first).  The decision at a categorical node for the tuple word x = x[f]:
+ *   x == the run's missing pattern (reg 205 at the call): right = bit 13, as at a numeric node;
+ *   else v = x read as fp32 is a valid category when it is not NaN, v >= 0 (-0 counts as category 0) and v < 2^24;
+ *   c = (uint32)trunc(v) (2.7 is category 2); right = valid && c is in set s.  In the set goes right, anything else left
+ *   (XGBoost's convention; LightGBM's in-the-set-goes-left is expressed by swapping the node's subtrees and bit 13).
+ * Numeric nodes, summation order (K, S, tree8 pairing, add.rn.ftz), multi-class [n][C] scores with argmax labels, D = 1,
+ * early leaves and the trees summed (the first min(T, 8 S K) single-class, every tree multi-class) are the fp32 walk's, so
+ * every word equals dte_infer_device's on the indicator expansion (each live categorical node a numeric node on a column
+ * of its own holding "in" / "out" words or the missing pattern).  Binned and sparse tuples are not taken. */
+/* dte_load_ensemble_classes (same placement: Dealt handles replicate, Chunked handles keep their ranges) plus the sets:
+ * set_offsets uint32 [n_sets + 1], set_words uint32.  n_sets = 0 with NULL arrays: no categorical node.  Refused before
+ * anything is uploaded (the resident ensemble stays): a live categorical node whose set number is >= n_sets, a decreasing
+ * set_offsets or n_sets > 0 with a NULL array (DTE_ERR_ARG); a set longer than 2^19 words (DTE_ERR_UNSUPPORTED); a
+ * feature index >= F (DTE_ERR_UNSUPPORTED).  The load does not time launch plans.  A categorical placement drops every
+ * other layout: dte_infer_device, _host, _accumulate, _sparse and the binned, leaf and attribution calls then return
+ * DTE_ERR_STATE, and a `start` that would stream tuples against it DTE_ERR_CONFIG.  Every other placement drops the
+ * categorical layout, after which the calls below return DTE_ERR_STATE. */
+int dte_load_ensemble_categorical(dte_t* engine, const void* weight_cls, size_t n_weight_cls, const void* findex_cls,
+                                  size_t n_findex_cls, uint32_t first_tree, uint32_t num_local_trees, uint32_t num_classes,
+                                  const uint32_t* set_offsets, size_t n_sets, const uint32_t* set_words);
+/* Scores [n][C] (and labels when d_labels is given) of n fp32 tuples [n][F] in device memory.  Single-device handles;
+ * stream as dte_infer_device.  d_tuples must be 16-byte aligned and d_scores 4-byte aligned, else DTE_ERR_ARG before any
+ * launch.  The plan is static (dte_autotune does not time it): DTE_KERNEL_GENERIC forces dt_walk_generic_cat, every other
+ * variant takes dt_walk_tile_cat wherever one 32-tuple group (F x 128 bytes) fits shared memory. */
+int dte_infer_device_categorical(dte_t* engine, const void* d_tuples, size_t n, float* d_scores, uint8_t* d_labels,
+                                 void* cuda_stream);
+/* The same from host memory through the landing pipeline, on every handle kind: Dealt handles return rows in global
+ * order, Chunked handles ring-combine the positions' partial scores in ring order as dte_infer_host does. */
+int dte_infer_host_categorical(dte_t* engine, const void* h_tuples, size_t n, float* h_scores, uint8_t* h_labels);
+/* "dt_walk_tile_cat<ILP> warps=G smem=..." or "dt_walk_generic_cat" (" classes=C" appended for C >= 2); DTE_ERR_STATE
+ * without the categorical layout. */
+int dte_kernel_name_categorical(dte_t* engine, char* buf, size_t len);
+
 /* ---- sparse tuples (DESIGN.md §11) ------------------------------------------------------------- */
 /* n tuples as CSR rows: indptr int64 [n + 1], indices uint32 [nnz] (feature numbers), values [nnz] 32-bit words (fp32 bit
  * patterns).  Row i's entries are k in [indptr[i], indptr[i+1]), indexing indices and values absolutely, so indptr[0]

@@ -99,6 +99,18 @@ done
 T="tests/test_gpu_interventional.py::test_background_sizes[33]"
 run synccheck "" ""; mv "$OUT/sanitizer_synccheck_auto.log" "$OUT/sanitizer_synccheck_interv.log"
 run racecheck "" "--racecheck-report all"; mv "$OUT/sanitizer_racecheck_auto.log" "$OUT/sanitizer_racecheck_interv.log"
+# the categorical walks: dt_walk_tile_cat and dt_walk_generic_cat, single-class and three classes, at D = 1 and D = 15,
+# at the tile's widest F and at F = 2048, and on the ragged tail of a warp
+for T in "tests/test_gpu_categorical.py::test_bit_exact_against_the_expansion[1-16-8-1-1-1-33]" \
+         "tests/test_gpu_categorical.py::test_bit_exact_against_the_expansion[15-8-16-1-1-1-200]" \
+         "tests/test_gpu_categorical.py::test_bit_exact_against_the_expansion[3-30-8-2-2-3-33]" \
+         "tests/test_gpu_categorical.py::test_bit_exact_against_the_expansion[15-6-8-1-1-3-64]" \
+         "tests/test_gpu_categorical.py::test_tile_generic_boundary_and_widest_tuples[1816]" \
+         "tests/test_gpu_categorical.py::test_tile_generic_boundary_and_widest_tuples[2048]" \
+         tests/test_gpu_categorical.py::test_kats_on_the_device; do
+  ctag=$(echo "${T##*::}" | tr -c 'A-Za-z0-9\n' '_')
+  run memcheck "" ""; mv "$OUT/sanitizer_memcheck_auto.log" "$OUT/sanitizer_memcheck_cat_${ctag}.log"
+done
 # leaks: the C++ host (no torch caching allocator in the process) over a handle's whole life, create to destroy, on three
 # ring positions sharing one GPU, data- and ensemble-sharded, fed by the line stream and by the host fast path
 for mode in stream host; do
