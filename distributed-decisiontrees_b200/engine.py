@@ -115,6 +115,8 @@ PLAN_SOURCES = {0: "static", 1: "measured"}    # dte_plan_source
 DTE_OPT_CYCLE_MHZ, DTE_OPT_COMBINE, DTE_OPT_RESULT_QUEUE_LINES, DTE_OPT_CHUNK_TUPLES = 1, 2, 3, 4
 DTE_OPT_LEAF_LAYOUT = 5
 DTE_OPT_INTERACTION_BLOCK = 6     # matrix rows per interaction pass (0 = the planner's)
+DTE_OK = 0
+DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG, DTE_ERR_UNSUPPORTED, DTE_ERR_CUDA, DTE_ERR_NOMEM = -1, -2, -3, -4, -5, -6
 DTE_ERR_BACKPRESSURE = -7
 DTE_SPARSE_ABSENT_MISSING = 0xFFFFFFFFFFFFFFFF   # sparse calls: an absent feature is the run's missing pattern (reg 205)
 CUDA_STREAM_LEGACY = 0x1        # cudaStreamLegacy: the handle value that NAMES the legacy default stream

@@ -12,10 +12,13 @@ from ddt_b200 import engine as E
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def header_symbols():
+def header_source():
     src = open(os.path.join(ROOT, "include", "dte.h")).read()
-    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(dte_[a-z_0-9]+)\s*\(", src)))
+    return re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+
+
+def header_symbols():
+    return sorted(set(re.findall(r"\b(dte_[a-z_0-9]+)\s*\(", header_source())))
 
 
 def test_library_exports_every_declared_symbol():
@@ -26,6 +29,15 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, s), "libdte.so does not export %s" % s
     # and the Python mirror binds exactly the header's set
     assert sorted(n for n, _, _ in E.ABI) == syms
+
+
+def test_status_codes_match_the_header():
+    """Every value of the dte_status enum in include/dte.h, and the Python mirror of it in engine.py."""
+    body = re.search(r"typedef enum \{([^}]*)\} dte_status;", header_source()).group(1)
+    codes = {name: int(value) for name, value in re.findall(r"\b(DTE_\w+)\s*=\s*(-?\d+)", body)}
+    assert codes["DTE_OK"] == 0 and len(codes) == 8, codes
+    for name, value in codes.items():
+        assert getattr(E, name) == value, name
 
 
 def test_version_string():
@@ -67,18 +79,18 @@ def test_no_cpu_fallback_without_device():
         pytest.skip("GPU present")
     with pytest.raises(E.DteError) as ei:
         ddt.Engine(0)
-    assert ei.value.code == -5          # DTE_ERR_CUDA
+    assert ei.value.code == E.DTE_ERR_CUDA
 
 
 def test_null_arguments_are_errors_not_crashes():
     lib = ddt.load_library()
-    assert lib.dte_create(None, 0) == -1
-    assert lib.dte_destroy(None) == -1
-    assert lib.dte_softreg_write(None, 200, 1) == -1
+    assert lib.dte_create(None, 0) == E.DTE_ERR_ARG
+    assert lib.dte_destroy(None) == E.DTE_ERR_ARG
+    assert lib.dte_softreg_write(None, 200, 1) == E.DTE_ERR_ARG
     v = C.c_uint64()
-    assert lib.dte_softreg_read(None, 220, C.byref(v)) == -1
+    assert lib.dte_softreg_read(None, 220, C.byref(v)) == E.DTE_ERR_ARG
     assert lib.dte_last_error(None) == b"null engine"
-    assert lib.dte_set_node(None, 0) == -1
+    assert lib.dte_set_node(None, 0) == E.DTE_ERR_ARG
 
 
 def test_product_does_not_touch_the_oracle():

@@ -11,68 +11,14 @@ import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from approx_ref import approx_contribs, tree_table
 from edge_operands import edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, oracle_scores, L
+from helpers import (assert_words, device_rows, early, efficiency, geometry_regs, host_rows, make_engine,
+                     multi_node_regs, oracle_scores, refused, torch_cuda, write_regs, CANARY, L)  # noqa: F401
 from leaf_oracle import leaf_cells
 from shap_ref import path_treeshap
 
 pytestmark = pytest.mark.gpu
 
 VARIANTS = [E.DTE_KERNEL_AUTO, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_TILE, E.DTE_KERNEL_GENERIC]
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG = -1, -2, -3
-U = 2.0 ** -24
-CANARY = 0x7A7A7A7A
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def early(FI, D, seed):
-    """Bit 14 on one random node of every tree but the first, and on the root of tree 2."""
-    rng = np.random.default_rng(seed)
-    FI = FI.copy()
-    for t in range(1, FI.shape[0]):
-        lvl = int(rng.integers(0, D))
-        FI[t, (1 << lvl) - 1 + int(rng.integers(0, 1 << lvl))] |= 1 << 14
-    if FI.shape[0] > 2:
-        FI[2, 0] |= 1 << 14
-    return FI
-
-
-def device_approx(torch, e, x, C, F, stream=None):
-    """[n, C, F + 1] from dte_infer_device_approx_contribs, with a canary row after the last row."""
-    n, row = x.shape[0], C * (F + 1)
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    buf = torch.full((n * row + 64,), CANARY, dtype=torch.int32, device="cuda")
-    e.infer_device_approx_contribs(dx, n, buf, stream=stream)
-    torch.cuda.synchronize()
-    got = buf.cpu().numpy()
-    assert (got[n * row:] == CANARY).all(), "wrote past the last row"
-    return got[: n * row].view(np.float32).reshape(n, C, F + 1)
-
-
-def assert_words(got, want, what):
-    g, w = np.asarray(got, dtype=np.float32).view(np.uint32), np.asarray(want, dtype=np.float32).view(np.uint32)
-    assert g.shape == w.shape, (what, g.shape, w.shape)
-    bad = np.argwhere(g != w)
-    assert bad.size == 0, "%s: %d words differ, first at %s: %r instead of %r" % (
-        what, len(bad), tuple(bad[0]), g[tuple(bad[0])].view(np.float32), w[tuple(bad[0])].view(np.float32))
-
-
-def host3(e, x, C):
-    out = e.infer_host_approx_contribs(x)
-    return out[:, None, :] if C == 1 else out
 
 
 def check_all(torch, e, x, want, C, F, variants=VARIANTS, what=""):
@@ -81,25 +27,11 @@ def check_all(torch, e, x, want, C, F, variants=VARIANTS, what=""):
         e.set_kernel_variant(v)
         name = e.kernel_name_approx_contribs()
         assert name.endswith(" + dt_approx_generic"), name
-        assert_words(host3(e, x, C), want, "%s host %s" % (what, name))
+        assert_words(host_rows(e, "_approx_contribs", x, C), want, "%s host %s" % (what, name))
         s = torch.cuda.Stream()
-        assert_words(device_approx(torch, e, x, C, F, stream=s.cuda_stream), want, "%s device %s" % (what, name))
+        assert_words(device_rows(torch, e, "_approx_contribs", x, (C, F + 1), stream=s.cuda_stream), want,
+                     "%s device %s" % (what, name))
     e.set_kernel_variant(E.DTE_KERNEL_AUTO)
-
-
-def efficiency(torch, e, x, phi, T_used_leaf_abs, T):
-    """phi [n, C, F + 1] against the same handle's dte_infer_device score words, with the form test_gpu_contribs uses:
-    the fp32 rounding of every word, and (T + 1) fp32 roundings of the score words' leaf sum (the exact sum of the
-    deltas along a path telescopes to the leaf minus E[root], so the fp64 accumulators sum to the score in exact
-    arithmetic up to their own roundings, which are far below these)."""
-    n, C = x.shape[0], phi.shape[1]
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    ds = torch.empty(n * C, dtype=torch.float32, device="cuda")
-    e.infer_device(dx, n, ds)
-    score = ds.cpu().numpy().astype(np.float64).reshape(n, C)
-    p = phi.astype(np.float64)
-    bound = U * np.abs(p).sum(axis=2) + (T + 1) * U * T_used_leaf_abs + 1e-12 * T_used_leaf_abs
-    assert (np.abs(p.sum(axis=2) - score) <= bound).all()
 
 
 # (D, F): every depth of the list, every F of the list (2048 the widest the engine takes)
@@ -204,8 +136,7 @@ def test_missing_pattern_rewritten_after_the_load(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, covers=cov, approx=True)
-        for a, v in sorted(geometry_regs(T, D, F, 8, 2, 0x00000000).items()):
-            e.softreg_write(a, v)
+        write_regs(e, geometry_regs(T, D, F, 8, 2, 0x00000000))
         want = approx_contribs(W, FI, cov, x, D, F, missing=0x00000000)
         check_all(torch_cuda, e, x, want, 1, F, variants=[E.DTE_KERNEL_AUTO, E.DTE_KERNEL_GENERIC])
 
@@ -256,8 +187,7 @@ def test_multi_device_handles(torch_cuda, mode):
         single = e.infer_host_approx_contribs(x)
     assert_words(single[:, None, :], approx_contribs(W, FI, cov, x, D, F), "single")
     with ddt.Engine([0, 0, 0]) as e:
-        for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, mode).items()):
-            e.softreg_write(a, v)
+        write_regs(e, multi_node_regs(T, D, F, K, n, 3, mode))
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 64)
         e.load_ensemble(wl, fl, covers=cov, approx=True)
         if mode == "data":
@@ -265,9 +195,7 @@ def test_multi_device_handles(torch_cuda, mode):
                 e.set_kernel_variant(v)
                 assert_words(e.infer_host_approx_contribs(x), single, "Dealt %s" % E.KERNEL_NAMES[v])
         else:
-            with pytest.raises(E.DteError) as ex:
-                e.infer_host_approx_contribs(x)
-            assert ex.value.code == DTE_ERR_CONFIG
+            refused(lambda: e.infer_host_approx_contribs(x), E.DTE_ERR_CONFIG)
         dx = torch_cuda.zeros((n, F), dtype=torch_cuda.float32, device="cuda")
         out = torch_cuda.empty(n * (F + 1), dtype=torch_cuda.float32, device="cuda")
         with pytest.raises(E.DteError):
@@ -289,41 +217,31 @@ def test_refusals(torch_cuda):
         for load in (lambda: e.load_ensemble(wl, fl), lambda: e.load_ensemble(wl, fl, covers=cov)):
             load()                                        # no table: a plain or a TreeSHAP load
             for call in calls:
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE and "dte_load_ensemble_approx_contribs" in str(ex.value)
+                refused(call, E.DTE_ERR_STATE, "dte_load_ensemble_approx_contribs")
         with pytest.raises(ValueError):
             e.load_ensemble(wl, fl, covers=cov, approx=True, binned=True)
         junk = cov.copy()
         junk[3, [7, 8, 9, 10, 15, 16]] = [0, -1, np.nan, np.inf, 0, -5]      # below the early leaf: never read
         e.load_ensemble(wl, fl, covers=junk, approx=True)
         want = approx_contribs(W, FI, cov, x, D, F)
-        assert_words(host3(e, x, 1), want, "garbage below an early leaf")
-        with pytest.raises(E.DteError) as ex:                # the TreeSHAP layout is not built by this load
-            e.infer_host_contribs(x)
-        assert ex.value.code == DTE_ERR_STATE
+        assert_words(host_rows(e, "_approx_contribs", x, 1), want, "garbage below an early leaf")
+        refused(lambda: e.infer_host_contribs(x), E.DTE_ERR_STATE)        # the TreeSHAP layout is not built by this load
         scores = e.infer_host(x)[0]
         for cell, bad in ((0, 0.0), (4, -1.0), (1, np.nan), (20, np.inf), (30, 0.0)):
             c = cov.copy()
             c[5, cell] = bad
-            with pytest.raises(E.DteError) as ex:
-                e.load_ensemble(wl, fl, covers=c, approx=True)
-            assert ex.value.code == DTE_ERR_ARG and "tree 5 cell %d" % cell in str(ex.value), str(ex.value)
-            assert_words(host3(e, x, 1), want, "after a refused load")           # the previous ensemble still answers
+            refused(lambda: e.load_ensemble(wl, fl, covers=c, approx=True), E.DTE_ERR_ARG, "tree 5 cell %d" % cell)
+            assert_words(host_rows(e, "_approx_contribs", x, 1), want, "after a refused load")   # the previous ensemble still answers
             assert (e.infer_host(x)[0].view(np.uint32) == scores.view(np.uint32)).all()
         for args in ((dx[:, 1:].reshape(-1)[1:], 1, out), (dx, n, out[1:].view(torch_cuda.uint8)[1:])):
-            with pytest.raises(E.DteError) as ex:
-                e.infer_device_approx_contribs(*args)
-            assert ex.value.code == DTE_ERR_ARG
+            refused(lambda: e.infer_device_approx_contribs(*args), E.DTE_ERR_ARG)
         for drop in (lambda: e.load_ensemble(wl, fl), lambda: e.load_ensemble(wl, fl, binned=True),
                      lambda: e.load_ensemble(wl, fl, covers=cov)):
             e.load_ensemble(wl, fl, covers=cov, approx=True)
-            assert_words(host3(e, x, 1), want, "reloaded")
+            assert_words(host_rows(e, "_approx_contribs", x, 1), want, "reloaded")
             drop()                                        # a later load of any other kind drops the table
             for call in calls[:2]:
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE
+                refused(call, E.DTE_ERR_STATE)
 
 
 def test_line_stream_placement_drops_the_table(torch_cuda):
@@ -336,12 +254,10 @@ def test_line_stream_placement_drops_the_table(torch_cuda):
     with ddt.Engine(0) as e:
         e.configure(T, D, 4 * F, clusters=2, n_tuples=n)
         e.load_ensemble(wl, fl, covers=cov, approx=True)
-        assert_words(host3(e, x, 1), approx_contribs(W, FI, cov, x, D, F), "before the stream")
+        assert_words(host_rows(e, "_approx_contribs", x, 1), approx_contribs(W, FI, cov, x, D, F), "before the stream")
         e.start()
         e.stream_write(wl)
         e.stream_write(fl)
         e.stream_write(x)
         e.stream_flush()
-        with pytest.raises(E.DteError) as ex:
-            e.infer_host_approx_contribs(x)
-        assert ex.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_approx_contribs(x), E.DTE_ERR_STATE)

@@ -2,61 +2,28 @@
 
 Bar everywhere: every score word and every label equals the oracle's on the fp32 tuples (or, on multi-device handles,
 the engine's own fp32 path, which the rest of the suite holds to the oracle)."""
-import collections
-import lzma
-import os
-
 import numpy as np
 import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_leaves
-from helpers import geometry_regs, multi_node_regs, oracle_scores, L
+from helpers import (assert_scores, make_engine, multi_node_regs, oracle_scores, oracle_words, plan_groups, plan_rows,
+                     refused, torch_cuda, write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-TABLE = os.path.join(HERE, "golden", "plan_table_binned.txt.xz")
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_UNSUPPORTED = -1, -2, -4
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-Row = collections.namedtuple("Row", "tune D F C variant name")
-
-
-def plan_rows():
-    rows, tune = [], None
-    with lzma.open(TABLE, "rt") as f:
-        for line in f:
-            line = line.rstrip("\n")
-            if line.startswith("DTE_TUNE="):
-                tune = line[len("DTE_TUNE="):]
-                continue
-            D, F, C, variant, _phased, name = line.split(" ", 5)
-            rows.append(Row(tune, int(D), int(F), int(C), int(variant), name))
-    return rows
 
 
 def matrix_cases():
     """One typical (|D - 10|, F smallest) and one extreme (largest D, F) row per (binned kernel template, C), as
     (row, None); then the typical row of every group on edge operands (tests/edge_operands.py), as (row, missing
     pattern) with the pattern taken from MISSING_ROTATION by group index."""
-    groups = collections.OrderedDict()
-    for r in plan_rows():
-        groups.setdefault((r.name.split(">")[0] + ">", r.C), []).append(r)
     out, edge = [], []
-    for i, ((t, C), rs) in enumerate(groups.items()):
-        typical = min(rs, key=lambda r: (abs(r.D - 10), r.F))
-        for kind, r in (("typical", typical), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
+    for i, ((t, C), (typical, extreme)) in enumerate(plan_groups(plan_rows("plan_table_binned.txt.xz")).items()):
+        for kind, r in (("typical", typical), ("extreme", extreme)):
             out.append(pytest.param(r, None, id="%s-C%d-%s-D%d-F%d" % (t.replace(" ", ""), C, kind, r.D, r.F)))
         m = MISSING_ROTATION[i % len(MISSING_ROTATION)]
         edge.append(pytest.param(typical, m, id="%s-C%d-edge-D%d-F%d-m%08x" % (t.replace(" ", ""), C, typical.D, typical.F, m)))
@@ -81,36 +48,6 @@ def hist_ensemble(T, D, F, seed, cuts=254, wide=None):
     if wide:
         FI[0, (1 << D) - 2] = (FI[0, (1 << D) - 2] & 0x2000) | (F - 1)
     return W, FI
-
-
-def oracle_words(W, FI, x, D, K, S, C, missing=L.MISSING_DEFAULT):
-    kw = dict(threads=O.max_threads())
-    if C == 1:
-        return oracle_scores(W, FI, x, D, K, S, missing, **kw)
-    out = np.zeros((x.shape[0], C), dtype=np.uint32)
-    for c in range(C):
-        if W[c::C].shape[0]:
-            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, missing, **kw)
-    return out
-
-
-def labels_of(want, C):
-    return O.labels(want) if C == 1 else np.argmax(want.view(np.float32), axis=1).astype(np.uint8)
-
-
-def assert_words(sc, lb, want, C, what):
-    got = np.asarray(sc).view(np.uint32).reshape(want.shape)
-    bad = np.argwhere(got != want)
-    assert bad.size == 0, "%s: %d words differ, first at %s" % (what, len(bad), bad[0])
-    if lb is not None:
-        assert (np.asarray(lb) == labels_of(want, C)).all(), what + ": labels differ"
-
-
-def make_engine(T, D, F, K, S, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
 
 
 def run_case(torch, T, D, F, K, S, C, n, seed, variants=VARIANTS, missing=None):
@@ -143,16 +80,16 @@ def run_case(torch, T, D, F, K, S, C, n, seed, variants=VARIANTS, missing=None):
                 e.set_kernel_variant(v)
                 names[v] = e.kernel_name_binned()
                 sc, lb = e.infer_host_binned(b)
-                assert_words(sc, lb, want, C, "host %s" % names[v])
+                assert_scores(sc, lb, want, C, "host %s" % names[v])
                 ds = torch.empty((n, C) if C > 1 else (n,), dtype=torch.float32, device="cuda")
                 dl = torch.empty(n, dtype=torch.uint8, device="cuda")
                 e.infer_device_binned(db, n, ds, dl, stream=s.cuda_stream)
                 s.synchronize()
-                assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "device %s" % names[v])
+                assert_scores(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "device %s" % names[v])
             # the fp32 calls still score a binned load correctly
             e.set_kernel_variant(E.DTE_KERNEL_AUTO)
             sc, lb = e.infer_host(x)
-            assert_words(sc, lb, want, C, "fp32 after a binned load")
+            assert_scores(sc, lb, want, C, "fp32 after a binned load")
     return names
 
 
@@ -227,8 +164,7 @@ def test_host_binned_on_multi_device_handles_and_pageable(torch_cuda):
         regs = multi_node_regs(T, D, F, K, n, 2, mode, batch_tuples=64)
         with ddt.Engine([0, 0]) as e:
             e.set_option(E.DTE_OPT_CHUNK_TUPLES, 5000)
-            for a, v in sorted(regs.items()):
-                e.softreg_write(a, v)
+            write_regs(e, regs)
             e.load_ensemble(wl, fl, binned=True)
             want, wlb = e.infer_host(x)
             off, edges = e.bin_edges()
@@ -241,9 +177,7 @@ def test_host_binned_on_multi_device_handles_and_pageable(torch_cuda):
             e.host_free(pinned)
             sc, lb = e.infer_host(x)
             assert (sc.view(np.uint32) == want.view(np.uint32)).all(), mode
-            with pytest.raises(E.DteError) as ei:
-                e.infer_device_binned(0, 0, 0)
-            assert ei.value.code == DTE_ERR_UNSUPPORTED
+            refused(lambda: e.infer_device_binned(0, 0, 0), E.DTE_ERR_UNSUPPORTED)
 
 
 def test_chunks_share_edges_and_ring_combine(torch_cuda):
@@ -285,51 +219,33 @@ def test_refusals(torch_cuda):
     want = oracle_words(W, FI, x, D, K, S, 1)
     with make_engine(T, D, F, K, S) as e:
         e.load_ensemble(wl, fl)
-        with pytest.raises(E.DteError) as ei:                # binned call after a plain load
-            e.infer_host_binned(np.zeros((n, F), np.uint8))
-        assert ei.value.code == DTE_ERR_STATE
-        with pytest.raises(E.DteError) as ei:
-            e.kernel_name_binned()
-        assert ei.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_binned(np.zeros((n, F), np.uint8)), E.DTE_ERR_STATE)      # binned call after a plain load
+        refused(e.kernel_name_binned, E.DTE_ERR_STATE)
         d8 = torch.zeros(n * F, dtype=torch.uint8, device="cuda")
         d32 = torch.zeros(n * F, dtype=torch.float32, device="cuda")
         ds = torch.zeros(n, dtype=torch.float32, device="cuda")
-        with pytest.raises(E.DteError) as ei:
-            e.infer_device_binned(d8, n, ds)
-        assert ei.value.code == DTE_ERR_STATE
-        with pytest.raises(E.DteError) as ei:
-            e.bin_tuples_device(d32, n, d8)
-        assert ei.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_device_binned(d8, n, ds), E.DTE_ERR_STATE)
+        refused(lambda: e.bin_tuples_device(d32, n, d8), E.DTE_ERR_STATE)
         Wb, FIb = L.synth_ensemble(T, D, F, seed=7202)       # U[0,1) thresholds: > 254 distinct on some feature
         wb, fb = L.pack_streams(Wb, FIb, D)
-        with pytest.raises(E.DteError) as ei:
-            e.load_ensemble(wb, fb, binned=True)
-        assert ei.value.code == DTE_ERR_UNSUPPORTED and "distinct thresholds" in str(ei.value)
+        refused(lambda: e.load_ensemble(wb, fb, binned=True), E.DTE_ERR_UNSUPPORTED, "distinct thresholds")
         sc, lb = e.infer_host(x)                              # the old ensemble still scores
-        assert_words(sc, lb, want, 1, "after a refused binned load")
+        assert_scores(sc, lb, want, 1, "after a refused binned load")
         e.load_ensemble(wl, fl, binned=True)
         off = np.empty(F + 1, dtype=np.uint32)
         total = E.C.c_size_t()
         assert e._lib.dte_bin_edges(e._h, off.ctypes.data, None, 0, E.C.byref(total)) == 0 and total.value >= 2
         small = np.empty(total.value, dtype=np.uint32)
-        assert e._lib.dte_bin_edges(e._h, off.ctypes.data, small.ctypes.data, total.value - 1, E.C.byref(total)) == DTE_ERR_ARG
+        assert e._lib.dte_bin_edges(e._h, off.ctypes.data, small.ctypes.data, total.value - 1, E.C.byref(total)) == E.DTE_ERR_ARG
         base = torch.zeros(n * F + 64, dtype=torch.uint8, device="cuda")
         scores = torch.zeros(n + 4, dtype=torch.float32, device="cuda")
         fx = torch.zeros(n * F + 16, dtype=torch.float32, device="cuda")
         for args in ((base.data_ptr() + 4, n, scores), (base.data_ptr(), n, scores.data_ptr() + 2)):
-            with pytest.raises(E.DteError) as ei:
-                e.infer_device_binned(*args)
-            assert ei.value.code == DTE_ERR_ARG
-        with pytest.raises(E.DteError) as ei:
-            e.bin_tuples_device(fx.data_ptr() + 4, n, base)
-        assert ei.value.code == DTE_ERR_ARG
-        with pytest.raises(E.DteError) as ei:
-            e.bin_tuples_device(fx, n, base.data_ptr() + 8)
-        assert ei.value.code == DTE_ERR_ARG
+            refused(lambda: e.infer_device_binned(*args), E.DTE_ERR_ARG)
+        refused(lambda: e.bin_tuples_device(fx.data_ptr() + 4, n, base), E.DTE_ERR_ARG)
+        refused(lambda: e.bin_tuples_device(fx, n, base.data_ptr() + 8), E.DTE_ERR_ARG)
         e.load_ensemble(wl, fl)                               # a plain load drops the binned layout
-        with pytest.raises(E.DteError) as ei:
-            e.bin_edges()
-        assert ei.value.code == DTE_ERR_STATE
+        refused(e.bin_edges, E.DTE_ERR_STATE)
 
 
 def test_headline_binned_multi_tile(torch_cuda):

@@ -13,33 +13,12 @@ import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from cat_ref import cat_scores, oracle_expanded
 from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, oracle_scores
+from helpers import (assert_scores, device_scores, geometry_regs, labels_of, make_engine, multi_node_regs,
+                     oracle_scores, refused, torch_cuda, write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 
 pytestmark = pytest.mark.gpu
 
-L = ddt.layout
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG, DTE_ERR_UNSUPPORTED = -1, -2, -3, -4
-CANARY = 0x7A7A7A7A
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def write_regs(e, regs):
-    for a, v in sorted(regs.items()):
-        e.softreg_write(a, v)
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    write_regs(e, geometry_regs(T, D, F, K, S, missing))
-    return e
 
 
 def categorical_case(T, D, F, seed, share, n, C_f=(5, 40, 300), early=False, cat_f=None):
@@ -62,26 +41,6 @@ def reference(W, FI, x, D, K, S, missing, off, words, C=1):
     return cat_scores(W, FI, x, D, K, S, missing, off, words, C=C)
 
 
-def labels_of(want):
-    w = want.view(np.float32)
-    return (w > 0).astype(np.uint8) if w.ndim == 1 else np.argmax(w, axis=1).astype(np.uint8)
-
-
-def device_scores(torch, e, x, C, stream=None):
-    """scores [n] or [n, C] and labels of dte_infer_device_categorical, with a canary after the last score word."""
-    n = x.shape[0]
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    buf = torch.full((n * C + 64,), CANARY, dtype=torch.int32, device="cuda")
-    lb = torch.full((n + 16,), 0xA5, dtype=torch.uint8, device="cuda")
-    e.infer_device_categorical(dx, n, buf, lb, stream=stream)
-    torch.cuda.synchronize()
-    got = buf.cpu().numpy()
-    assert (got[n * C:] == CANARY).all(), "wrote past the last score"
-    assert (lb.cpu().numpy()[n:] == 0xA5).all(), "wrote past the last label"
-    sc = got[: n * C].view(np.uint32)
-    return (sc if C == 1 else sc.reshape(n, C)), lb.cpu().numpy()[:n]
-
-
 def check(torch, e, x, want, C, variants=(E.DTE_KERNEL_TILE, E.DTE_KERNEL_GENERIC), what=""):
     names = []
     for v in variants:
@@ -91,12 +50,10 @@ def check(torch, e, x, want, C, variants=(E.DTE_KERNEL_TILE, E.DTE_KERNEL_GENERI
         if v == E.DTE_KERNEL_GENERIC:
             assert name.startswith("dt_walk_generic_cat"), name
         sc, lb = e.infer_host_categorical(x)
-        assert (sc.view(np.uint32) == want).all(), "%s host %s: %d words differ" % (what, name, int((sc.view(np.uint32) != want).sum()))
-        assert (lb == labels_of(want)).all(), "%s host labels %s" % (what, name)
+        assert_scores(sc, lb, want, C, "%s host %s" % (what, name))
         s = torch.cuda.Stream()
-        dsc, dlb = device_scores(torch, e, x, C, stream=s.cuda_stream)
-        assert (dsc == want).all(), "%s device %s: %d words differ" % (what, name, int((dsc != want).sum()))
-        assert (dlb == labels_of(want)).all(), "%s device labels %s" % (what, name)
+        dsc, dlb = device_scores(torch, e, "_categorical", x, C, stream=s.cuda_stream)
+        assert_scores(dsc, dlb, want, C, "%s device %s" % (what, name))
     e.set_kernel_variant(E.DTE_KERNEL_AUTO)
     return names
 
@@ -192,7 +149,7 @@ def test_kats_on_the_device(torch_cuda):
             for v in (E.DTE_KERNEL_TILE, E.DTE_KERNEL_GENERIC):
                 e.set_kernel_variant(v)
                 bits = int(e.infer_host_categorical(x)[0][0])
-                dsc, _ = device_scores(torch_cuda, e, x, 1)
+                dsc, _ = device_scores(torch_cuda, e, "_categorical", x, 1)
                 assert dsc[0] == np.float32(bits).view(np.uint32)
                 for k, c in enumerate(group):
                     assert (bits >> k) & 1 == c["right"], (c["why"], E.KERNEL_NAMES[v])
@@ -246,7 +203,7 @@ def test_host_path_pinned_and_pageable(torch_cuda):
         hs = e.host_alloc((n,), np.float32)
         hx[:] = x
         sc, lb = e.infer_host_categorical(hx, out_scores=hs)
-        assert (hs.view(np.uint32) == want).all() and (lb == labels_of(want)).all()
+        assert (hs.view(np.uint32) == want).all() and (lb == labels_of(want, 1)).all()
         sc, lb = e.infer_host_categorical(x)
         assert (sc.view(np.uint32) == want).all()
         e.host_free(hx)
@@ -277,19 +234,8 @@ def test_dealt_and_chunked_handles(mode):
             e.set_kernel_variant(v)
             sc, lb = e.infer_host_categorical(x)
             assert (sc.view(np.uint32) == want).all(), (mode, E.KERNEL_NAMES[v])
-            assert (lb == labels_of(want)).all()
-        with pytest.raises(E.DteError) as ei:                  # device pointers belong to one device
-            e.infer_device_categorical(0x1000, 4, 0x2000)
-        assert ei.value.code == DTE_ERR_UNSUPPORTED
-
-
-def raises(code, fn, *needles):
-    with pytest.raises(E.DteError) as ex:
-        fn()
-    assert ex.value.code == code, str(ex.value)
-    for s in needles:
-        assert s in str(ex.value), str(ex.value)
-    return str(ex.value)
+            assert (lb == labels_of(want, 1)).all()
+        refused(lambda: e.infer_device_categorical(0x1000, 4, 0x2000), E.DTE_ERR_UNSUPPORTED)   # device pointers belong to one device
 
 
 def test_refusals(torch_cuda):
@@ -306,7 +252,7 @@ def test_refusals(torch_cuda):
         plain = e.infer_host(x)[0].copy()
         for call in (lambda: e.infer_host_categorical(x), lambda: e.infer_device_categorical(dx, n, ds),
                      lambda: e.kernel_name_categorical()):
-            raises(DTE_ERR_STATE, call, "no categorical layout resident: load the ensemble with dte_load_ensemble_categorical")
+            refused(call, E.DTE_ERR_STATE, "no categorical layout resident: load the ensemble with dte_load_ensemble_categorical")
         for kw in (dict(binned=True), dict(covers=cov), dict(covers=cov, approx=True), dict(background=x[:4])):
             with pytest.raises(ValueError):
                 e.load_ensemble(wl, fl, categories=(off, words), **kw)
@@ -314,19 +260,19 @@ def test_refusals(torch_cuda):
         tc, nc = np.nonzero(FI & 0x8000)
         t0, node = int(tc[0]), int(nc[0])                # the first categorical node, set 0
         last = off.size - 2                              # the last one holds the last set, which a shorter CSR lacks
-        raises(DTE_ERR_ARG, lambda: e.load_ensemble(wl, fl, categories=(off[:-1], words)),
-               "tree %d node %d: categorical node with set number %d, but %d sets were given" % (tc[-1], nc[-1], last, last))
+        refused(lambda: e.load_ensemble(wl, fl, categories=(off[:-1], words)), E.DTE_ERR_ARG,
+                "tree %d node %d: categorical node with set number %d, but %d sets were given" % (tc[-1], nc[-1], last, last))
         bad = off.copy()
         bad[2] = bad[3] + 1
-        raises(DTE_ERR_ARG, lambda: e.load_ensemble(wl, fl, categories=(bad, words)),
-               "dte_load_ensemble_categorical: set_offsets decreases at set 2")
+        refused(lambda: e.load_ensemble(wl, fl, categories=(bad, words)), E.DTE_ERR_ARG,
+                "dte_load_ensemble_categorical: set_offsets decreases at set 2")
         big = np.array([0, (1 << 19) + 1], np.uint32)
-        raises(DTE_ERR_UNSUPPORTED, lambda: e.load_ensemble(wl, fl, categories=(big, np.zeros((1 << 19) + 1, np.uint32))),
-               "dte_load_ensemble_categorical: set 0 has 524289 words: a set holds at most 2^19 words")
+        refused(lambda: e.load_ensemble(wl, fl, categories=(big, np.zeros((1 << 19) + 1, np.uint32))), E.DTE_ERR_UNSUPPORTED,
+                "dte_load_ensemble_categorical: set 0 has 524289 words: a set holds at most 2^19 words")
         FIw = FI.copy()
         FIw[t0, node] = (FIw[t0, node] & ~np.uint16(0x7FF)) | np.uint16(F)
-        raises(DTE_ERR_UNSUPPORTED, lambda: e.load_ensemble(*L.pack_streams(W, FIw, D), categories=(off, words)),
-               "tree %d node %d: feature index %d >= %d features" % (t0, node, F, F))
+        refused(lambda: e.load_ensemble(*L.pack_streams(W, FIw, D), categories=(off, words)), E.DTE_ERR_UNSUPPORTED,
+                "tree %d node %d: feature index %d >= %d features" % (t0, node, F, F))
         assert (e.infer_host(x)[0].view(np.uint32) == plain.view(np.uint32)).all()
         # a categorical load: every other kind is refused with a message naming the categorical calls
         e.load_ensemble(wl, fl, categories=(off, words))
@@ -340,27 +286,29 @@ def test_refusals(torch_cuda):
                   lambda: e.infer_device_leaves(dx, n, ds), lambda: e.kernel_name(), lambda: e.kernel_name_leaves(),
                   lambda: e.kernel_name_contribs()]
         for call in others:
-            raises(DTE_ERR_STATE, call, "a categorical ensemble is resident: walk it with dte_infer_device_categorical / "
-                                        "dte_infer_host_categorical")
-        raises(DTE_ERR_STATE, lambda: e.autotune(1000), "dte_autotune times the fp32 walk's plans")
+            refused(call, E.DTE_ERR_STATE, "a categorical ensemble is resident: walk it with dte_infer_device_categorical / "
+                                           "dte_infer_host_categorical")
+        refused(lambda: e.autotune(1000), E.DTE_ERR_STATE, "dte_autotune times the fp32 walk's plans")
         # misaligned pointers are refused before any launch
         raw = torch_cuda.empty(n * F + 8, dtype=torch_cuda.int32, device="cuda")
-        raises(DTE_ERR_ARG, lambda: e.infer_device_categorical(raw.data_ptr() + 4, n, ds), "dte_infer_device_categorical: d_tuples not 16-byte aligned")
-        raises(DTE_ERR_ARG, lambda: e.infer_device_categorical(dx, n, ds.data_ptr() + 2), "dte_infer_device_categorical: d_scores not 4-byte aligned")
+        refused(lambda: e.infer_device_categorical(raw.data_ptr() + 4, n, ds), E.DTE_ERR_ARG,
+                "dte_infer_device_categorical: d_tuples not 16-byte aligned")
+        refused(lambda: e.infer_device_categorical(dx, n, ds.data_ptr() + 2), E.DTE_ERR_ARG,
+                "dte_infer_device_categorical: d_scores not 4-byte aligned")
         # a tuple-only line stream cannot reuse a categorical ensemble
         regs = geometry_regs(T, D, F, K, 1, L.MISSING_DEFAULT, n)
         regs[201] = (regs[201] & ~0x2) | 0x1 | 0x40              # data_distributed, no host node: the run reuses the ensemble
         write_regs(e, regs)
-        raises(DTE_ERR_CONFIG, lambda: e.start(), "a categorical ensemble is resident: the line stream walks numeric trees only")
+        refused(lambda: e.start(), E.DTE_ERR_CONFIG, "a categorical ensemble is resident: the line stream walks numeric trees only")
         write_regs(e, geometry_regs(T, D, F, K, 1, L.MISSING_DEFAULT))
         assert (e.infer_host_categorical(x)[0].view(np.uint32) == want).all()
         # any other placement drops the categorical layout
         e.load_ensemble(wl, fl, covers=cov)
-        raises(DTE_ERR_STATE, lambda: e.infer_host_categorical(x), "dte_load_ensemble_categorical")
+        refused(lambda: e.infer_host_categorical(x), E.DTE_ERR_STATE, "dte_load_ensemble_categorical")
         e.load_ensemble(wl, fl, leaves=True)
-        raises(DTE_ERR_STATE, lambda: e.kernel_name_categorical(), "dte_load_ensemble_categorical")
+        refused(lambda: e.kernel_name_categorical(), E.DTE_ERR_STATE, "dte_load_ensemble_categorical")
         assert (e.infer_host(x)[0].view(np.uint32) == plain.view(np.uint32)).all()
         info = e.info()
         e.load_ensemble(wl, fl, categories=(off, words), leaves=True)   # no leaf layout next to a categorical one
-        raises(DTE_ERR_STATE, lambda: e.infer_host_leaves(x), "a categorical ensemble is resident")
+        refused(lambda: e.infer_host_leaves(x), E.DTE_ERR_STATE, "a categorical ensemble is resident")
         assert e.info()["ensemble_bytes"] > 0 and e.info()["num_classes"] == 1 and info["num_classes"] == 1

@@ -9,87 +9,24 @@ import pytest
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, L
+from helpers import (assert_words, device_rows, early, efficiency, geometry_regs, host_rows, make_engine,
+                     multi_node_regs, refused, torch_cuda, write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 from shap_ref import path_treeshap
 
 pytestmark = pytest.mark.gpu
 
 VARIANTS = [E.DTE_KERNEL_AUTO, E.DTE_KERNEL_TILE, E.DTE_KERNEL_GENERIC]
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG = -1, -2, -3
-U = 2.0 ** -24
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def early(FI, D, seed):
-    rng = np.random.default_rng(seed)
-    FI = FI.copy()
-    for t in range(1, FI.shape[0]):
-        lvl = int(rng.integers(0, D))
-        FI[t, (1 << lvl) - 1 + int(rng.integers(0, 1 << lvl))] |= 1 << 14
-    if FI.shape[0] > 2:
-        FI[2, 0] |= 1 << 14
-    return FI
-
-
-def device_contribs(torch, e, x, C, F, stream=None):
-    """[n, C, F + 1] from dte_infer_device_contribs, with a canary word row after the last row."""
-    n, row = x.shape[0], C * (F + 1)
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    buf = torch.full((n * row + 64,), 0x7A7A7A7A, dtype=torch.int32, device="cuda")
-    e.infer_device_contribs(dx, n, buf, stream=stream)
-    torch.cuda.synchronize()
-    got = buf.cpu().numpy()
-    assert (got[n * row:] == 0x7A7A7A7A).all(), "wrote past the last row"
-    return got[: n * row].view(np.float32).reshape(n, C, F + 1)
-
-
-def assert_words(got, want, what):
-    g, w = np.asarray(got, dtype=np.float32).view(np.uint32), np.asarray(want, dtype=np.float32).view(np.uint32)
-    assert g.shape == w.shape, (what, g.shape, w.shape)
-    bad = np.argwhere(g != w)
-    assert bad.size == 0, "%s: %d words differ, first at %s: %r instead of %r" % (
-        what, len(bad), tuple(bad[0]), g[tuple(bad[0])].view(np.float32), w[tuple(bad[0])].view(np.float32))
-
-
-def host3(e, x, C):
-    out = e.infer_host_contribs(x)
-    return out[:, None, :] if C == 1 else out
 
 
 def check_all(torch, e, x, want, C, F, variants=VARIANTS, what=""):
     for v in variants:
         e.set_kernel_variant(v)
-        assert_words(host3(e, x, C), want, "%s host %s %s" % (what, E.KERNEL_NAMES[v], e.kernel_name_contribs()))
+        assert_words(host_rows(e, "_contribs", x, C), want,
+                     "%s host %s %s" % (what, E.KERNEL_NAMES[v], e.kernel_name_contribs()))
         s = torch.cuda.Stream()
-        assert_words(device_contribs(torch, e, x, C, F, stream=s.cuda_stream), want,
+        assert_words(device_rows(torch, e, "_contribs", x, (C, F + 1), stream=s.cuda_stream), want,
                      "%s device %s %s" % (what, E.KERNEL_NAMES[v], e.kernel_name_contribs()))
     e.set_kernel_variant(E.DTE_KERNEL_AUTO)
-
-
-def efficiency(torch, e, x, phi, T_used_leaf_abs, T):
-    """phi [n, C, F + 1] against the same handle's dte_infer_device score words."""
-    n, C = x.shape[0], phi.shape[1]
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    ds = torch.empty(n * C, dtype=torch.float32, device="cuda")
-    e.infer_device(dx, n, ds)
-    score = ds.cpu().numpy().astype(np.float64).reshape(n, C)
-    p = phi.astype(np.float64)
-    bound = U * np.abs(p).sum(axis=2) + (T + 1) * U * T_used_leaf_abs + 1e-12 * T_used_leaf_abs
-    assert (np.abs(p.sum(axis=2) - score) <= bound).all()
 
 
 # (D, F): every depth of the contract's list, every F of the tile, 516 near the tile's shared-memory limit
@@ -143,7 +80,7 @@ def test_generic_launches_in_chunks(torch_cuda):
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, covers=cov)
         launches = e.info()["kernel_launches"]
-        assert_words(device_contribs(torch_cuda, e, x, 1, F), want, "device")
+        assert_words(device_rows(torch_cuda, e, "_contribs", x, (1, F + 1)), want, "device")
         assert e.info()["kernel_launches"] - launches == 2
 
 
@@ -188,8 +125,7 @@ def test_missing_pattern_rewritten_after_the_load(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, covers=cov)
-        for a, v in sorted(geometry_regs(T, D, F, 8, 2, 0x00000000).items()):
-            e.softreg_write(a, v)
+        write_regs(e, geometry_regs(T, D, F, 8, 2, 0x00000000))
         want = path_treeshap(W, FI, cov, x, D, F, missing=0x00000000)
         check_all(torch_cuda, e, x, want, 1, F, variants=[E.DTE_KERNEL_AUTO, E.DTE_KERNEL_GENERIC])
 
@@ -223,7 +159,7 @@ def test_many_classes_wide_rows(torch_cuda):
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, num_classes=C, covers=cov)
         assert e.kernel_name_contribs().startswith("dt_shap_generic<")
-        want = device_contribs(torch_cuda, e, x, C, F)
+        want = device_rows(torch_cuda, e, "_contribs", x, (C, F + 1))
         launches = e.info()["kernel_launches"]
         got = e.infer_host_contribs(x)
         assert e.info()["kernel_launches"] - launches == 3       # one dt_shap_generic launch per slot
@@ -243,8 +179,7 @@ def test_multi_device_handles(torch_cuda, mode):
         e.load_ensemble(wl, fl, covers=cov)
         single = e.infer_host_contribs(x)
     with ddt.Engine([0, 0, 0]) as e:
-        for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, mode).items()):
-            e.softreg_write(a, v)
+        write_regs(e, multi_node_regs(T, D, F, K, n, 3, mode))
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 64)
         e.load_ensemble(wl, fl, covers=cov)
         if mode == "data":
@@ -253,9 +188,7 @@ def test_multi_device_handles(torch_cuda, mode):
                 assert_words(e.infer_host_contribs(x), single, "Dealt %s" % E.KERNEL_NAMES[v])
             assert_words(single[:, None, :], path_treeshap(W, FI, cov, x, D, F), "single")
         else:
-            with pytest.raises(E.DteError) as ex:
-                e.infer_host_contribs(x)
-            assert ex.value.code == DTE_ERR_CONFIG
+            refused(lambda: e.infer_host_contribs(x), E.DTE_ERR_CONFIG)
         dx = torch_cuda.zeros((n, F), dtype=torch_cuda.float32, device="cuda")
         out = torch_cuda.empty(n * (F + 1), dtype=torch_cuda.float32, device="cuda")
         with pytest.raises(E.DteError):
@@ -274,35 +207,27 @@ def test_refusals(torch_cuda):
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl)                           # no contribution layout
         for call in (lambda: e.infer_host_contribs(x), lambda: e.infer_device_contribs(dx, n, out), e.kernel_name_contribs):
-            with pytest.raises(E.DteError) as ex:
-                call()
-            assert ex.value.code == DTE_ERR_STATE
+            refused(call, E.DTE_ERR_STATE)
         junk = cov.copy()
         junk[3, [7, 8, 9, 10, 15, 16]] = [0, -1, np.nan, np.inf, 0, -5]      # below the early leaf: never read
         e.load_ensemble(wl, fl, covers=junk)
         want = path_treeshap(W, FI, cov, x, D, F)
-        assert_words(host3(e, x, 1), want, "garbage below an early leaf")
+        assert_words(host_rows(e, "_contribs", x, 1), want, "garbage below an early leaf")
         scores = e.infer_host(x)[0]
         for cell, bad in ((0, 0.0), (4, -1.0), (1, np.nan), (20, np.inf), (30, 0.0)):
             c = cov.copy()
             c[5, cell] = bad
-            with pytest.raises(E.DteError) as ex:
-                e.load_ensemble(wl, fl, covers=c)
-            assert ex.value.code == DTE_ERR_ARG and "tree 5 cell %d" % cell in str(ex.value), str(ex.value)
-            assert_words(host3(e, x, 1), want, "after a refused load")           # the previous ensemble still answers
+            refused(lambda: e.load_ensemble(wl, fl, covers=c), E.DTE_ERR_ARG, "tree 5 cell %d" % cell)
+            assert_words(host_rows(e, "_contribs", x, 1), want, "after a refused load")   # the previous ensemble still answers
             assert (e.infer_host(x)[0].view(np.uint32) == scores.view(np.uint32)).all()
         for args in ((dx[:, 1:].reshape(-1)[1:], 1, out), (dx, n, out[1:].view(torch_cuda.uint8)[1:])):
-            with pytest.raises(E.DteError) as ex:
-                e.infer_device_contribs(*args)
-            assert ex.value.code == DTE_ERR_ARG
+            refused(lambda: e.infer_device_contribs(*args), E.DTE_ERR_ARG)
         for drop in (lambda: e.load_ensemble(wl, fl), lambda: e.load_ensemble(wl, fl, binned=True)):
             e.load_ensemble(wl, fl, covers=cov)
-            assert_words(host3(e, x, 1), want, "reloaded")
+            assert_words(host_rows(e, "_contribs", x, 1), want, "reloaded")
             drop()                                        # a later load without covers drops the layout
             for call in (lambda: e.infer_host_contribs(x), lambda: e.infer_device_contribs(dx, n, out)):
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE
+                refused(call, E.DTE_ERR_STATE)
 
 
 def test_line_stream_placement_drops_the_layout(torch_cuda):
@@ -315,15 +240,13 @@ def test_line_stream_placement_drops_the_layout(torch_cuda):
     with ddt.Engine(0) as e:
         e.configure(T, D, 4 * F, clusters=2, n_tuples=n)
         e.load_ensemble(wl, fl, covers=cov)
-        assert_words(host3(e, x, 1), path_treeshap(W, FI, cov, x, D, F), "before the stream")
+        assert_words(host_rows(e, "_contribs", x, 1), path_treeshap(W, FI, cov, x, D, F), "before the stream")
         e.start()
         e.stream_write(wl)
         e.stream_write(fl)
         e.stream_write(x)
         e.stream_flush()
-        with pytest.raises(E.DteError) as ex:
-            e.infer_host_contribs(x)
-        assert ex.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_contribs(x), E.DTE_ERR_STATE)
 
 
 def test_generic_scratch_follows_a_wider_reload(torch_cuda):
@@ -334,8 +257,7 @@ def test_generic_scratch_follows_a_wider_reload(torch_cuda):
     with make_engine(T, D, 4) as e:
         e.set_kernel_variant(E.DTE_KERNEL_GENERIC)
         for F, n, seed in ((4, 40000, 790), (1700, 32, 791), (4, 5000, 792)):
-            for a, v in sorted(geometry_regs(T, D, F, 8, 1, L.MISSING_DEFAULT).items()):
-                e.softreg_write(a, v)
+            write_regs(e, geometry_regs(T, D, F, 8, 1, L.MISSING_DEFAULT))
             W, FI = L.synth_ensemble(T, D, F, seed=seed)
             cov = L.synth_covers(FI, D, seed=seed)
             x = L.synth_tuples(0, n, F, seed=seed + 1, missing_ppm=50000)
@@ -343,8 +265,8 @@ def test_generic_scratch_follows_a_wider_reload(torch_cuda):
             e.load_ensemble(wl, fl, covers=cov)
             assert e.kernel_name_contribs() == "dt_shap_generic<3>"
             want = path_treeshap(W, FI, cov, x, D, F)
-            assert_words(device_contribs(torch_cuda, e, x, 1, F), want, "F=%d device" % F)
-            assert_words(host3(e, x, 1), want, "F=%d host" % F)
+            assert_words(device_rows(torch_cuda, e, "_contribs", x, (1, F + 1)), want, "F=%d device" % F)
+            assert_words(host_rows(e, "_contribs", x, 1), want, "F=%d host" % F)
 
 
 def test_headline_geometry(torch_cuda):

@@ -9,23 +9,16 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
-from helpers import oracle_scores, L
+from helpers import efficiency, make_engine, oracle_scores, torch_cuda, L  # noqa: F401 (torch_cuda: a fixture)
 from leaf_oracle import leaf_cells
 from shap_exact import exact_treeshap, leafwise_covers, leafwise_ensemble, leafwise_tuples
 from shap_ref import path_treeshap
-from test_gpu_contribs import check_all, efficiency, make_engine
+from test_gpu_contribs import check_all
 from test_shap_exact import bound_violations
 
 pytestmark = pytest.mark.gpu
 
 EXACT_TUPLES = 8                                    # tuples checked against exact TreeSHAP per case
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
 
 
 def leaf_abs(W, D, trees):

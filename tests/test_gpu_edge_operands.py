@@ -7,7 +7,8 @@ import pytest
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import MISSING_ROTATION, brute_bins, edge_ensemble, edge_table, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, oracle_cfg, L
+from helpers import (assert_scores, assert_words, geometry_regs, make_engine, multi_node_regs, oracle_words, torch_cuda,
+                     write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 from leaf_oracle import leaf_cells
 from oracle import oracle as O
 
@@ -16,57 +17,9 @@ pytestmark = pytest.mark.gpu
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K, S, missing):
-    e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
 def set_missing(e, r205, missing):
     """Rewrite only the low word of reg 205 (the missing pattern) of the value r205 written before; D, S and K stay."""
     e.softreg_write(205, (int(r205) & ~0xFFFFFFFF) | int(missing))
-
-
-def oracle_words(W, FI, x, D, K, S, C, missing):
-    """[n] (C = 1) or [n, C] oracle score words; tree t of the stream belongs to class t % C."""
-    kw = dict(threads=O.max_threads())
-    F = x.shape[1]
-    if C == 1:
-        return O.scores(oracle_cfg(D, K, S, missing, F, W.shape[0]), *L.pack_streams(W, FI, D), x, **kw)
-    out = np.zeros((x.shape[0], C), dtype=np.uint32)
-    for c in range(C):
-        if W[c::C].shape[0]:
-            out[:, c] = O.scores(oracle_cfg(D, K, S, missing, F, W[c::C].shape[0]), *L.pack_streams(W[c::C], FI[c::C], D), x, **kw)
-    return out
-
-
-def labels_of(want, C):
-    """C = 1: score > 0 (label 0 at +0); C >= 2: the first class of maximal score."""
-    return O.labels(want) if C == 1 else np.argmax(want.view(np.float32), axis=1).astype(np.uint8)
-
-
-def assert_words(sc, lb, want, C, what):
-    got = np.asarray(sc).view(np.uint32).reshape(want.shape)
-    bad = np.argwhere(got != want)
-    assert bad.size == 0, "%s: %d words differ, first at %s: got %08x want %08x" % (
-        what, len(bad), bad[0], got[tuple(bad[0])], want[tuple(bad[0])])
-    if lb is not None:
-        lw = labels_of(want, C)
-        bad = np.flatnonzero(np.asarray(lb) != lw)
-        assert bad.size == 0, "%s: %d labels differ, first at tuple %d: got %d want %d" % (what, bad.size, bad[0], lb[bad[0]], lw[bad[0]])
-
-
-def assert_same(got, want, what):
-    bad = np.argwhere(np.asarray(got) != want)
-    assert bad.size == 0, "%s: %d differ, first at %s: got %s want %s" % (what, len(bad), bad[0], got[tuple(bad[0])], want[tuple(bad[0])])
 
 
 def every_path(torch, e, W, FI, x, D, K, S, C, missing, what, binned=True, leaves=True):
@@ -75,7 +28,7 @@ def every_path(torch, e, W, FI, x, D, K, S, C, missing, what, binned=True, leave
     n, F = x.shape
     want = oracle_words(W, FI, x, D, K, S, C, missing)
     sc, lb = e.infer_host(x)
-    assert_words(sc, lb, want, C, "%s infer_host" % what)
+    assert_scores(sc, lb, want, C, "%s infer_host" % what)
     st = torch.cuda.Stream()
     dx = torch.from_numpy(x.view(np.int32)).cuda()
     shape = (n, C) if C > 1 else (n,)
@@ -84,28 +37,28 @@ def every_path(torch, e, W, FI, x, D, K, S, C, missing, what, binned=True, leave
     torch.cuda.synchronize()
     e.infer_device(dx, n, ds, dl, stream=st.cuda_stream)
     st.synchronize()
-    assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "%s infer_device" % what)
+    assert_scores(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "%s infer_device" % what)
     if binned:
         off, edges = e.bin_edges()
         b = L.bin_tuples(x, off, edges, missing)
         sc, lb = e.infer_host_binned(b)
-        assert_words(sc, lb, want, C, "%s infer_host_binned" % what)
+        assert_scores(sc, lb, want, C, "%s infer_host_binned" % what)
         db = torch.empty((n, F), dtype=torch.uint8, device="cuda")
         e.bin_tuples_device(dx, n, db, stream=st.cuda_stream)
         ds.fill_(float("nan"))
         dl.fill_(77)
         e.infer_device_binned(db, n, ds, dl, stream=st.cuda_stream)
         st.synchronize()
-        assert_same(db.cpu().numpy(), b, "%s bin_tuples_device" % what)
-        assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "%s infer_device_binned" % what)
+        assert_words(db.cpu().numpy(), b, "%s bin_tuples_device" % what)
+        assert_scores(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "%s infer_device_binned" % what)
     if leaves:
         T = W.shape[0]
         cells = leaf_cells(W, FI, x, D, missing)
-        assert_same(e.infer_host_leaves(x), cells, "%s infer_host_leaves" % what)
+        assert_words(e.infer_host_leaves(x), cells, "%s infer_host_leaves" % what)
         out = torch.full((n * T,), 0x7777, dtype=torch.int16, device="cuda")
         e.infer_device_leaves(dx, n, out, stream=st.cuda_stream)
         st.synchronize()
-        assert_same(out.cpu().numpy().view(np.uint16).reshape(n, T), cells, "%s infer_device_leaves" % what)
+        assert_words(out.cpu().numpy().view(np.uint16).reshape(n, T), cells, "%s infer_device_leaves" % what)
     return want
 
 
@@ -156,7 +109,7 @@ def test_device_binning_at_the_edges(torch_cuda, F):
             dx = torch_cuda.from_numpy(X.view(np.int32)).cuda()
             db = torch_cuda.full((n, F), 0x5A, dtype=torch_cuda.uint8, device="cuda")
             e.bin_tuples_device(dx, n, db)
-            assert_same(db.cpu().numpy(), brute_bins(X, off, edges, missing), "F=%d missing=%08x" % (F, missing))
+            assert_words(db.cpu().numpy(), brute_bins(X, off, edges, missing), "F=%d missing=%08x" % (F, missing))
 
 
 # ---- don't-care nodes ---------------------------------------------------------------------------------------------------
@@ -257,15 +210,14 @@ def test_class_labels_of_a_chunked_handle_at_ties(torch_cuda):
     with ddt.Engine([0] * G) as e:
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 4096)
         regs = multi_node_regs(T, D, F, K, n, G, "ensemble", batch_tuples=64)
-        for a, val in sorted(regs.items()):
-            e.softreg_write(a, val)
+        write_regs(e, regs)
         set_missing(e, regs[205], missing)
         e.load_ensemble(*L.pack_streams(W, FI, D), num_classes=C, binned=True)
         sc, lb = e.infer_host(x)
-        assert_words(sc, lb, want, C, "chunked C=3 infer_host")
+        assert_scores(sc, lb, want, C, "chunked C=3 infer_host")
         off, edges = e.bin_edges()
         sc, lb = e.infer_host_binned(L.bin_tuples(x, off, edges, missing))
-        assert_words(sc, lb, want, C, "chunked C=3 infer_host_binned")
+        assert_scores(sc, lb, want, C, "chunked C=3 infer_host_binned")
 
 
 # ---- multi-device handles -----------------------------------------------------------------------------------------------
@@ -283,12 +235,11 @@ def test_multi_device_handles_on_edge_data(torch_cuda, mode):
     with ddt.Engine([0] * G) as e:
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 5000)
         regs = multi_node_regs(T, D, F, K, n, G, mode, batch_tuples=64)
-        for a, val in sorted(regs.items()):
-            e.softreg_write(a, val)
+        write_regs(e, regs)
         set_missing(e, regs[205], missing)
         e.load_ensemble(*L.pack_streams(W, FI, D), binned=True)
         sc, lb = e.infer_host(x)
-        assert_words(sc, lb, want, 1, "%s infer_host" % mode)
+        assert_scores(sc, lb, want, 1, "%s infer_host" % mode)
         off, edges = e.bin_edges()
         sc, lb = e.infer_host_binned(L.bin_tuples(x, off, edges, missing))
-        assert_words(sc, lb, want, 1, "%s infer_host_binned" % mode)
+        assert_scores(sc, lb, want, 1, "%s infer_host_binned" % mode)

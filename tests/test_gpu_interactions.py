@@ -10,85 +10,26 @@ import pytest
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, L
+from helpers import (U, assert_words, device_rows, early, geometry_regs, host_rows, make_engine, multi_node_regs,
+                     refused, torch_cuda, write_regs, CANARY, L)  # noqa: F401 (torch_cuda: a fixture)
 from shap_exact import leafwise_covers, leafwise_ensemble, leafwise_tuples
 from shap_inter_ref import path_interactions
 
 pytestmark = pytest.mark.gpu
 
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG, DTE_ERR_UNSUPPORTED = -1, -2, -3, -4
-U = 2.0 ** -24
-CANARY = 0x7A7A7A7A
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def early(FI, D, seed):
-    rng = np.random.default_rng(seed)
-    FI = FI.copy()
-    for t in range(1, FI.shape[0]):
-        lvl = int(rng.integers(0, D))
-        FI[t, (1 << lvl) - 1 + int(rng.integers(0, 1 << lvl))] |= 1 << 14
-    return FI
-
-
-def device_inter(torch, e, x, C, F, stream=None):
-    """[n, C, F + 1, F + 1] from dte_infer_device_interactions, with canary words after the last row."""
-    n, row = x.shape[0], C * (F + 1) * (F + 1)
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    buf = torch.full((n * row + 64,), CANARY, dtype=torch.int32, device="cuda")
-    e.infer_device_interactions(dx, n, buf, stream=stream)
-    torch.cuda.synchronize()
-    got = buf.cpu().numpy()
-    assert (got[n * row:] == CANARY).all(), "wrote past the last row"
-    return got[: n * row].view(np.float32).reshape(n, C, F + 1, F + 1)
-
-
-def device_contribs(torch, e, x, C, F):
-    n = x.shape[0]
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    out = torch.empty(n * C * (F + 1), dtype=torch.float32, device="cuda")
-    e.infer_device_contribs(dx, n, out)
-    return out.cpu().numpy().reshape(n, C, F + 1)
-
-
-def assert_words(got, want, what):
-    g, w = np.asarray(got, dtype=np.float32).view(np.uint32), np.asarray(want, dtype=np.float32).view(np.uint32)
-    assert g.shape == w.shape, (what, g.shape, w.shape)
-    bad = np.argwhere(g != w)
-    assert bad.size == 0, "%s: %d words differ, first at %s: %r instead of %r" % (
-        what, len(bad), tuple(bad[0]), g[tuple(bad[0])].view(np.float32), w[tuple(bad[0])].view(np.float32))
-
-
-def host4(e, x, C):
-    out = e.infer_host_interactions(x)
-    return out[:, None] if C == 1 else out
-
 
 def check_both(torch, e, x, want, C, F, what=""):
     """Host call, device call on a torch side stream: every word equal to want."""
-    assert_words(host4(e, x, C), want, "%s host %s" % (what, e.kernel_name_interactions()))
+    assert_words(host_rows(e, "_interactions", x, C), want, "%s host %s" % (what, e.kernel_name_interactions()))
     s = torch.cuda.Stream()
-    assert_words(device_inter(torch, e, x, C, F, stream=s.cuda_stream), want, "%s device %s" % (what, e.kernel_name_interactions()))
+    assert_words(device_rows(torch, e, "_interactions", x, (C, F + 1, F + 1), stream=s.cuda_stream), want,
+                 "%s device %s" % (what, e.kernel_name_interactions()))
 
 
 def against_other_walks(torch, e, x, inter, leaf_abs, T):
     """inter [n, C, F + 1, F + 1] against the same handle's contribution and score words."""
     n, C, F = x.shape[0], inter.shape[1], inter.shape[2] - 1
-    phi = device_contribs(torch, e, x, C, F)
+    phi = device_rows(torch, e, "_contribs", x, (C, F + 1))
     assert_words(inter[:, :, F, F], phi[:, :, F], "bias word")
     assert (inter[:, :, F, :F] == 0).all() and (inter[:, :, :F, F] == 0).all()
     p = inter.astype(np.float64)
@@ -118,7 +59,7 @@ def test_depths_and_widths(torch_cuda, D, F):
     T, n = 11, 9 if F > 100 else 6 if D >= 12 else 40
     W, FI = L.synth_ensemble(T, D, F, seed=800 + D * 7 + F)
     if D >= 2:
-        FI = early(FI, D, 801 + D)
+        FI = early(FI, D, 801 + D, root_tree=None)
     cov = L.synth_covers(FI, D, seed=D)
     x = L.synth_tuples(0, n, F, seed=802 + D, missing_ppm=50000)
     wl, fl = L.pack_streams(W, FI, D)
@@ -148,7 +89,7 @@ def test_classes_and_a_chunk(torch_cuda):
     """C = 3 on stream trees [2, 12) of 14: class of stream tree s = s % 3, every tree of every class."""
     T_all, D, F, first, cnt, n = 14, 4, 20, 2, 10, 50
     W, FI = L.synth_ensemble(T_all, D, F, seed=820)
-    FI = early(FI, D, 821)
+    FI = early(FI, D, 821, root_tree=None)
     cov = L.synth_covers(FI, D, seed=822)
     x = L.synth_tuples(0, n, F, seed=823, missing_ppm=50000)
     wl, fl = L.pack_streams(W, FI, D)
@@ -185,8 +126,7 @@ def test_missing_pattern_rewritten_after_the_load(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, covers=cov)
-        for a, v in sorted(geometry_regs(T, D, F, 8, 2, 0x00000000).items()):
-            e.softreg_write(a, v)
+        write_regs(e, geometry_regs(T, D, F, 8, 2, 0x00000000))
         check_both(torch_cuda, e, x, path_interactions(W, FI, cov, x, D, F, missing=0x00000000), 1, F)
 
 
@@ -194,7 +134,7 @@ def test_missing_pattern_rewritten_after_the_load(torch_cuda):
 def test_tuple_counts(torch_cuda, n):
     T, D, F = 6, 3, 4
     W, FI = L.synth_ensemble(T, D, F, seed=850)
-    FI = early(FI, D, 851)
+    FI = early(FI, D, 851, root_tree=None)
     cov = L.synth_covers(FI, D, seed=852)
     x = L.synth_tuples(0, n, F, seed=853, missing_ppm=50000)
     wl, fl = L.pack_streams(W, FI, D)
@@ -259,7 +199,7 @@ def test_row_blocks_give_the_same_bytes(torch_cuda):
     tuples (24 on 132 SMs); these 70 tuples let it take all 41 rows in one pass."""
     T, D, F, n = 7, 6, 40, 70
     W, FI = L.synth_ensemble(T, D, F, seed=880)
-    FI = early(FI, D, 881)
+    FI = early(FI, D, 881, root_tree=None)
     cov = L.synth_covers(FI, D, seed=882)
     x = L.synth_tuples(0, n, F, seed=883, missing_ppm=50000)
     wl, fl = L.pack_streams(W, FI, D)
@@ -273,9 +213,9 @@ def test_row_blocks_give_the_same_bytes(torch_cuda):
             if B:
                 assert e.kernel_name_interactions() == "dt_shap_inter<7> rows=%d" % B
             launches = e.info()["kernel_launches"]
-            assert_words(device_inter(torch_cuda, e, x, 1, F), want, "B=%d" % B)
+            assert_words(device_rows(torch_cuda, e, "_interactions", x, (1, F + 1, F + 1)), want, "B=%d" % B)
             assert e.info()["kernel_launches"] - launches == -(-(F + 1) // (B or F + 1))
-            assert_words(host4(e, x, 1), want, "host B=%d" % B)
+            assert_words(host_rows(e, "_interactions", x, 1), want, "host B=%d" % B)
 
 
 @pytest.mark.parametrize("mode", ["data", "ensemble"])
@@ -284,7 +224,7 @@ def test_multi_device_handles(torch_cuda, mode):
     refuses; the device call is refused on any multi-device handle."""
     T, D, F, K, n = 20, 5, 16, 2, 300
     W, FI = L.synth_ensemble(T, D, F, seed=890)
-    FI = early(FI, D, 891)
+    FI = early(FI, D, 891, root_tree=None)
     cov = L.synth_covers(FI, D, seed=892)
     x = L.synth_tuples(0, n, F, seed=893, missing_ppm=20000)
     wl, fl = L.pack_streams(W, FI, D)
@@ -292,22 +232,17 @@ def test_multi_device_handles(torch_cuda, mode):
         e.load_ensemble(wl, fl, covers=cov)
         single = e.infer_host_interactions(x)
     with ddt.Engine([0, 0, 0]) as e:
-        for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, mode).items()):
-            e.softreg_write(a, v)
+        write_regs(e, multi_node_regs(T, D, F, K, n, 3, mode))
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 64)
         e.load_ensemble(wl, fl, covers=cov)
         if mode == "data":
             assert_words(e.infer_host_interactions(x), single, "data-sharded")
             assert_words(single[:, None], path_interactions(W, FI, cov, x, D, F), "single")
         else:
-            with pytest.raises(E.DteError) as ex:
-                e.infer_host_interactions(x)
-            assert ex.value.code == DTE_ERR_CONFIG
+            refused(lambda: e.infer_host_interactions(x), E.DTE_ERR_CONFIG)
         dx = torch_cuda.zeros((n, F), dtype=torch_cuda.float32, device="cuda")
         out = torch_cuda.empty(n * (F + 1) ** 2, dtype=torch_cuda.float32, device="cuda")
-        with pytest.raises(E.DteError) as ex:
-            e.infer_device_interactions(dx, n, out)
-        assert ex.value.code == DTE_ERR_UNSUPPORTED
+        refused(lambda: e.infer_device_interactions(dx, n, out), E.DTE_ERR_UNSUPPORTED)
 
 
 def test_refusals(torch_cuda):
@@ -323,23 +258,17 @@ def test_refusals(torch_cuda):
         e.load_ensemble(wl, fl)                           # no contribution layout
         for call in (lambda: e.infer_host_interactions(x), lambda: e.infer_device_interactions(dx, n, out),
                      e.kernel_name_interactions):
-            with pytest.raises(E.DteError) as ex:
-                call()
-            assert ex.value.code == DTE_ERR_STATE
+            refused(call, E.DTE_ERR_STATE)
         e.load_ensemble(wl, fl, covers=cov)
         for args in ((dx[:, 1:].reshape(-1)[1:], 1, out), (dx, n, out[1:].view(torch_cuda.uint8)[1:])):
-            with pytest.raises(E.DteError) as ex:
-                e.infer_device_interactions(*args)
-            assert ex.value.code == DTE_ERR_ARG
-            assert_words(host4(e, x, 1), want, "after a misaligned pointer")
+            refused(lambda: e.infer_device_interactions(*args), E.DTE_ERR_ARG)
+            assert_words(host_rows(e, "_interactions", x, 1), want, "after a misaligned pointer")
         for drop in (lambda: e.load_ensemble(wl, fl), lambda: e.load_ensemble(wl, fl, binned=True)):
             e.load_ensemble(wl, fl, covers=cov)
-            assert_words(host4(e, x, 1), want, "reloaded")
+            assert_words(host_rows(e, "_interactions", x, 1), want, "reloaded")
             drop()                                        # a later load without covers drops the layout
             for call in (lambda: e.infer_host_interactions(x), lambda: e.infer_device_interactions(dx, n, out)):
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE
+                refused(call, E.DTE_ERR_STATE)
             assert e.infer_host(x)[0].shape == (n,)       # the ensemble itself still answers
 
 
@@ -356,9 +285,7 @@ def test_row_over_64_mib(torch_cuda):
         e.load_ensemble(wl, fl, num_classes=4, covers=cov)
         launches = e.info()["kernel_launches"]
         for call in (lambda: e.infer_host_interactions(x), lambda: e.infer_device_interactions(dx, n, out)):
-            with pytest.raises(E.DteError) as ex:
-                call()
-            assert ex.value.code == DTE_ERR_UNSUPPORTED and "64 MiB" in str(ex.value)
+            refused(call, E.DTE_ERR_UNSUPPORTED, "64 MiB")
         assert e.info()["kernel_launches"] == launches
         phi = e.infer_host_contribs(x)                    # the handle still answers the other walks
         assert phi.shape == (n, 4, F + 1)
@@ -377,12 +304,10 @@ def test_line_stream_placement_drops_the_layout(torch_cuda):
     with ddt.Engine(0) as e:
         e.configure(T, D, 4 * F, clusters=2, n_tuples=n)
         e.load_ensemble(wl, fl, covers=cov)
-        assert_words(host4(e, x, 1), path_interactions(W, FI, cov, x, D, F), "before the stream")
+        assert_words(host_rows(e, "_interactions", x, 1), path_interactions(W, FI, cov, x, D, F), "before the stream")
         e.start()
         e.stream_write(wl)
         e.stream_write(fl)
         e.stream_write(x)
         e.stream_flush()
-        with pytest.raises(E.DteError) as ex:
-            e.infer_host_interactions(x)
-        assert ex.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_interactions(x), E.DTE_ERR_STATE)

@@ -12,42 +12,12 @@ import pytest
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, multi_node_regs, L
+from helpers import (assert_words, device_rows, early, efficiency, geometry_regs, host_rows, make_engine,
+                     multi_node_regs, refused, torch_cuda, write_regs, CANARY, L)  # noqa: F401 (torch_cuda: a fixture)
 from interv_ref import interventional
 from shap_ref import end_cells
 
 pytestmark = pytest.mark.gpu
-
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG, DTE_ERR_UNSUPPORTED = -1, -2, -3, -4
-U = 2.0 ** -24
-CANARY = 0x7A7A7A7A
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def early(FI, D, seed):
-    """Bit 14 on one random node of every tree but the first, and on the root of tree 2."""
-    rng = np.random.default_rng(seed)
-    FI = FI.copy()
-    for t in range(1, FI.shape[0]):
-        lvl = int(rng.integers(0, D))
-        FI[t, (1 << lvl) - 1 + int(rng.integers(0, 1 << lvl))] |= 1 << 14
-    if FI.shape[0] > 2:
-        FI[2, 0] |= 1 << 14
-    return FI
 
 
 def leafwise(FI, D, M, seed):
@@ -67,31 +37,6 @@ def leafwise(FI, D, M, seed):
     return FI
 
 
-def device_interv(torch, e, x, C, F, stream=None):
-    """[n, C, F + 1] from dte_infer_device_interventional, with a canary row after the last row."""
-    n, row = x.shape[0], C * (F + 1)
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    buf = torch.full((n * row + 64,), CANARY, dtype=torch.int32, device="cuda")
-    e.infer_device_interventional(dx, n, buf, stream=stream)
-    torch.cuda.synchronize()
-    got = buf.cpu().numpy()
-    assert (got[n * row:] == CANARY).all(), "wrote past the last row"
-    return got[: n * row].view(np.float32).reshape(n, C, F + 1)
-
-
-def assert_words(got, want, what):
-    g, w = np.asarray(got, dtype=np.float32).view(np.uint32), np.asarray(want, dtype=np.float32).view(np.uint32)
-    assert g.shape == w.shape, (what, g.shape, w.shape)
-    bad = np.argwhere(g != w)
-    assert bad.size == 0, "%s: %d words differ, first at %s: %r instead of %r" % (
-        what, len(bad), tuple(bad[0]), g[tuple(bad[0])].view(np.float32), w[tuple(bad[0])].view(np.float32))
-
-
-def host3(e, x, C):
-    out = e.infer_host_interventional(x)
-    return out[:, None, :] if C == 1 else out
-
-
 def check_all(torch, e, x, want, C, F, what=""):
     """Host words, and device words on a torch side stream, against want; every forced variant names the same kernel."""
     name = e.kernel_name_interventional()
@@ -100,24 +45,11 @@ def check_all(torch, e, x, want, C, F, what=""):
         e.set_kernel_variant(v)
         assert e.kernel_name_interventional() == name
     e.set_kernel_variant(E.DTE_KERNEL_AUTO)
-    assert_words(host3(e, x, C), want, "%s host %s" % (what, name))
+    assert_words(host_rows(e, "_interventional", x, C), want, "%s host %s" % (what, name))
     s = torch.cuda.Stream()
-    assert_words(device_interv(torch, e, x, C, F, stream=s.cuda_stream), want, "%s device %s" % (what, name))
+    assert_words(device_rows(torch, e, "_interventional", x, (C, F + 1), stream=s.cuda_stream), want,
+                 "%s device %s" % (what, name))
     return name
-
-
-def efficiency(torch, e, x, phi, leaf_abs, T):
-    """phi [n, C, F + 1] against the same handle's dte_infer_device score words.  In exact arithmetic sum phi + bias is
-    the tuple's score (the sum of its leaf words); the words carry one fp32 rounding each (U |word|) and the fp64 roundings
-    before them (far below 1e-12 of the leaf magnitudes), and the score word (T + 1) fp32 roundings of its leaf sum."""
-    n, C = x.shape[0], phi.shape[1]
-    dx = torch.from_numpy(np.ascontiguousarray(x).view(np.int32)).cuda()
-    ds = torch.empty(n * C, dtype=torch.float32, device="cuda")
-    e.infer_device(dx, n, ds)
-    score = ds.cpu().numpy().astype(np.float64).reshape(n, C)
-    p = phi.astype(np.float64)
-    bound = U * np.abs(p).sum(axis=2) + (T + 1) * U * leaf_abs + 1e-12 * leaf_abs
-    assert (np.abs(p.sum(axis=2) - score) <= bound).all()
 
 
 def early_leaf_abs(W, FI, D, trees):
@@ -259,10 +191,9 @@ def test_missing_pattern_rewritten_after_the_load(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, background=bg)
-        before = host3(e, x, 1)
+        before = host_rows(e, "_interventional", x, 1)
         assert_words(before, interventional(W, FI, x, bg, D, F), "default pattern")
-        for a, v in sorted(geometry_regs(T, D, F, 8, 2, 0x00000000).items()):
-            e.softreg_write(a, v)
+        write_regs(e, geometry_regs(T, D, F, 8, 2, 0x00000000))
         want = interventional(W, FI, x, bg, D, F, missing=0x00000000)
         assert (want[:, 0, F] != before[:, 0, F]).any()                 # the bias moved with the pattern
         check_all(torch_cuda, e, x, want, 1, F, what="pattern 0")
@@ -283,16 +214,13 @@ def test_multi_device_handles(torch_cuda, mode):
         single = e.infer_host_interventional(x)
     assert_words(single[:, None, :], interventional(W, FI, x, bg, D, F), "single")
     with ddt.Engine([0, 0, 0]) as e:
-        for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, mode).items()):
-            e.softreg_write(a, v)
+        write_regs(e, multi_node_regs(T, D, F, K, n, 3, mode))
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 64)
         e.load_ensemble(wl, fl, background=bg)
         if mode == "data":
             assert_words(e.infer_host_interventional(x), single, "Dealt")
         else:
-            with pytest.raises(E.DteError) as ex:
-                e.infer_host_interventional(x)
-            assert ex.value.code == DTE_ERR_CONFIG
+            refused(lambda: e.infer_host_interventional(x), E.DTE_ERR_CONFIG)
         dx = torch_cuda.zeros((n, F), dtype=torch_cuda.float32, device="cuda")
         out = torch_cuda.empty(n * (F + 1), dtype=torch_cuda.float32, device="cuda")
         with pytest.raises(E.DteError):
@@ -316,48 +244,38 @@ def test_refusals(torch_cuda):
                      lambda: e.load_ensemble(wl, fl, covers=cov, approx=True)):
             load()                                        # no interventional layout
             for call in calls:
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE and "dte_load_ensemble_interventional" in str(ex.value)
+                refused(call, E.DTE_ERR_STATE, "dte_load_ensemble_interventional")
         for kw in (dict(covers=cov), dict(approx=True, covers=cov), dict(binned=True)):
             with pytest.raises(ValueError):
                 e.load_ensemble(wl, fl, background=bg, **kw)
         e.load_ensemble(wl, fl, background=bg)
-        assert_words(host3(e, x, 1), want, "loaded")
+        assert_words(host_rows(e, "_interventional", x, 1), want, "loaded")
         for narrow in (bg[:, : F - 4], np.zeros((N, F + 4), dtype=np.uint32), bg.reshape(-1)):
             with pytest.raises(ValueError):               # rows of another width than register 204's F
                 e.load_ensemble(wl, fl, background=narrow)
-        assert_words(host3(e, x, 1), want, "after a refused background width")
+        assert_words(host_rows(e, "_interventional", x, 1), want, "after a refused background width")
         for call in (lambda: e.infer_host_contribs(x), lambda: e.infer_host_approx_contribs(x)):
-            with pytest.raises(E.DteError) as ex:          # the other attribution layouts are not built by this load
-                call()
-            assert ex.value.code == DTE_ERR_STATE
+            refused(call, E.DTE_ERR_STATE)                # the other attribution layouts are not built by this load
         lib, h = e._lib, e._h
-        for ptr, cnt, code in ((None, N, DTE_ERR_ARG), (bg, 0, DTE_ERR_ARG), (bg, 1 << 32, DTE_ERR_ARG)):
+        for ptr, cnt, code in ((None, N, E.DTE_ERR_ARG), (bg, 0, E.DTE_ERR_ARG), (bg, 1 << 32, E.DTE_ERR_ARG)):
             rc = lib.dte_load_ensemble_interventional(h, wl.ctypes.data, wl.nbytes // 16, fl.ctypes.data, fl.nbytes // 16,
                                                       0, 0, 1, None if ptr is None else C.c_void_p(ptr.ctypes.data), cnt)
             assert rc == code
-            assert_words(host3(e, x, 1), want, "after a refused load")            # the previous layout still answers
+            assert_words(host_rows(e, "_interventional", x, 1), want, "after a refused load")   # the previous layout still answers
         bad = FI.copy()
         bad[7, 2] = (bad[7, 2] & ~np.uint16(0x7FF)) | np.uint16(F + 3)
         bwl, bfl = L.pack_streams(W, bad, D)
-        with pytest.raises(E.DteError) as ex:
-            e.load_ensemble(bwl, bfl, background=bg)
-        assert ex.value.code == DTE_ERR_UNSUPPORTED
-        assert_words(host3(e, x, 1), want, "after a refused feature index")
+        refused(lambda: e.load_ensemble(bwl, bfl, background=bg), E.DTE_ERR_UNSUPPORTED)
+        assert_words(host_rows(e, "_interventional", x, 1), want, "after a refused feature index")
         for args in ((dx[:, 1:].reshape(-1)[1:], 1, out), (dx, n, out[1:].view(torch_cuda.uint8)[1:])):
-            with pytest.raises(E.DteError) as ex:
-                e.infer_device_interventional(*args)
-            assert ex.value.code == DTE_ERR_ARG
+            refused(lambda: e.infer_device_interventional(*args), E.DTE_ERR_ARG)
         for drop in (lambda: e.load_ensemble(wl, fl), lambda: e.load_ensemble(wl, fl, binned=True),
                      lambda: e.load_ensemble(wl, fl, covers=cov), lambda: e.load_ensemble(wl, fl, covers=cov, approx=True)):
             e.load_ensemble(wl, fl, background=bg)
-            assert_words(host3(e, x, 1), want, "reloaded")
+            assert_words(host_rows(e, "_interventional", x, 1), want, "reloaded")
             drop()                                        # a later load of any other kind drops the layout
             for call in calls[:2]:
-                with pytest.raises(E.DteError) as ex:
-                    call()
-                assert ex.value.code == DTE_ERR_STATE
+                refused(call, E.DTE_ERR_STATE)
 
 
 def test_line_stream_placement_drops_the_layout(torch_cuda):
@@ -370,12 +288,10 @@ def test_line_stream_placement_drops_the_layout(torch_cuda):
     with ddt.Engine(0) as e:
         e.configure(T, D, 4 * F, clusters=2, n_tuples=n)
         e.load_ensemble(wl, fl, background=bg)
-        assert_words(host3(e, x, 1), interventional(W, FI, x, bg, D, F), "before the stream")
+        assert_words(host_rows(e, "_interventional", x, 1), interventional(W, FI, x, bg, D, F), "before the stream")
         e.start()
         e.stream_write(wl)
         e.stream_write(fl)
         e.stream_write(x)
         e.stream_flush()
-        with pytest.raises(E.DteError) as ex:
-            e.infer_host_interventional(x)
-        assert ex.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_interventional(x), E.DTE_ERR_STATE)

@@ -9,63 +9,27 @@ from the table shows that the live planner (SM count, opt-in shared memory) disa
 The edge tests then drive single kernels to the depths, feature counts, record formats, tuple and tree counts, class
 layouts, ring-fill knobs, pointer alignments and 64-bit offsets where a tile kernel could go wrong without the
 headline geometry noticing.  Bar everywhere: every score word and every label equals the oracle's."""
-import collections
-import lzma
 import os
 import re
 
 import numpy as np
 import pytest
 
-import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_leaves
-from helpers import geometry_regs, oracle_scores, L
-from oracle import oracle as O
+from helpers import (assert_scores, labels_of, make_engine, oracle_words, plan_groups, plan_rows, refused, torch_cuda,
+                     L)  # noqa: F401 (torch_cuda: a fixture)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-TABLE = os.path.join(HERE, "golden", "plan_table.txt.xz")
 KERNELS = os.path.join(os.path.dirname(HERE), "distributed-decisiontrees_b200", "csrc", "dte_kernels.cuh")
 
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
-DTE_ERR_ARG = -1
 SANITIZER = bool(os.environ.get("DTE_TEST_SANITIZER"))
 
 
 # ---- the plan table ------------------------------------------------------------------------------------------------
-class Row(collections.namedtuple("Row", "tune D F C variant name")):
-    @property
-    def template(self):
-        """Kernel template of the row: "dt_walk_tile<4, 2, 1, 0, 384>" or "dt_walk_generic<1>"."""
-        return self.name.split(">")[0] + ">"
-
-
-def plan_rows():
-    """Rows of the plan table in file order: (DTE_TUNE pin, D, F, C, requested variant, kernel name)."""
-    rows, tune = [], None
-    with lzma.open(TABLE, "rt") as f:
-        for line in f:
-            line = line.rstrip("\n")
-            if line.startswith("DTE_TUNE="):
-                tune = line[len("DTE_TUNE="):]
-                continue
-            D, F, C, variant, _phased, name = line.split(" ", 5)
-            rows.append(Row(tune, int(D), int(F), int(C), int(variant), name))
-    return rows
-
-
-ROWS = plan_rows()
+ROWS = plan_rows("plan_table.txt.xz")
 NAME_OF = {(r.tune, r.D, r.F, r.C, r.variant): r.name for r in ROWS}
-
-
-def kernel_groups():
-    """{(template, C): (typical row, extreme row)}, groups in order of first appearance.  Typical: the smallest
-    (|D - 10|, F), extreme: the largest (D, F); ties go to the first row in table order."""
-    groups = collections.OrderedDict()
-    for r in ROWS:
-        groups.setdefault((r.template, r.C), []).append(r)
-    return collections.OrderedDict(
-        (k, (min(rs, key=lambda r: (abs(r.D - 10), r.F)), max(rs, key=lambda r: (r.D, r.F)))) for k, rs in groups.items())
 
 
 def compiled_templates():
@@ -88,7 +52,7 @@ def compiled_templates():
 def matrix_cases():
     """(row, None): the typical and the extreme row of every group on the standard data."""
     out = []
-    for (template, C), (typical, extreme) in kernel_groups().items():
+    for (template, C), (typical, extreme) in plan_groups(ROWS).items():
         for kind, row in (("typical", typical), ("extreme", extreme)):
             out.append(pytest.param(row, None, id="%s-C%d-%s-D%d-F%d" % (template.replace(" ", ""), C, kind, row.D, row.F)))
     return out
@@ -98,7 +62,7 @@ def edge_cases():
     """(row, missing pattern): the typical row of every group on edge operands (tests/edge_operands.py), the missing
     pattern taken from MISSING_ROTATION by group index."""
     out = []
-    for i, ((template, C), (typical, _)) in enumerate(kernel_groups().items()):
+    for i, ((template, C), (typical, _)) in enumerate(plan_groups(ROWS).items()):
         missing = MISSING_ROTATION[i % len(MISSING_ROTATION)]
         out.append(pytest.param(typical, missing, id="%s-C%d-edge-D%d-F%d-m%08x" % (
             template.replace(" ", ""), C, typical.D, typical.F, missing)))
@@ -106,20 +70,6 @@ def edge_cases():
 
 
 # ---- helpers --------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K, S, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
 def tuples(first, n, F, seed, missing_ppm=15000):
     """L.synth_tuples in pieces of ~4 M words, so a wide batch does not hold several full-size temporaries."""
     out = np.empty((n, F), dtype=np.uint32)
@@ -141,35 +91,6 @@ def ensemble(T, D, F, seed, max_index=None):
     return W, FI
 
 
-def oracle_words(W, FI, x, D, K, S, C, missing=L.MISSING_DEFAULT):
-    """uint32 words [n] (C = 1) or [n, C]: column c is the oracle's score of the class-c trees alone (tree t of the
-    stream belongs to class t % C); a class without trees scores +0."""
-    kw = dict(threads=O.max_threads())
-    if C == 1:
-        return oracle_scores(W, FI, x, D, K, S, missing, **kw)
-    out = np.zeros((x.shape[0], C), dtype=np.uint32)
-    for c in range(C):
-        if W[c::C].shape[0]:
-            out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, missing, **kw)
-    return out
-
-
-def oracle_labels(want, C):
-    """C = 1: score > 0; C >= 2: the first class of maximal score."""
-    if C == 1:
-        return O.labels(want)
-    return np.argmax(want.view(np.float32), axis=1).astype(np.uint8)
-
-
-def assert_words(sc, lb, want, C, what):
-    got = np.asarray(sc).view(np.uint32).reshape(want.shape)
-    bad = np.argwhere(got != want)
-    assert bad.size == 0, "%s: %d words differ, first at %s: got %08x want %08x" % (
-        what, len(bad), bad[0], got[tuple(bad[0])], want[tuple(bad[0])])
-    if lb is not None:
-        assert (np.asarray(lb) == oracle_labels(want, C)).all(), what + ": labels differ"
-
-
 def check(W, FI, x, D, K, S, C=1, variants=VARIANTS, want=None):
     """Every requested variant on one engine against the oracle; returns (oracle words, {variant: kernel name})."""
     T, F = W.shape[0], x.shape[1]
@@ -183,7 +104,7 @@ def check(W, FI, x, D, K, S, C=1, variants=VARIANTS, want=None):
             e.set_kernel_variant(v)
             names[v] = e.kernel_name()
             sc, lb = e.infer_host(x)
-            assert_words(sc, lb, want, C, "variant %s (%s)" % (E.KERNEL_NAMES[v], names[v]))
+            assert_scores(sc, lb, want, C, "variant %s (%s)" % (E.KERNEL_NAMES[v], names[v]))
     return want, names
 
 
@@ -205,7 +126,7 @@ def test_plan_table_reaches_42_kernel_groups():
     """The planner reaches 21 of the 26 walk templates, each single- and multi-class: 42 (template, C) groups, each with
     a typical and an extreme row, and every template it names is one that kTileFamilies instantiates.  A planner change
     that makes another kernel reachable shows up here as a count, not as a kernel no GPU test launches."""
-    groups = kernel_groups()
+    groups = plan_groups(ROWS)
     assert len(groups) == 42
     compiled = compiled_templates()
     assert len(compiled) == 26                            # x 2 (single-, multi-class) = the 52 walk kernels of libdte.so
@@ -264,7 +185,7 @@ def test_reachable_instantiation_bit_exact(row, missing, monkeypatch, torch_cuda
             assert cap < n
             want = oracle_words(Wl, FI, x, D, K, S, C, missing)
             sc, lb = e.infer_host(x)
-            assert_words(sc, lb, want, C, "infer_host %s" % row.name)
+            assert_scores(sc, lb, want, C, "infer_host %s" % row.name)
             st = torch.cuda.Stream()
             with torch.cuda.stream(st):
                 dx = torch.from_numpy(x.view(np.int32)).cuda()
@@ -272,7 +193,7 @@ def test_reachable_instantiation_bit_exact(row, missing, monkeypatch, torch_cuda
                 dl = torch.full((n,), 77, dtype=torch.uint8, device="cuda")
                 e.infer_device(dx, n, ds, dl, stream=st.cuda_stream)
             st.synchronize()
-            assert_words(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "infer_device %s" % row.name)
+            assert_scores(ds.cpu().numpy(), dl.cpu().numpy(), want, C, "infer_device %s" % row.name)
             del dx, ds, dl
 
 
@@ -383,7 +304,7 @@ def test_tuple_count_edges(tune, monkeypatch):
             want = oracle_words(W, FI, x, D, K, S, 1)
             for n in ns:
                 sc, lb = e.infer_host(x[:n])
-                assert_words(sc, lb, want[:n], 1, "%s n=%d" % (e.kernel_name(), n))
+                assert_scores(sc, lb, want[:n], 1, "%s n=%d" % (e.kernel_name(), n))
 
 
 @pytest.mark.gpu
@@ -419,7 +340,7 @@ def test_one_group_per_class(tune, pref, monkeypatch, torch_cuda):
         st = torch.cuda.current_stream().cuda_stream
         e.infer_device_accumulate(dx, x.shape[0], acc, stream=st)
         torch.cuda.synchronize()
-        assert_words(acc.cpu().numpy(), None, want, C, "accumulate %s" % e.kernel_name())
+        assert_scores(acc.cpu().numpy(), None, want, C, "accumulate %s" % e.kernel_name())
 
 
 @pytest.mark.gpu
@@ -434,7 +355,7 @@ def test_classes_without_trees():
     x = tuples(0, 3001, F, seed=6102, missing_ppm=20000)
     want, _ = check(W, FI, x, D, 1, 1, C)
     assert (want[:, 3:] == 0).all() and (want[:, :3].view(np.float32) < 0).all()
-    assert (oracle_labels(want, C) == 3).all()
+    assert (labels_of(want, C) == 3).all()
 
 
 @pytest.mark.gpu
@@ -447,7 +368,7 @@ def test_256_classes():
     W[255, n_int:] = (W[255, n_int:].view(np.float32) * np.float32(4096.0)).view(np.uint32)
     x = tuples(0, 2000, F, seed=6202, missing_ppm=20000)
     want, names = check(W, FI, x, D, 1, 1, C)
-    lab = oracle_labels(want, C)
+    lab = labels_of(want, C)
     assert (lab == 255).any() and (lab != 255).any()
     assert all(n.endswith(" classes=256") for n in names.values())
 
@@ -496,19 +417,15 @@ def test_misaligned_device_pointers_are_refused(torch_cuda):
             e.set_kernel_variant(v)
             for call in (lambda t, s: e.infer_device(t, n, s, None, stream=st),
                          lambda t, s: e.infer_device_accumulate(t, n, s, stream=st)):
-                with pytest.raises(E.DteError) as ei:
-                    call(dx.data_ptr() + 4, ds.data_ptr())
-                assert ei.value.code == DTE_ERR_ARG and "d_tuples not 16-byte aligned" in str(ei.value)
-                with pytest.raises(E.DteError) as ei:
-                    call(dx.data_ptr(), ds.data_ptr() + 2)
-                assert ei.value.code == DTE_ERR_ARG and "not 4-byte aligned" in str(ei.value)
+                refused(lambda: call(dx.data_ptr() + 4, ds.data_ptr()), E.DTE_ERR_ARG, "d_tuples not 16-byte aligned")
+                refused(lambda: call(dx.data_ptr(), ds.data_ptr() + 2), E.DTE_ERR_ARG, "not 4-byte aligned")
         torch.cuda.synchronize()
         for v in VARIANTS:
             e.set_kernel_variant(v)
             out = torch.full((n,), float("nan"), dtype=torch.float32, device="cuda")
             e.infer_device(dx, n, out, None, stream=st)
             torch.cuda.synchronize()
-            assert_words(out.cpu().numpy(), None, want, 1, "aligned call after refusals, %s" % e.kernel_name())
+            assert_scores(out.cpu().numpy(), None, want, 1, "aligned call after refusals, %s" % e.kernel_name())
 
 
 @pytest.mark.gpu
@@ -548,4 +465,4 @@ def test_tuple_offsets_beyond_4_gib(F, torch_cuda):
     for first, count in ((0, 256), (n - 512, 512)):
         x = L.synth_tuples(first, count, F, seed=seed, missing_ppm=15000)
         want = oracle_words(W, FI, x, D, K, S, 1)
-        assert_words(got[first:first + count], None, want, 1, "%s tuples %d..%d" % (name, first, first + count))
+        assert_scores(got[first:first + count], None, want, 1, "%s tuples %d..%d" % (name, first, first + count))

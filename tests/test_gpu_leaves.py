@@ -3,52 +3,20 @@
 Bar everywhere: every cell equals the oracle's (tests/leaf_oracle.py: the oracle's own walk over trees whose end
 cells are labelled with their index), and the scores rebuilt from the cells with the oracle's adder equal the same
 handle's score words."""
-import collections
-import lzma
-import os
-
 import numpy as np
 import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples
-from helpers import geometry_regs, multi_node_regs, L
+from helpers import (assert_words, early, make_engine, multi_node_regs, plan_groups, plan_rows, refused, torch_cuda,
+                     write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 from leaf_oracle import leaf_cells
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-TABLE = os.path.join(HERE, "golden", "plan_table_leaf.txt.xz")
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
-DTE_ERR_ARG, DTE_ERR_STATE = -1, -2
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K=8, S=None, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    S = S if S is not None else max(1, -(-T // (8 * K)))
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def early(FI, D, seed):
-    rng = np.random.default_rng(seed)
-    FI = FI.copy()
-    for t in range(1, FI.shape[0]):
-        lvl = int(rng.integers(0, D))
-        FI[t, (1 << lvl) - 1 + int(rng.integers(0, 1 << lvl))] |= 1 << 14
-    if FI.shape[0] > 2:
-        FI[2, 0] |= 1 << 14
-    return FI
 
 
 def device_leaves(torch, e, x, T, stream=None, offset=0):
@@ -62,12 +30,6 @@ def device_leaves(torch, e, x, T, stream=None, offset=0):
     return out.cpu().numpy().view(np.uint16).reshape(n, T)
 
 
-def assert_cells(got, want, what):
-    bad = np.argwhere(got != want)
-    assert bad.size == 0, "%s: %d cells differ; tuple %d tree %d: cell %d instead of %d" % (
-        what, len(bad), bad[0][0], bad[0][1], got[tuple(bad[0])], want[tuple(bad[0])])
-
-
 def run(torch, T, D, F, n, seed, C=1, variants=VARIANTS, early_leaves=True, K=8, S=None):
     W, FI = L.synth_ensemble(T, D, F, seed=seed)
     if early_leaves and D >= 2:
@@ -79,39 +41,19 @@ def run(torch, T, D, F, n, seed, C=1, variants=VARIANTS, early_leaves=True, K=8,
         e.load_ensemble(wl, fl, num_classes=C, leaves=True)
         for v in variants:
             e.set_kernel_variant(v)
-            assert_cells(e.infer_host_leaves(x), want, "host %s" % E.KERNEL_NAMES[v])
+            assert_words(e.infer_host_leaves(x), want, "host %s" % E.KERNEL_NAMES[v])
             s = torch.cuda.Stream()
-            assert_cells(device_leaves(torch, e, x, T, stream=s.cuda_stream), want, "device %s" % E.KERNEL_NAMES[v])
+            assert_words(device_leaves(torch, e, x, T, stream=s.cuda_stream), want, "device %s" % E.KERNEL_NAMES[v])
     return W, FI, x, want
-
-
-Row = collections.namedtuple("Row", "tune D F C variant name")
-
-
-def plan_rows():
-    rows, tune = [], None
-    with lzma.open(TABLE, "rt") as f:
-        for line in f:
-            line = line.rstrip("\n")
-            if line.startswith("DTE_TUNE="):
-                tune = line[len("DTE_TUNE="):]
-                continue
-            D, F, C, variant, _phased, name = line.split(" ", 5)
-            rows.append(Row(tune, int(D), int(F), int(C), int(variant), name))
-    return rows
 
 
 def matrix_cases():
     """(row, whole, missing): one typical and one extreme row per (leaf kernel template, C) of the leaf plan table, each
     at a ragged and at a whole T on the standard data (missing None); then the typical row of every group at the ragged
     T on edge operands (tests/edge_operands.py), the missing pattern taken from MISSING_ROTATION by group index."""
-    groups = collections.OrderedDict()
-    for r in plan_rows():
-        groups.setdefault((r.name.split(">")[0] + ">", r.C), []).append(r)
     out, edge = [], []
-    for i, ((t, C), rs) in enumerate(groups.items()):
-        typical = min(rs, key=lambda r: (abs(r.D - 10), r.F))
-        for kind, r in (("typical", typical), ("extreme", max(rs, key=lambda r: (r.D, r.F)))):
+    for i, ((t, C), (typical, extreme)) in enumerate(plan_groups(plan_rows("plan_table_leaf.txt.xz")).items()):
+        for kind, r in (("typical", typical), ("extreme", extreme)):
             for whole, wid in ((False, "T-ragged"), (True, "T-whole")):
                 out.append(pytest.param(r, whole, None, id="%s-C%d-%s-D%d-F%d-%s" % (t.replace(" ", ""), C, kind, r.D, r.F, wid)))
         m = MISSING_ROTATION[i % len(MISSING_ROTATION)]
@@ -154,7 +96,7 @@ def test_every_reachable_leaf_kernel(torch_cuda, row, whole, missing, monkeypatc
             x = L.synth_tuples(0, n, F, seed=801, missing_ppm=20000)
         want = leaf_cells(W, FI, x, D, missing)
         s = torch_cuda.cuda.Stream()
-        assert_cells(device_leaves(torch_cuda, e, x, T, stream=s.cuda_stream), want, name)
+        assert_words(device_leaves(torch_cuda, e, x, T, stream=s.cuda_stream), want, name)
 
 
 @pytest.mark.parametrize("D", list(range(1, 16)))
@@ -175,7 +117,7 @@ def test_small_batches(torch_cuda, n):
             got = e.infer_host_leaves(x)
             assert got.shape == (n, T)
             if n:
-                assert_cells(got, leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "n=%d" % n)
+                assert_words(got, leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "n=%d" % n)
 
 
 def test_tile_edges_over_several_waves(torch_cuda):
@@ -190,7 +132,7 @@ def test_tile_edges_over_several_waves(torch_cuda):
             M = int(e.info()["tuples_per_cta"])
             for n in (3 * 132 * M - 1, 3 * 132 * M + 1, M - 1, M + 1):
                 x = L.synth_tuples(0, n, F, seed=962, missing_ppm=20000)
-                assert_cells(device_leaves(torch_cuda, e, x, T), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "n=%d" % n)
+                assert_words(device_leaves(torch_cuda, e, x, T), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "n=%d" % n)
 
 
 def test_trees_beyond_the_score_slots(torch_cuda):
@@ -209,8 +151,8 @@ def test_classes_with_a_chunk_and_256_classes(torch_cuda):
         e.load_ensemble(wl, fl, first_tree=first, num_local_trees=cnt, num_classes=3, leaves=True)
         for v in VARIANTS:
             e.set_kernel_variant(v)
-            assert_cells(e.infer_host_leaves(x), want, "C=3 %s" % E.KERNEL_NAMES[v])
-            assert_cells(device_leaves(torch_cuda, e, x, cnt), want, "C=3 device %s" % E.KERNEL_NAMES[v])
+            assert_words(e.infer_host_leaves(x), want, "C=3 %s" % E.KERNEL_NAMES[v])
+            assert_words(device_leaves(torch_cuda, e, x, cnt), want, "C=3 device %s" % E.KERNEL_NAMES[v])
     run(torch_cuda, 300, 6, 16, 300, 990, C=256, variants=[E.DTE_KERNEL_AUTO, E.DTE_KERNEL_GENERIC])
 
 
@@ -261,7 +203,7 @@ def test_large_output_offset(torch_cuda):
         e.infer_device_leaves(dx, n, out)
         tail = out[(n - 500) * T:].cpu().numpy().view(np.uint16).reshape(500, T)
         x = L.synth_tuples(n - 500, 500, F, seed=5, missing_ppm=20000)
-        assert_cells(tail, leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "rows past 4 GiB")
+        assert_words(tail, leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "rows past 4 GiB")
         del out, dx
 
 
@@ -280,7 +222,7 @@ def test_ordered_with_torch_work_on_a_stream(torch_cuda):
             e.infer_device_leaves(dx, n, out, stream=s.cuda_stream)
             got = out.view(n, T).to("cpu", non_blocking=True)
         s.synchronize()
-        assert_cells(got.numpy().view(np.uint16), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "stream")
+        assert_words(got.numpy().view(np.uint16), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "stream")
 
 
 def test_refusals_and_binned_load(torch_cuda):
@@ -293,22 +235,16 @@ def test_refusals_and_binned_load(torch_cuda):
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl)                            # no leaf layout
         for call in (lambda: e.infer_host_leaves(x), lambda: e.infer_device_leaves(dx, n, out), e.kernel_name_leaves):
-            with pytest.raises(E.DteError) as ex:
-                call()
-            assert ex.value.code == DTE_ERR_STATE
+            refused(call, E.DTE_ERR_STATE)
         base = e.info()["ensemble_bytes"]
         e.load_ensemble(wl, fl, leaves=True)
         assert e.info()["ensemble_bytes"] > base
         for bad_x, bad_o in ((dx.view(-1)[1:], out), (dx, out[1:]), (dx, out[4:])):
-            with pytest.raises(E.DteError) as ex:
-                e.infer_device_leaves(bad_x, n - 1, bad_o)
-            assert ex.value.code == DTE_ERR_ARG
+            refused(lambda: e.infer_device_leaves(bad_x, n - 1, bad_o), E.DTE_ERR_ARG)
         e.load_ensemble(wl, fl, binned=True, leaves=True)  # a binned load with the option on answers the fp32 leaf calls
-        assert_cells(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "binned load")
+        assert_words(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "binned load")
         e.load_ensemble(wl, fl)                            # a placement without the option drops the layout
-        with pytest.raises(E.DteError) as ex:
-            e.infer_host_leaves(x)
-        assert ex.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_leaves(x), E.DTE_ERR_STATE)
         assert e.info()["ensemble_bytes"] == base
 
 
@@ -327,7 +263,7 @@ def test_line_stream_placement(torch_cuda):
         e.stream_write(fl)
         e.stream_write(x)
         e.stream_flush()
-        assert_cells(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "line stream")
+        assert_words(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "line stream")
 
 
 @pytest.mark.parametrize("mode", ["data", "ensemble"])
@@ -340,13 +276,12 @@ def test_multi_device_handles(torch_cuda, mode):
     wl, fl = L.pack_streams(W, FI, D)
     want = leaf_cells(W, FI, x, D, L.MISSING_DEFAULT)
     with ddt.Engine([0, 0, 0]) as e:
-        for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, mode).items()):
-            e.softreg_write(a, v)
+        write_regs(e, multi_node_regs(T, D, F, K, n, 3, mode))
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 256)
         e.load_ensemble(wl, fl, leaves=True)
         for v in (E.DTE_KERNEL_AUTO, E.DTE_KERNEL_GENERIC):
             e.set_kernel_variant(v)
-            assert_cells(e.infer_host_leaves(x), want, "%s %s" % (mode, E.KERNEL_NAMES[v]))
+            assert_words(e.infer_host_leaves(x), want, "%s %s" % (mode, E.KERNEL_NAMES[v]))
 
 
 def test_headline_leaf_plan_multi_tile(torch_cuda):
@@ -362,7 +297,7 @@ def test_headline_leaf_plan_multi_tile(torch_cuda):
         assert name.startswith("dt_walk_tile_leaf<4, 2, 1, 0, 384>") and "phased=1" in name, name
         n = 3 * 132 * int(e.info()["tuples_per_cta"]) - 5
         x = L.synth_tuples(0, n, F, seed=1062, missing_ppm=20000)
-        assert_cells(device_leaves(torch_cuda, e, x, T), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), name)
+        assert_words(device_leaves(torch_cuda, e, x, T), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), name)
 
 
 def test_many_trees_few_features(torch_cuda):
@@ -374,5 +309,5 @@ def test_many_trees_few_features(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F) as e:
         e.load_ensemble(wl, fl, leaves=True)
-        assert_cells(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "T=2048, F=4")
+        assert_words(e.infer_host_leaves(x), leaf_cells(W, FI, x, D, L.MISSING_DEFAULT), "T=2048, F=4")
 

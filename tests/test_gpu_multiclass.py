@@ -12,13 +12,12 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
-from helpers import geometry_regs, multi_node_regs, oracle_scores, L
+from helpers import labels_of, make_engine, multi_node_regs, oracle_scores, refused, torch_cuda, write_regs, L  # noqa: F401
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
 
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
-DTE_ERR_ARG, DTE_ERR_CONFIG = -1, -3
 
 
 def oracle_class_scores(W, FI, x, D, K, S, missing, C, tree_range=None):
@@ -34,27 +33,9 @@ def oracle_class_scores(W, FI, x, D, K, S, missing, C, tree_range=None):
     return out
 
 
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K, S, devs=0):
-    e = ddt.Engine(devs)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, L.MISSING_DEFAULT).items()):
-        e.softreg_write(a, v)
-    return e
-
-
 def slots_for(T, nc, K):
     """Smallest S whose S*K*8 slots hold the largest class."""
     return -(-(-(-T // nc)) // (8 * K))
-
-
-def argmax_labels(words):
-    return np.argmax(words.view(np.float32), axis=1).astype(np.uint8)       # first maximum wins
 
 
 def check_mc(W, FI, x, D, K, S, nc, variants=VARIANTS, singles=True):
@@ -71,7 +52,7 @@ def check_mc(W, FI, x, D, K, S, nc, variants=VARIANTS, singles=True):
             got = sc.view(np.uint32)
             bad = np.argwhere(got != want)
             assert bad.size == 0, "variant %s (%s): %d words differ, first at %s" % (E.KERNEL_NAMES[v], e.kernel_name(), len(bad), bad[0])
-            assert (lb == argmax_labels(want)).all()
+            assert (lb == labels_of(want, nc)).all()
     if singles:
         # the same words from C single-class handles, each loaded with every C-th tree
         for c in range(nc):
@@ -132,7 +113,7 @@ def test_multiclass_headline_geometry_multi_tile(capsys):
             print("\n[multiclass-plan] DTE_TUNE=%r -> %s" % (os.environ.get("DTE_TUNE", ""), name))
         sc, lb = e.infer_host(x)
         assert e.info()["tuples_per_cta"] * e.info()["sm_count"] < n
-    assert (sc.view(np.uint32) == want).all() and (lb == argmax_labels(want)).all()
+    assert (sc.view(np.uint32) == want).all() and (lb == labels_of(want, nc)).all()
 
 
 def test_device_pointer_path_and_accumulate(torch_cuda):
@@ -157,13 +138,13 @@ def test_device_pointer_path_and_accumulate(torch_cuda):
         st.synchronize()
         got = ds.cpu().numpy().view(np.uint32)
         assert (got == want).all()
-        assert (dl.cpu().numpy() == argmax_labels(want)).all()
+        assert (dl.cpu().numpy() == labels_of(want, nc)).all()
         assert (acc.cpu().numpy().view(np.uint32) == want).all()
         # the device-side argmax over the same matrix
         dl2 = torch.zeros(n, dtype=torch.uint8, device="cuda")
         e.class_labels_device(ds, n, nc, dl2, stream=st.cuda_stream)
         st.synchronize()
-        assert (dl2.cpu().numpy() == argmax_labels(want)).all()
+        assert (dl2.cpu().numpy() == labels_of(want, nc)).all()
 
 
 def test_ties_go_to_the_lower_class():
@@ -185,7 +166,7 @@ def test_ties_go_to_the_lower_class():
     want = check_mc(W3, FI3, x, D, K, slots_for(W3.shape[0], 3, K), 3, variants=[E.DTE_KERNEL_AUTO, E.DTE_KERNEL_GENERIC], singles=False)
     s1 = want[:, 1].view(np.float32)
     assert (want[:, 1] == want[:, 2]).all() and (s1 > 0).any() and (s1 < 0).any()
-    assert (argmax_labels(want) == np.where(s1 > 0, 1, 0)).all()
+    assert (labels_of(want, 3) == np.where(s1 > 0, 1, 0)).all()
 
 
 def test_one_class_through_the_new_call_is_the_old_call():
@@ -253,8 +234,7 @@ def test_multi_device_handle_dealt_and_chunked(devs):
                 else _mc_ring_reference(W, FI, x, D, K, S, nc, G))
         with ddt.Engine(devs) as e:
             e.set_option(E.DTE_OPT_CHUNK_TUPLES, 700)      # several landing buffers, chunks that are not line-aligned x C
-            for a, v in sorted(regs.items()):
-                e.softreg_write(a, v)
+            write_regs(e, regs)
             e.load_ensemble(wl, fl, num_classes=nc)
             info = e.info()
             assert info["num_classes"] == nc and info["partition"] == (1 if mode == "data" else 2)
@@ -262,7 +242,7 @@ def test_multi_device_handle_dealt_and_chunked(devs):
                 sc, lb = e.infer_host(x)
                 assert sc.shape == (n, nc)
                 assert (sc.view(np.uint32) == want).all(), mode
-                assert (lb == argmax_labels(want)).all(), mode
+                assert (lb == labels_of(want, nc)).all(), mode
             assert e.info()["tuples_out"] - info["tuples_out"] == 2 * n       # tuples, not score words
 
 
@@ -281,12 +261,11 @@ def test_multi_device_nccl_combine(devs):
     with ddt.Engine(devs) as e:
         e.set_option(E.DTE_OPT_COMBINE, 1)
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 4096)
-        for a, v in sorted(regs.items()):
-            e.softreg_write(a, v)
+        write_regs(e, regs)
         e.load_ensemble(wl, fl, num_classes=nc)
         sc, lb = e.infer_host(x)
         assert np.allclose(sc, want.view(np.float32), rtol=1e-5, atol=1e-7)
-        assert (lb == argmax_labels(sc.view(np.uint32))).all()
+        assert (lb == labels_of(sc.view(np.uint32), nc)).all()
 
 
 def test_two_engines_adjacent_chunks_ring_combined(torch_cuda):
@@ -320,7 +299,7 @@ def test_two_engines_adjacent_chunks_ring_combined(torch_cuda):
     engines[0].class_labels_device(out, n, nc, lab, stream=st)
     torch.cuda.synchronize()
     assert (out.cpu().numpy().view(np.uint32) == want).all()
-    assert (lab.cpu().numpy() == argmax_labels(want)).all()
+    assert (lab.cpu().numpy() == labels_of(want, nc)).all()
     for e in engines:
         e.close()
 
@@ -332,22 +311,16 @@ def test_refusals_and_info():
     wl, fl = L.pack_streams(W, FI, D)
     with make_engine(T, D, F, K, 1) as e:                # S*K*8 = 16 slots
         for bad in (0, 257):
-            with pytest.raises(E.DteError) as ei:
-                e.load_ensemble(wl, fl, num_classes=bad)
-            assert ei.value.code == DTE_ERR_ARG
+            refused(lambda: e.load_ensemble(wl, fl, num_classes=bad), E.DTE_ERR_ARG)
         e.load_ensemble(wl, fl, num_classes=2)            # 20 trees per class > 16 slots
         assert e.info()["num_classes"] == 2
-        with pytest.raises(E.DteError) as ei:
-            e.infer_host(x)
-        assert ei.value.code == DTE_ERR_CONFIG and "S >= 2" in str(ei.value)
+        refused(lambda: e.infer_host(x), E.DTE_ERR_CONFIG, "S >= 2")
         e.load_ensemble(wl, fl, num_classes=3)            # 14 / 13 / 13 trees fit 16 slots
         sc, lb = e.infer_host(x)
         assert sc.shape == (n, 3) and (sc.view(np.uint32) == oracle_class_scores(W, FI, x, D, K, 1, L.MISSING_DEFAULT, 3)).all()
         # a data-only line-stream run would reuse the resident 3-class ensemble: the result stream has one score per tuple
         e.softreg_write(201, 0x41 | ((F // 4) << 32))     # data_distributed | pcie_receiver_enabled, not host node
-        with pytest.raises(E.DteError) as ei:
-            e.start()
-        assert ei.value.code == DTE_ERR_CONFIG
+        refused(e.start, E.DTE_ERR_CONFIG)
         # a single-class load makes the same data-only run legal again
         e.load_ensemble(wl, fl)
         assert e.info()["num_classes"] == 1
@@ -356,8 +329,8 @@ def test_refusals_and_info():
     with make_engine(T, D, F, K, 1) as e:
         assert e.info()["num_classes"] == 0               # nothing resident
         lib = e._lib
-        assert lib.dte_class_labels_device(e._h, None, 0, 0, None, None) == DTE_ERR_ARG
-        assert lib.dte_class_labels_device(e._h, None, 0, 257, None, None) == DTE_ERR_ARG
+        assert lib.dte_class_labels_device(e._h, None, 0, 0, None, None) == E.DTE_ERR_ARG
+        assert lib.dte_class_labels_device(e._h, None, 0, 257, None, None) == E.DTE_ERR_ARG
 
 
 def test_autotune_on_a_multiclass_ensemble():
@@ -372,4 +345,4 @@ def test_autotune_on_a_multiclass_ensemble():
         rep = e.autotune(100_000)
         assert "chosen: dt_walk_tile<" in rep and "classes=10" in rep, rep
         sc, lb = e.infer_host(x)
-        assert (sc.view(np.uint32) == want).all() and (lb == argmax_labels(want)).all()
+        assert (sc.view(np.uint32) == want).all() and (lb == labels_of(want, nc)).all()

@@ -8,47 +8,19 @@ import pytest
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
 from edge_operands import edge_ensemble, edge_tuples
-from helpers import geometry_regs, multi_node_regs, oracle_scores, L
-from oracle import oracle as O
+from helpers import (assert_words, geometry_regs, make_engine, multi_node_regs, oracle_words, refused, torch_cuda,
+                     write_regs, L)  # noqa: F401 (torch_cuda: a fixture)
 from sparse_ref import densify, density_mask, sparse_rows
 
 pytestmark = pytest.mark.gpu
 
 VARIANTS = [E.DTE_KERNEL_GENERIC, E.DTE_KERNEL_TILE, E.DTE_KERNEL_TILE_STAGED, E.DTE_KERNEL_AUTO]
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_UNSUPPORTED = -1, -2, -4
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-def make_engine(T, D, F, K, S, missing=L.MISSING_DEFAULT):
-    e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, missing).items()):
-        e.softreg_write(a, v)
-    return e
-
-
-def oracle_words(W, FI, x, D, K, S, C, missing):
-    kw = dict(threads=O.max_threads())
-    if C == 1:
-        return oracle_scores(W, FI, x, D, K, S, missing, **kw)
-    out = np.zeros((x.shape[0], C), dtype=np.uint32)
-    for c in range(C):
-        out[:, c] = oracle_scores(W[c::C], FI[c::C], x, D, K, S, missing, **kw)
-    return out
 
 
 def assert_same(got, want, what):
     """(scores, labels) against (scores, labels), word for word."""
-    g, w = np.asarray(got[0]).view(np.uint32), np.asarray(want[0]).view(np.uint32)
-    bad = np.argwhere(g != w)
-    assert bad.size == 0, "%s: %d score words differ, first at %s" % (what, len(bad), bad[0])
-    if want[1] is not None:
-        assert (np.asarray(got[1]) == np.asarray(want[1])).all(), what + ": labels differ"
+    assert_words(got[0], want[0], what + ": scores")
+    assert_words(got[1], want[1], what + ": labels")
 
 
 def to_device(torch, indptr, indices, values):
@@ -233,8 +205,7 @@ def test_multi_device_handles(torch_cuda, mode):
     regs = multi_node_regs(T, D, F, K, n, G, mode, batch_tuples=64)
     with ddt.Engine([0] * G) as e:
         e.set_option(E.DTE_OPT_CHUNK_TUPLES, 900)
-        for a, v in sorted(regs.items()):
-            e.softreg_write(a, v)
+        write_regs(e, regs)
         e.load_ensemble(wl, fl)
         ref = e.infer_host(dense)
         for _ in range(2):
@@ -245,9 +216,7 @@ def test_multi_device_handles(torch_cuda, mode):
             e.host_free(p)
         assert_same(e.infer_host(dense), ref, mode + ", dense after sparse")
         for call in (lambda: e.infer_device_sparse(0, 0, 0, 0, 0), lambda: e.sparse_to_dense_device(0, 0, 0, 0, 0)):
-            with pytest.raises(E.DteError) as ei:
-                call()
-            assert ei.value.code == DTE_ERR_UNSUPPORTED
+            refused(call, E.DTE_ERR_UNSUPPORTED)
     if mode == "data":
         S = (regs[205] >> 36) & 0xFF
         with make_engine(T, D, F, K, S) as e:
@@ -290,9 +259,7 @@ def test_refusals_before_any_launch(torch_cuda):
     wl, fl = L.pack_streams(W, FI, D)
     rows = sparse_rows(x, density_mask(n, F, 0.5, 902), 903)
     with make_engine(T, D, F, K, S) as e:
-        with pytest.raises(E.DteError) as ei:                  # no ensemble
-            e.infer_host_sparse(rows)
-        assert ei.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_sparse(rows), E.DTE_ERR_STATE)        # no ensemble
         e.load_ensemble(wl, fl)
         info = e.info()
         p, i, v = to_device(torch, *rows)
@@ -301,29 +268,21 @@ def test_refusals_before_any_launch(torch_cuda):
         P, I, V, B, SC = p.data_ptr(), i.data_ptr(), v.data_ptr(), big.data_ptr(), sc.data_ptr()
         for args in ((P + 4, I, V), (P, I + 2, V), (P, I, V + 2)):
             for call in (lambda a: e.infer_device_sparse(*a, n, SC), lambda a: e.sparse_to_dense_device(*a, n, B)):
-                with pytest.raises(E.DteError) as ei:
-                    call(args)
-                assert ei.value.code == DTE_ERR_ARG and "aligned" in str(ei.value)
+                refused(lambda: call(args), E.DTE_ERR_ARG, "aligned")
         for call in (lambda: e.infer_device_sparse(P, I, V, n, SC + 2), lambda: e.sparse_to_dense_device(P, I, V, n, B + 4),
                      lambda: e.infer_device_sparse(P, I, V, n, SC, absent=2 ** 32)):
-            with pytest.raises(E.DteError) as ei:
-                call()
-            assert ei.value.code == DTE_ERR_ARG
+            refused(call, E.DTE_ERR_ARG)
         hp, hi, hv = rows
         raw = np.zeros(hp.size + 1, dtype=np.int64)
         mis = raw.view(np.uint8)[4:4 + 8 * hp.size].view(np.int64)       # 4 bytes off an 8-byte boundary
         mis[:] = hp
         fn = e._lib.dte_infer_host_sparse
         out = np.empty(n, np.float32)
-        assert fn(e._h, E._ptr(mis), E._ptr(hi), E._ptr(hv), n, E.DTE_SPARSE_ABSENT_MISSING, E._ptr(out), None) == DTE_ERR_ARG
+        assert fn(e._h, E._ptr(mis), E._ptr(hi), E._ptr(hv), n, E.DTE_SPARSE_ABSENT_MISSING, E._ptr(out), None) == E.DTE_ERR_ARG
         bad = hp.copy()
         bad[40] = bad[39] - 1
-        with pytest.raises(E.DteError) as ei:
-            e.infer_host_sparse((bad, hi, hv))
-        assert ei.value.code == DTE_ERR_ARG and "row 39" in str(ei.value)
-        with pytest.raises(E.DteError) as ei:
-            e.infer_host_sparse(rows, absent=2 ** 40)
-        assert ei.value.code == DTE_ERR_ARG
+        refused(lambda: e.infer_host_sparse((bad, hi, hv)), E.DTE_ERR_ARG, "row 39")
+        refused(lambda: e.infer_host_sparse(rows, absent=2 ** 40), E.DTE_ERR_ARG)
         after = e.info()
         assert after["kernel_launches"] == info["kernel_launches"] and after["tuples_in"] == info["tuples_in"]
         # a partial tuple pending in the line stream
@@ -332,9 +291,7 @@ def test_refusals_before_any_launch(torch_cuda):
         e.stream_write(wl)
         e.stream_write(fl)
         e.stream_write(x.reshape(-1, 4)[:5])                  # one tuple and a quarter
-        with pytest.raises(E.DteError) as ei:
-            e.infer_host_sparse(rows)
-        assert ei.value.code == DTE_ERR_STATE
+        refused(lambda: e.infer_host_sparse(rows), E.DTE_ERR_STATE)
 
 
 def test_dense_binned_and_leaf_calls_after_sparse(torch_cuda):

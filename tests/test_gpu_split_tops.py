@@ -6,27 +6,18 @@ import pytest
 
 import ddt_b200 as ddt
 from edge_operands import MISSING_ROTATION, edge_ensemble, edge_tuples, with_early_leaves
-from helpers import geometry_regs, oracle_cfg, L
+from helpers import make_engine, oracle_cfg, torch_cuda, L  # noqa: F401 (torch_cuda: a fixture)
 from oracle import oracle as O
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
 
 
 def run(monkeypatch, tune, W, FI, D, F, K, S, missing, x=None, n_of=None):
     """Scores, labels and kernel name of a handle created under DTE_TUNE=tune; x = n_of(tuples per CTA, SMs) tuples
     when x is None is built by the caller from the returned n."""
     monkeypatch.setenv("DTE_TUNE", tune)
-    e = ddt.Engine(0)
+    e = make_engine(W.shape[0], D, F, K, S, missing)
     try:
-        for a, v in sorted(geometry_regs(W.shape[0], D, F, K, S, missing).items()):
-            e.softreg_write(a, v)
         e.load_ensemble(*L.pack_streams(W, FI, D))
         info = e.info()
         if x is None:

@@ -8,11 +8,10 @@ import pytest
 
 import ddt_b200 as ddt
 from ddt_b200 import engine as E
-from helpers import geometry_regs, multi_node_regs, L
+from helpers import make_engine, multi_node_regs, refused_exactly, torch_cuda, write_regs, L  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-DTE_ERR_ARG, DTE_ERR_STATE, DTE_ERR_CONFIG, DTE_ERR_UNSUPPORTED = -1, -2, -3, -4
 T, D, F, K, n = 40, 5, 32, 2, 8
 
 # the suffix of each kind's calls: infer_host<sfx>, infer_device<sfx>, kernel_name<sfx>
@@ -48,13 +47,6 @@ SLOTS = ("reg 205: S=1 x K=2 x 8 slots hold fewer trees than the largest of the 
 
 
 @pytest.fixture(scope="module")
-def torch_cuda():
-    import torch
-    assert torch.cuda.is_available(), "these tests need the H100"
-    return torch
-
-
-@pytest.fixture(scope="module")
 def case():
     W, FI = L.synth_ensemble(T, D, F, seed=5101, cuts=16)     # binnable: 16 cuts per feature
     wl, fl = L.pack_streams(W, FI, D)
@@ -64,17 +56,9 @@ def case():
     return wl, fl, cov, bg, x
 
 
-def single(S=1):
-    e = ddt.Engine(0)
-    for a, v in sorted(geometry_regs(T, D, F, K, S, L.MISSING_DEFAULT).items()):
-        e.softreg_write(a, v)
-    return e
-
-
 def sharded():
     e = ddt.Engine([0, 0, 0])
-    for a, v in sorted(multi_node_regs(T, D, F, K, n, 3, "ensemble").items()):
-        e.softreg_write(a, v)
+    write_regs(e, multi_node_regs(T, D, F, K, n, 3, "ensemble"))
     return e
 
 
@@ -98,26 +82,19 @@ def name(e, sfx):
     return getattr(e, "kernel_name" + sfx)
 
 
-def refused(call, code, msg):
-    with pytest.raises(E.DteError) as ei:
-        call()
-    assert ei.value.code == code, str(ei.value)
-    assert str(ei.value) == "dte error %d: %s" % (code, msg)
-
-
 @pytest.mark.parametrize("sfx", KINDS, ids=lambda s: s[1:] or "fp32")
 def test_missing_layout_single(torch_cuda, case, sfx):
     """No ensemble: every infer call says so, the name call names the kind's layout; a plain load: every call of
     another kind names the layout it reads."""
     wl, fl, cov, bg, x = case
-    with single() as e:
-        refused(host(e, sfx, x), DTE_ERR_STATE, NO_ENSEMBLE)
-        refused(device(e, sfx), DTE_ERR_STATE, NO_ENSEMBLE)
-        refused(name(e, sfx), DTE_ERR_STATE, MISSING[sfx])
+    with make_engine(T, D, F, K, 1) as e:
+        refused_exactly(host(e, sfx, x), E.DTE_ERR_STATE, NO_ENSEMBLE)
+        refused_exactly(device(e, sfx), E.DTE_ERR_STATE, NO_ENSEMBLE)
+        refused_exactly(name(e, sfx), E.DTE_ERR_STATE, MISSING[sfx])
         if sfx:
             e.load_ensemble(wl, fl)
             for call in (host(e, sfx, x), device(e, sfx), name(e, sfx)):
-                refused(call, DTE_ERR_STATE, MISSING[sfx])
+                refused_exactly(call, E.DTE_ERR_STATE, MISSING[sfx])
 
 
 @pytest.mark.parametrize("sfx", KINDS, ids=lambda s: s[1:] or "fp32")
@@ -128,21 +105,21 @@ def test_missing_layout_and_attribution_sharded(torch_cuda, case, sfx):
     with sharded() as e:
         sharded_msg = SHARDED % (sfx, ATTRIBUTION[sfx]) if sfx in ATTRIBUTION else None
         if sharded_msg:
-            refused(host(e, sfx, x), DTE_ERR_CONFIG, sharded_msg)
+            refused_exactly(host(e, sfx, x), E.DTE_ERR_CONFIG, sharded_msg)
         else:
-            refused(host(e, sfx, x), DTE_ERR_STATE, NO_ENSEMBLE)
-        refused(name(e, sfx), DTE_ERR_STATE, MISSING[sfx])
+            refused_exactly(host(e, sfx, x), E.DTE_ERR_STATE, NO_ENSEMBLE)
+        refused_exactly(name(e, sfx), E.DTE_ERR_STATE, MISSING[sfx])
         if not sfx:
             return
         e.load_ensemble(wl, fl)
         if sharded_msg:
-            refused(host(e, sfx, x), DTE_ERR_CONFIG, sharded_msg)
+            refused_exactly(host(e, sfx, x), E.DTE_ERR_CONFIG, sharded_msg)
         else:
-            refused(host(e, sfx, x), DTE_ERR_STATE, MISSING[sfx])
-        refused(name(e, sfx), DTE_ERR_STATE, MISSING[sfx])
+            refused_exactly(host(e, sfx, x), E.DTE_ERR_STATE, MISSING[sfx])
+        refused_exactly(name(e, sfx), E.DTE_ERR_STATE, MISSING[sfx])
         if sharded_msg:
             load(e, sfx, wl, fl, cov, bg)
-            refused(host(e, sfx, x), DTE_ERR_CONFIG, sharded_msg)
+            refused_exactly(host(e, sfx, x), E.DTE_ERR_CONFIG, sharded_msg)
 
 
 @pytest.mark.parametrize("sfx", KINDS, ids=lambda s: s[1:] or "fp32")
@@ -153,17 +130,17 @@ def test_misaligned_device_pointers(torch_cuda, case, sfx):
     base = buf.data_ptr()
     bad_out = base + (8 if sfx == "_leaves" else 2)
     want_in, want_out = MISALIGNED[sfx]
-    with single() as e:
+    with make_engine(T, D, F, K, 1) as e:
         for loaded in (False, True):
             if loaded:
                 load(e, sfx, wl, fl, cov, bg)
-            refused(device(e, sfx, base + 4, base), DTE_ERR_ARG, want_in)
-            refused(device(e, sfx, base, bad_out), DTE_ERR_ARG, want_out)
+            refused_exactly(device(e, sfx, base + 4, base), E.DTE_ERR_ARG, want_in)
+            refused_exactly(device(e, sfx, base, bad_out), E.DTE_ERR_ARG, want_out)
             if not sfx:
-                refused(lambda: e.infer_device_accumulate(base + 4, 0, base), DTE_ERR_ARG,
-                        "dte_infer_device_accumulate: d_tuples not 16-byte aligned")
-                refused(lambda: e.infer_device_accumulate(base, 0, base + 2), DTE_ERR_ARG,
-                        "dte_infer_device_accumulate: d_scores_accum not 4-byte aligned")
+                refused_exactly(lambda: e.infer_device_accumulate(base + 4, 0, base), E.DTE_ERR_ARG,
+                                "dte_infer_device_accumulate: d_tuples not 16-byte aligned")
+                refused_exactly(lambda: e.infer_device_accumulate(base, 0, base + 2), E.DTE_ERR_ARG,
+                                "dte_infer_device_accumulate: d_scores_accum not 4-byte aligned")
 
 
 @pytest.mark.parametrize("sfx", KINDS, ids=lambda s: s[1:] or "fp32")
@@ -171,13 +148,13 @@ def test_multi_class_slots(torch_cuda, case, sfx):
     """S = 1, K = 2: 16 slots for 20 trees per class.  Every kind but the leaf walk, which walks every tree whatever K
     and S say, refuses the run."""
     wl, fl, cov, bg, x = case
-    with single(S=1) as e:
+    with make_engine(T, D, F, K, 1) as e:
         load(e, sfx, wl, fl, cov, bg, num_classes=2)
         if sfx == "_leaves":
             assert e.infer_host_leaves(x).shape == (n, T)
             return
-        refused(host(e, sfx, x), DTE_ERR_CONFIG, SLOTS)
-        refused(device(e, sfx), DTE_ERR_CONFIG, SLOTS)
+        refused_exactly(host(e, sfx, x), E.DTE_ERR_CONFIG, SLOTS)
+        refused_exactly(device(e, sfx), E.DTE_ERR_CONFIG, SLOTS)
 
 
 def test_interaction_row_cap(torch_cuda):
@@ -188,12 +165,10 @@ def test_interaction_row_cap(torch_cuda):
     wl, fl = L.pack_streams(W, FI, Dw)
     x = L.synth_tuples(0, 2, Fw, seed=5113)
     msg = "an interaction row of 4 classes x 2049 x 2049 words exceeds 64 MiB (2^24 words)"
-    with ddt.Engine(0) as e:
-        for a, v in sorted(geometry_regs(8, Dw, Fw, 8, 1, L.MISSING_DEFAULT).items()):
-            e.softreg_write(a, v)
+    with make_engine(8, Dw, Fw, 8, 1) as e:
         e.load_ensemble(wl, fl, num_classes=4, covers=cov)
-        refused(lambda: e.infer_host_interactions(x), DTE_ERR_UNSUPPORTED, msg)
-        refused(lambda: e.infer_device_interactions(None, 0, None), DTE_ERR_UNSUPPORTED, msg)
+        refused_exactly(lambda: e.infer_host_interactions(x), E.DTE_ERR_UNSUPPORTED, msg)
+        refused_exactly(lambda: e.infer_device_interactions(None, 0, None), E.DTE_ERR_UNSUPPORTED, msg)
 
 
 # Every row of the load table: the load, the kinds whose layouts it leaves resident (the leaf ids too when `leaves`), and
@@ -232,18 +207,18 @@ def test_resident_layouts_per_load(torch_cuda, case):
 
     rows = [
         ("plain", dict(), {""},
-         (lambda e: e.load_ensemble(wl_wide, fl_wide), DTE_ERR_UNSUPPORTED, "tree 0 node 0: feature index 32 >= 32 features")),
+         (lambda e: e.load_ensemble(wl_wide, fl_wide), E.DTE_ERR_UNSUPPORTED, "tree 0 node 0: feature index 32 >= 32 features")),
         ("classes", dict(num_classes=2), {""},
-         (lambda e: e.load_ensemble(wl, fl, num_classes=257), DTE_ERR_ARG, "num_classes = 257, need 1..256")),
+         (lambda e: e.load_ensemble(wl, fl, num_classes=257), E.DTE_ERR_ARG, "num_classes = 257, need 1..256")),
         ("binned", dict(binned=True), {"", "_binned"},
-         (lambda e: e.load_ensemble(wl_many, fl_many, binned=True), DTE_ERR_UNSUPPORTED,
+         (lambda e: e.load_ensemble(wl_many, fl_many, binned=True), E.DTE_ERR_UNSUPPORTED,
           "feature 0 has %d distinct thresholds: a binned layout holds at most 254 per feature" % n_edges)),
         ("contribs", dict(covers=cov), {"", "_contribs", "_interactions"},
-         (lambda e: e.load_ensemble(wl, fl, covers=cov_bad), DTE_ERR_ARG, bad_cover)),
+         (lambda e: e.load_ensemble(wl, fl, covers=cov_bad), E.DTE_ERR_ARG, bad_cover)),
         ("approx", dict(covers=cov, approx=True), {"", "_approx_contribs", "_leaves"},
-         (lambda e: e.load_ensemble(wl, fl, covers=cov_bad, approx=True), DTE_ERR_ARG, bad_cover)),
+         (lambda e: e.load_ensemble(wl, fl, covers=cov_bad, approx=True), E.DTE_ERR_ARG, bad_cover)),
         ("interventional", dict(background=bg), {"", "_interventional"},
-         (null_background, DTE_ERR_ARG, "dte_load_ensemble_interventional: background is NULL")),
+         (null_background, E.DTE_ERR_ARG, "dte_load_ensemble_interventional: background is NULL")),
     ]
 
     def check(e, answers, key):
@@ -251,14 +226,14 @@ def test_resident_layouts_per_load(torch_cuda, case):
             if sfx in answers:
                 assert isinstance(name(e, sfx)(), str), (key, sfx)
             else:
-                refused(name(e, sfx), DTE_ERR_STATE, MISSING[sfx])
+                refused_exactly(name(e, sfx), E.DTE_ERR_STATE, MISSING[sfx])
         assert e.info()["ensemble_bytes"] == BYTES[key], key
 
     for leaves in (False, True):
-        with single() as e:
+        with make_engine(T, D, F, K, 1) as e:
             answers, key = set(), ("none", leaves)
             for row, kw, builds, (bad_load, code, msg) in rows:
-                refused(lambda: bad_load(e), code, msg)
+                refused_exactly(lambda: bad_load(e), code, msg)
                 check(e, answers, key)
                 e.load_ensemble(wl, fl, leaves=leaves, **kw)
                 answers, key = builds | ({"_leaves"} if leaves else set()), (row, leaves)
